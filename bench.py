@@ -1,16 +1,17 @@
 #!/usr/bin/env python
-"""bench.py - throughput of the UNet training / sampling hot path on B200.
+"""bench.py - throughput of the UNet training / sampling hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            # this repo (libfdx kernels)
     python bench.py --impl reference --gpus N --steps K ...  # CPU reference arm (oracle on host cores)
+    python bench.py ... --dump-outputs DIR                   # also write the last step's outputs as .npy
 
 A "step" is one data-parallel training step of the EDM UNet (noise-add -> UNet fwd -> weighted
 L2 -> UNet bwd -> bucketed NCCL grad all-reduce overlapped with bwd -> AdamW + EMA) on a synthetic batch.
 The headline keys are BASELINE.json configs[1] (unconditional EDM UNet 64x64x3, bf16, batch 256 per GPU);
 the same default run covers the rest of the metric ("@64^2 & 256^2"): `sample` = Euler 50 steps at 64^2,
-`train_256` = configs[2] (EDM UNet 256^2 with self-attention, B = 64 per GPU = 512 over 8 GPUs),
+`train_256` = configs[2] (EDM UNet 256^2 with self-attention, B = 32 per GPU = 256 over 8 GPUs),
 `sample_256_heun` = configs[4] (Heun 18/50/100 steps, B = 32 per GPU, replicas), `sample_256_text_cfg` =
-configs[3] (text cross-attention, CFG Euler-ancestral 30 steps, B = 64).  Prints ONE JSON line.
+configs[3] (text cross-attention, CFG Euler-ancestral 30 steps, B = 32).  Prints ONE JSON line.
 """
 from __future__ import annotations
 
@@ -31,10 +32,12 @@ FWD_GFLOP = {  # algorithmic forward GFLOP per image (BASELINE.md $2)
 WORKLOADS = {
     # name: (resolution, per-GPU batch, attention configs, description)
     "c2": (64, 256, (None, None, None, None), "EDM UNet 64x64x3 bf16 B=256/GPU (BASELINE configs[1])"),
-    "c3": (256, 64, (None, None, None, {"heads": 8}), "EDM UNet 256x256x3 self-attn bf16 B=64/GPU (configs[2])"),
+    # c3: B = 32 per GPU - its saved-for-backward set plus the eager profiling step must fit the 80 GB of an H100
+    "c3": (256, 32, (None, None, None, {"heads": 8}), "EDM UNet 256x256x3 self-attn bf16 B=32/GPU (configs[2])"),
     # sampling-only workloads (python bench.py --workload c4|c5): value = denoise steps / s
-    "c4": (256, 64, (None, {"heads": 8}, {"heads": 8}, {"heads": 8}),
-           "text-cond UNet 256x256x3 (frozen random 77x768 text emb), CFG g=3, Euler-ancestral 30 steps, B=64 (configs[3])"),
+    # c4: B = 32 - CFG doubles the model batch, and 2 x 64 images at 256x256 do not fit the 80 GB of an H100
+    "c4": (256, 32, (None, {"heads": 8}, {"heads": 8}, {"heads": 8}),
+           "text-cond UNet 256x256x3 (frozen random 77x768 text emb), CFG g=3, Euler-ancestral 30 steps, B=32 (configs[3])"),
     "c5": (256, 32, (None, None, None, {"heads": 8}),
            "EDM UNet 256x256x3 self-attn, Heun 18/50/100 steps, B=32/GPU (configs[4])"),
 }
@@ -63,11 +66,13 @@ def usable_cores() -> int:
 
 
 def load_peaks():
+    """HBM GB/s, bf16 TFLOP/s, sustained bf16 TFLOP/s.  Without a measured file: NVIDIA's H100 SXM data sheet
+    (3.35 TB/s, 989 dense bf16 TFLOP/s at up to 700 W), never reached in practice."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet"
 
 
 _JSON_OUT = None
@@ -477,7 +482,7 @@ def run_train(D, args, workload, steps, warmup, with_cpu_baseline):
                                          "overlapped with backward" if trainer._overlap else
                                          "one fdx_comm_allreduce_avg (gradient + loss) after backward")
                        if trainer._exchange is not None else "none (single GPU)",
-                       "l2": "per-step activation traffic (>= 9 GB) exceeds the 126 MB L2; no explicit flush needed"},
+                       "l2": "per-step activation traffic (>= 9 GB) exceeds the 50 MB L2; no explicit flush needed"},
             "e2e": {"value": world * B / (ms_e2e / 1e3), "unit": "images/s", "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": B * E, "d2h_bytes_per_step": 4, "last_loss": last},
             "gpu_launches": launches_per_step * steps, "launches_per_step": launches_per_step,
@@ -525,6 +530,7 @@ def run_euler_c2(D, args, trainer, model, workload="c2"):
     s1.record()
     D.sync()
     (ms_s,) = D.max_ms(s0.elapsed_time(s1))
+    args.last_samples = imgs
     return {"sampler": "EulerSampler", "diffusion_steps": n_s, "batch_per_gpu": B,
             "denoise_steps_per_sec": n_s / (ms_s / 1e3), "image_steps_per_sec": world * B * n_s / (ms_s / 1e3),
             "ms_per_denoise_step": ms_s / n_s,
@@ -608,7 +614,10 @@ def main():
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--ref-batch", type=int, default=16)
     ap.add_argument("--ref-max-steps", type=int, default=3)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write what the headline path computed in its last step to DIR/*.npy")
     args = ap.parse_args()
+    args.last_samples = None
     import faulthandler
     faulthandler.enable()
     if os.environ.get("FDX_BENCH_WATCHDOG"):
@@ -647,14 +656,16 @@ def main():
     sample = None
     if not args.no_sample and first == "c2":
         sample = run_euler_c2(D, args, trainer, model)
+    if args.dump_outputs and D.rank == 0:
+        dump_outputs(args.dump_outputs, trainer, blk["e2e"]["last_loss"], args.last_samples)
     del trainer, model
     gc.collect()
     torch.cuda.empty_cache()
     extra = {}
     if args.workload == "all" and not args.no_256:
-        # the 256x256 half of the metric: C3 training (B = 64 per GPU: global 512 at --gpus 8 = BASELINE
+        # the 256x256 half of the metric: C3 training (B = 32 per GPU: global 256 at --gpus 8 = BASELINE
         # configs[2]), C5 Heun sweep and C4 CFG sampling as per-GPU replicas
-        steps256 = max(5, args.steps // 4)
+        steps256 = args.steps
         b3, tr3, m3 = run_train(D, args, "c3", steps256, 3, with_cpu_baseline=False)
         del tr3, m3
         gc.collect()
@@ -677,6 +688,29 @@ def main():
         out.update(extra)
         emit(out)
     D.close()
+
+
+DUMP_SAMPLE = 1 << 22     # elements kept per parameter vector (16 MB of f32); the dump stays below 64 MB
+
+
+def dump_outputs(out_dir, trainer, last_loss, samples):
+    """What a caller of the timed path receives after its last step: the loss, the updated parameters and EMA
+    parameters (a fixed, seeded sample of positions when larger than DUMP_SAMPLE) and the Euler samples.  Inputs
+    are seeded, so two builds run with the same arguments can be compared output for output."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "train_loss.npy"), np.array([last_loss], dtype=np.float64))
+    n = trainer.state.params.flat.numel()
+    idx = None
+    if n > DUMP_SAMPLE:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randperm(n, generator=g)[:DUMP_SAMPLE].sort().values
+    for name, fp in (("train_params", trainer.state.params), ("train_ema_params", trainer.state.ema_params)):
+        v = fp.flat.detach().float().cpu()
+        np.save(os.path.join(out_dir, f"{name}.npy"), (v if idx is None else v[idx]).numpy())
+    if samples is not None:
+        np.save(os.path.join(out_dir, "sample_images.npy"), samples.detach().float().cpu().numpy())
 
 
 def cpu_baseline(args, model, res, acfg):

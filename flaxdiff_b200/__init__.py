@@ -1,4 +1,4 @@
-"""flaxdiff_b200 - a B200-native (sm_100a) diffusion training / sampling engine with the
+"""flaxdiff_b200 - an H100-native (sm_90a) diffusion training / sampling engine with the
 flaxdiff.schedulers / predictors / samplers / trainer / models.simple_unet.Unet API surface.
 
 Host code is Python (PyTorch tensors as the container); all image- and activation-sized

@@ -7,14 +7,12 @@ import os
 ROUND2_DEFAULTS = {
     # name: (enabled, environment variable that selects the predecessor)
     "fused_attention": (True, "FDX_ATTN_UNFUSED"),     # fdx_attention_fwd/bwd vs separate QK^T / softmax / PV launches
-    "wgrad9k": (True, "FDX_WGRAD9_V1"),                # ky-pairs-in-M weight gradient vs the round-1 nine-tap kernels
-    # one-launch cluster GroupNorm backward vs the two-pass one: MEASURED SLOWER on B200 (profiles/layers_r02_gn_*.txt:
-    # 2.65 vs 1.81 ms over the C2 tensor set - fewer resident warps per SM cost more than the saved re-read), so off
+    # one-launch cluster GroupNorm backward vs the two-pass one: fewer resident warps per SM against one saved
+    # re-read of x and dy; off by default, kept tested (tests/test_optin_kernels_gpu.py)
     "gn_cluster_bwd": (False, "FDX_GN_2PASS"),
     # bucketed all-reduce launched from the backward pass inside the training graph vs ONE fdx_comm call after it:
-    # MEASURED on 8 B200s (profiles/bench_r02_*_n8.json): C2 23.34 vs 23.11 ms/step, C3 91.0 vs 89.9 - the NCCL
-    # CTAs take SMs from the persistent one-CTA-per-SM tensor-core kernels, which then need a second wave; the
-    # exposed all-reduce (128 MB over NVSwitch) is only ~0.5 ms.  Overlap stays available (FDX_NO_DP_OVERLAP=0).
+    # the NCCL CTAs take SMs from the persistent one-CTA-per-SM tensor-core kernels, which then need a second
+    # wave.  Overlap stays available (FDX_NO_DP_OVERLAP=0).
     "dp_overlap": (False, "FDX_NO_DP_OVERLAP"),
 }
 

@@ -1,4 +1,4 @@
-"""ctypes binding of libfdx.so (the sm_100a kernel library; C-ABI in include/fdx.h).
+"""ctypes binding of libfdx.so (the sm_90a kernel library; C-ABI in include/fdx.h).
 
 PyTorch is only the container: tensors provide device memory (`data_ptr`) and the
 current CUDA stream.  There is no CPU or eager fallback: if the shared library is

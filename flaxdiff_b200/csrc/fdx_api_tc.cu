@@ -1,4 +1,4 @@
-// fdx_api_tc.cu -- C-ABI entry points built on the tcgen05 tap-GEMM engine:
+// fdx_api_tc.cu -- C-ABI entry points built on the wgmma tap-GEMM engine:
 // conv3x3 (fwd / dgrad / wgrad, stride 1 and 2), conv1x1 / dense / batched GEMM.
 //
 // Reference interfaces replaced (all lowered by XLA in the reference):

@@ -1,4 +1,4 @@
-// fdx_attn.cu -- fused scaled-dot-product attention for sm_100a: nn.dot_product_attention as used by
+// fdx_attn.cu -- fused scaled-dot-product attention for sm_90a: nn.dot_product_attention as used by
 // NormalAttention (flaxdiff/models/attention.py:156-177, softmax(q k^T / sqrt(d)) v, self- and cross-attention
 // to the 77 x 768 text context) and its backward (jax.value_and_grad, trainer/general_diffusion_trainer.py:321).
 //
@@ -6,18 +6,17 @@
 // P round-tripping HBM ((B, h, L, Lk): 2.1 GB + 1 GB per block at 256x256).  Here S and P never leave the SM:
 //
 //   forward  (one CTA per 128 queries x head x image; flash-style loop over 128-key blocks)
-//     warp 0      TMA: Q tile once, K_j / V_j tiles through a 3-stage mbarrier ring (128B-swizzled boxes of
+//     warp 4      TMA: Q tile once, K_j / V_j tiles through an mbarrier ring (128B-swizzled boxes of
 //                 64 channels; a head narrower than 64 is addressed by a byte offset inside the swizzle row)
-//     warp 1      tcgen05.mma: S_j = Q K_j^T into a double-buffered TMEM accumulator (2 x 128 columns), then
-//                 O_j = P_j V_j into a second pair (2 x 64 columns) once the softmax warps have published P_j
-//     warps 2..5  softmax: one query row per thread, tcgen05.ld of its S row, running max / sum in the log2
-//                 domain, P_j written as bf16 straight into the K-major swizzled shared-memory tile that is the
-//                 A operand of the PV MMA (fence.proxy.async), O accumulated in registers with the usual
-//                 exp2(m_old - m_new) correction, final O / l and the log-sum-exp row for the backward.
+//     warps 0..3  one warpgroup: wgmma S_j = Q K_j^T into registers, then softmax with one query row per
+//                 thread (WgAcc::row32), running max / sum in the log2 domain, P_j written as bf16 straight
+//                 into the K-major swizzled shared-memory tile that is the A operand of the wgmma
+//                 O_j = P_j V_j (fence.proxy.async), O accumulated per row with the usual exp2(m_old - m_new)
+//                 correction, final O / l and the log-sum-exp row for the backward.
 //   backward = two kernels with the same skeleton, S and dP recomputed on chip (FlashAttention-2 recipe,
 //     7 small GEMMs instead of 5, no atomics, deterministic):
 //       fdx_attn_bwd_dq   per 128-query tile, loop over key blocks:  dS = P o (dP - D) ;  dQ += dS K
-//       fdx_attn_bwd_dkv  per 128-key block, loop over query tiles (transposed tiles, TMEM lane = key):
+//       fdx_attn_bwd_dkv  per 128-key block, loop over query tiles (transposed tiles, tile row = key):
 //                         dV += P^T dO ;  dK += dS^T Q
 //     with P = exp2(s * scale*log2e - lse*log2e), D = rowsum(dO o O), dS including the 1/sqrt(d) factor.
 // Tensors are bf16 [B][L][heads * dh] (row stride and batch stride given), dh in {32, 64}; keys beyond Lk and
@@ -30,7 +29,7 @@
 
 namespace {
 
-constexpr int kThreads = 192;
+constexpr int kThreads = 160;           // forward: one consumer warpgroup + the producer warp
 constexpr int kTile = 128 * 128;          // bytes of one [128 rows][64 ch] bf16 swizzled tile
 constexpr int kKV = 3;                    // K/V ring stages (forward, dQ kernel)
 constexpr float kLog2e = 1.4426950408889634f;
@@ -75,49 +74,24 @@ __device__ __forceinline__ void store_p_chunk(uint32_t sP, int r, int c0, const 
 // ======================================================================================================
 // forward
 // ======================================================================================================
-// SHORT = the keys fit one 128-key block (77 text tokens): no ring, one P tile, 256 TMEM columns and 80 KB of
-// shared memory, so TWO CTAs share an SM - with L/128 x heads x B short-lived CTAs (131 072 at 128x128, B = 128)
-// the prologue (barrier init, TMEM allocation, first TMA round trip) of one overlaps the math of the other.
-// DUAL (long key sequences) = the same economy for the flash loop: S, P and O single-buffered (256 TMEM columns),
-// a two-stage K/V ring, 112 KB of shared memory - again two CTAs per SM.  Inside one CTA the chain
-// S_j -> softmax_j -> PV_j is then serial (the next S is issued as soon as the softmax warps have consumed the
-// current one), and the overlap the double buffers gave comes from the OTHER resident CTA instead - which also
-// doubles the softmax warps per scheduler, the actual limiter of the one-CTA arrangement (one warp per
-// scheduler cannot hide its tcgen05.ld / MUFU latencies) and hides the per-CTA prologue and epilogue.
-template <int DH, bool SHORT, bool DUAL>
-__global__ void __launch_bounds__(kThreads, (SHORT || DUAL) ? 2 : 1)
+// SHORT = the keys fit one 128-key block (77 text tokens): a single K/V stage.  Otherwise a ring of NKV stages
+// keeps the next key blocks in flight while the warpgroup works through the serial chain
+// S_j -> softmax_j -> PV_j.
+template <int DH, bool SHORT>
+__global__ void __launch_bounds__(kThreads, 1)
 fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                     const __grid_constant__ CUtensorMap mapV, const AttnDev p) {
-  static_assert(!(SHORT && DUAL), "SHORT has no loop to single-buffer");
-  extern __shared__ __align__(1024) uint8_t smem_fwd_raw[];
-  uint8_t* const smem_raw = smem_fwd_raw;
-  uint8_t* smem;
-  if constexpr (DUAL) {
-    // no alignment slack in the request (2 x 113 KB + the per-CTA reserve must fit the SM): the dynamic window
-    // has to start 1024-byte aligned by itself - fail loudly if it ever does not
-    smem = smem_raw;
-    if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
-  } else {
-    smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  }
-  constexpr bool ONE = SHORT || DUAL;                // single S / P / O buffers
-  constexpr int NKV = SHORT ? 1 : (DUAL ? 2 : kKV);  // K/V ring stages
-  constexpr int NPB = ONE ? 1 : 2;                   // P tiles
-  constexpr uint32_t O_COL = ONE ? 128u : 256u;      // first TMEM column of the O accumulator(s)
-  constexpr uint32_t TMEM_COLS = ONE ? 256u : 512u;
-  auto sb = [](int j) { return ONE ? 0 : (j & 1); };                 // S / P / O buffer of block j
-  auto sph = [](int j) { return ONE ? (j & 1) : ((j >> 1) & 1); };   // ... and the parity of its barrier phase
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  constexpr int NKV = SHORT ? 1 : kKV;               // K/V ring stages
   uint8_t* sQ = smem;
   uint8_t* sKV = smem + kTile;                       // NKV x (K tile, V tile)
-  uint8_t* sP = sKV + NKV * 2 * kTile;               // NPB x (two 64-key chunks)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + NPB * 2 * kTile);
+  uint8_t* sP = sKV + NKV * 2 * kTile;               // two 64-key chunks
+  float* xs = reinterpret_cast<float*>(sP + 2 * kTile);   // accumulator exchange tile
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(xs) + kAccXchgBytes);
   uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;          // [kKV]
-  uint64_t* kv_empty = bars + 1 + kKV;   // [kKV]
-  uint64_t* s_full = bars + 1 + 2 * kKV; // [2]
-  uint64_t* p_full = s_full + 2;         // [2]
-  uint64_t* o_full = p_full + 2;         // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
+  uint64_t* kv_full = bars + 1;          // [NKV]
+  uint64_t* kv_empty = bars + 1 + kKV;   // [NKV]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
@@ -126,20 +100,15 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
   const int c0 = (head * DH) / 64 * 64;                     // first channel of the 64-wide TMA box
   const uint32_t koff = (uint32_t)((head * DH) % 64) * 2;   // byte offset of this head inside the swizzle row
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&mapQ); tma_prefetch_desc(&mapK); tma_prefetch_desc(&mapV);
     mbar_init(q_full, 1);
-    for (int i = 0; i < kKV; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&p_full[i], 4); mbar_init(&o_full[i], 1); }
+    for (int i = 0; i < NKV; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, TMEM_COLS); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       mbar_arrive_expect_tx(q_full, kTile);
       tma_load_4d(sQ, &mapQ, q_full, c0, q0, b, 0);
@@ -151,112 +120,68 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
         tma_load_4d(sKV + s * 2 * kTile + kTile, &mapV, &kv_full[s], c0, j * 128, b, 0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idS = umma_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idO = umma_idesc_bf16(128, DH, 0, 1);
-      const uint32_t aQ = smem_u32(sQ) + koff;
-      auto issue_s = [&](int j) {
-        const int s = j % NKV;
-        mbar_wait(&kv_full[s], (j / NKV) & 1);
-        tc_fence_after();
-        const uint32_t aK = smem_u32(sKV + s * 2 * kTile) + koff;
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k)
-          umma_f16(tmem_base + (uint32_t)(sb(j) * 128), umma_desc_sw128(aQ + k * 32, 16, 1024),
-                   umma_desc_sw128(aK + k * 32, 16, 1024), idS, k != 0 ? 1u : 0u);
-        umma_commit(&s_full[sb(j)]);
-      };
-      mbar_wait(q_full, 0);
-      tc_fence_after();
-      issue_s(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (!ONE && j + 1 < nblk) issue_s(j + 1);
-        mbar_wait(&p_full[sb(j)], sph(j));
-        tc_fence_after();
-        // single S buffer: the softmax warps have consumed S_j (they publish P_j after their last tcgen05.ld)
-        if (ONE && j + 1 < nblk) issue_s(j + 1);
-        const int s = j % NKV;
-        const uint32_t aP = smem_u32(sP + (j % NPB) * 2 * kTile);
-        const uint32_t aV = smem_u32(sKV + s * 2 * kTile + kTile) + koff;
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_f16(tmem_base + O_COL + (uint32_t)(sb(j) * 64),
-                   umma_desc_sw128(aP + (k >> 2) * kTile + (k & 3) * 32, 16, 1024),
-                   umma_desc_sw128(aV + k * 2048, 8192, 1024), idO, k != 0 ? 1u : 0u);
-        umma_commit(&o_full[sb(j)]);
-        umma_commit(&kv_empty[s]);
-      }
-    }
   } else {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    float m = -INFINITY, l = 0.f, corr_prev = 0.f;
+    const int row = warp * 32 + lane;
+    const uint32_t aQ = smem_u32(sQ) + koff;
+    const uint32_t sPa = smem_u32(sP);
+    float m = -INFINITY, l = 0.f;
     float acc[DH];
 #pragma unroll
     for (int i = 0; i < DH; ++i) acc[i] = 0.f;
-
-    auto fold_o = [&](int j, float corr) {      // acc = acc * corr + O_j
-      mbar_wait(&o_full[sb(j)], sph(j));
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < DH; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(lane_addr + O_COL + (uint32_t)(sb(j) * 64 + c), v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[c + i] = fmaf(acc[c + i], corr, __uint_as_float(v[i]));
-      }
-    };
+    mbar_wait(q_full, 0);
 
     for (int j = 0; j < nblk; ++j) {
-      mbar_wait(&s_full[sb(j)], sph(j));
-      tc_fence_after();
-      const uint32_t sa = lane_addr + (uint32_t)(sb(j) * 128);
+      const int s = j % NKV;
+      mbar_wait(&kv_full[s], (j / NKV) & 1);
+      const uint32_t aK = smem_u32(sKV + s * 2 * kTile) + koff;
+      const uint32_t aV = aK + kTile;
+      WgAcc<128> S;
+      S.zero();
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < DH / 16; ++k)
+        S.mma<0, 0>(gmma_desc_sw128(aQ + k * 32, 16, 1024), gmma_desc_sw128(aQ + 8192 + k * 32, 16, 1024),
+                    gmma_desc_sw128(aK + k * 32, 16, 1024));
+      wgmma_commit();
+      wgmma_wait<0>();
       const int kbase = j * 128;
       // pass A: row maximum over the valid keys (only the last key block can be partial)
       const bool partial = kbase + 128 > p.Lk;
       float mx = -INFINITY;
 #pragma unroll 1
       for (int c = 0; c < 128; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(sa + c, v);
-        tmem_ld_wait();
+        float v[32];
+        S.row32(xs, 1, c, v);
         if (partial) {
 #pragma unroll
           for (int i = 0; i < 32; ++i)
-            if (kbase + c + i < p.Lk) mx = fmaxf(mx, __uint_as_float(v[i]));
+            if (kbase + c + i < p.Lk) mx = fmaxf(mx, v[i]);
         } else {
           float m4[4] = {mx, -INFINITY, -INFINITY, -INFINITY};        // four independent chains
 #pragma unroll
           for (int i = 0; i < 32; i += 4) {
 #pragma unroll
-            for (int u = 0; u < 4; ++u) m4[u] = fmaxf(m4[u], __uint_as_float(v[i + u]));
+            for (int u = 0; u < 4; ++u) m4[u] = fmaxf(m4[u], v[i + u]);
           }
           mx = fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
         }
       }
       const float m_new = fmaxf(m, mx * p.scale_log2);
       const float corr = ex2(m - m_new);           // first block: exp2(-inf) = 0
-      // single P / O buffers: PV_{j-1} must have retired before P_j overwrites its operand, and O_{j-1} must be
-      // read before PV_j overwrites it - fold it in here, between the two passes
-      if (ONE && j > 0) fold_o(j - 1, corr_prev);
       // pass B: probabilities -> bf16 -> the swizzled A tile of the PV MMA
       float rs = 0.f;
-      const uint32_t sPj = smem_u32(sP + (j % NPB) * 2 * kTile);
 #pragma unroll 1
       for (int c = 0; c < 128; c += 32) {
-        uint32_t v[32], w[16];
-        tmem_ld_32x32(sa + c, v);
-        tmem_ld_wait();
+        float v[32];
+        uint32_t w[16];
+        S.row32(xs, 1, c, v);
         float rs4[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {
           float pe[4];
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
-            pe[u] = ex2(fmaf(__uint_as_float(v[i + u]), p.scale_log2, -m_new));
+            pe[u] = ex2(fmaf(v[i + u], p.scale_log2, -m_new));
             if (partial && !(kbase + c + i + u < p.Lk)) pe[u] = 0.f;
             rs4[u] += pe[u];
           }
@@ -264,18 +189,32 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
           w[(i >> 1) + 1] = pack_bf16x2(pe[2], pe[3]);
         }
         rs += (rs4[0] + rs4[1]) + (rs4[2] + rs4[3]);
-        store_p_chunk(sPj, row, c, w);
+        store_p_chunk(sPa, row, c, w);
       }
       l = fmaf(l, corr, rs);
       m = m_new;
-      tc_fence_before();
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[sb(j)]);
-      if (!ONE && j > 0) fold_o(j - 1, corr_prev);
-      corr_prev = corr;
+      named_bar_sync(1, 128);                      // every row of P_j is in shared memory
+      WgAcc<DH> O;
+      O.zero();
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const uint32_t ap = sPa + (k >> 2) * kTile + (k & 3) * 32;
+        O.mma<0, 1>(gmma_desc_sw128(ap, 16, 1024), gmma_desc_sw128(ap + 8192, 16, 1024),
+                    gmma_desc_sw128(aV + k * 2048, 8192, 1024));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (threadIdx.x == 0) mbar_arrive(&kv_empty[s]);
+#pragma unroll
+      for (int c = 0; c < DH; c += 32) {           // acc = acc * corr + O_j
+        float v[32];
+        O.row32(xs, 1, c, v);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[c + i] = fmaf(acc[c + i], corr, v[i]);
+      }
     }
-    fold_o(nblk - 1, corr_prev);
     if (q0 + row < p.L) {
       const float inv = 1.f / l;
       __nv_bfloat16* op = p.o + (long long)b * p.o_bs + (long long)(q0 + row) * p.o_ld + head * DH;
@@ -291,9 +230,6 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
       if (p.lse) p.lse[((long long)b * p.heads + head) * p.L + q0 + row] = m * kLn2 + logf(l);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, TMEM_COLS); }
 }
 
 // ======================================================================================================
@@ -324,22 +260,20 @@ __global__ void attn_dvec_kernel(const AttnDev p) {
 
 // ======================================================================================================
 // backward, shared skeleton.  ROWS_ARE_KEYS = false: the dQ kernel (tile rows = queries, loop over key blocks);
-// true: the dK / dV kernel (tile rows = keys, loop over query tiles).  Per loop step two 128 x 128 products land
-// in TMEM (cols 0..127: S or S^T; 128..255: dP or dP^T), the four softmax warps turn them into the bf16 tiles
-// E1 = P (only needed for dV) and E2 = dS in shared memory, and the MMA warp accumulates
-//   dQ  += dS  . K_j                (cols 256..319)                        [ROWS_ARE_KEYS = false]
-//   dV  += P^T . dO_i  (256..319),  dK += dS^T . Q_i  (320..383)           [ROWS_ARE_KEYS = true]
-// across the whole loop (no rescaling: P is recomputed from the saved log-sum-exp).
-// Shared memory: R1, R2 = the two row-side operands (Q, dO | K, V), ring of (C1, C2) = the column-side pair
-// (K_j, V_j | Q_i, dO_i), E1 / E2 tiles of 2 x 16 KB each.
+// true: the dK / dV kernel (tile rows = keys, loop over query tiles).  Per loop step two 128 x 128 products are
+// computed by two warpgroups, each owning 64 of the columns: S (or S^T) and dP (or dP^T) in registers.  Each
+// warpgroup turns its columns into the bf16 tiles E1 = P (only needed for dV) and E2 = dS in shared memory, and
+// once both halves are published the accumulating products run on the whole tiles:
+//   dQ  += dS  . K_j                (warpgroup 0)                          [ROWS_ARE_KEYS = false]
+//   dV  += P^T . dO_i  (warpgroup 0),  dK += dS^T . Q_i  (warpgroup 1)     [ROWS_ARE_KEYS = true]
+// with the accumulators in registers across the whole loop (no rescaling: P is recomputed from the saved
+// log-sum-exp).  Shared memory: R1, R2 = the two row-side operands (Q, dO | K, V), ring of (C1, C2) = the
+// column-side pair (K_j, V_j | Q_i, dO_i), E1 / E2 tiles of 2 x 16 KB each.
 // ======================================================================================================
-// EWG = number of 4-warp groups that turn S / dP into the E tiles.  The element-wise step (two tcgen05.ld, exp2,
-// two bf16 packs and swizzled stores per element) is what bounds the kernel - 128 columns per thread with one
-// warp per scheduler cannot hide its own latencies - and it has no cross-column dependency (the softmax
-// statistics are inputs), so with EWG = 2 the warps (2..5) take columns 0..63 of every row and (6..9) columns
-// 64..127: two warps per scheduler on the same TMEM lanes.
-template <int DH, bool ROWS_ARE_KEYS, int EWG>
-__global__ void __launch_bounds__(64 + 128 * EWG, 1)
+constexpr int kBwdThreads = 3 * 128;   // two consumer warpgroups + the producer warpgroup (one thread issues TMA)
+
+template <int DH, bool ROWS_ARE_KEYS>
+__global__ void __launch_bounds__(kBwdThreads, 1)
 fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_constant__ CUtensorMap mapR2,
                     const __grid_constant__ CUtensorMap mapC1, const __grid_constant__ CUtensorMap mapC2,
                     const AttnDev p) {
@@ -353,15 +287,11 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
   uint8_t* sE1 = sC + RING * 2 * kTile;                // 2 chunks
   uint8_t* sE2 = sE1 + 2 * kTile;                      // 2 chunks
   float* sStat = reinterpret_cast<float*>(sE2 + 2 * kTile);     // RING x (lse[128], dvec[128]) of the column side
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + RING * 256);
+  float* sX = sStat + RING * 256;                      // 2 x accumulator exchange tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sX) + 2 * kAccXchgBytes);
   uint64_t* r_full = bars;
   uint64_t* c_full = bars + 1;            // [RING]
   uint64_t* c_empty = c_full + RING;      // [RING]
-  uint64_t* s_full = c_empty + RING;      // S and dP of this step are in TMEM
-  uint64_t* e_full = s_full + 1;          // E tiles published (count 4)
-  uint64_t* e_free = e_full + 1;          // accumulating MMAs that read the E tiles retired
-  uint64_t* done = e_free + 1;            // all accumulation finished
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
@@ -372,24 +302,17 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
   const int c0 = (head * DH) / 64 * 64;
   const uint32_t koff = (uint32_t)((head * DH) % 64) * 2;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&mapR1); tma_prefetch_desc(&mapR2); tma_prefetch_desc(&mapC1); tma_prefetch_desc(&mapC2);
     mbar_init(r_full, 1);
-    for (int i = 0; i < RING; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 1); }
-    mbar_init(s_full, 1);
-    mbar_init(e_full, 4 * EWG);
-    mbar_init(e_free, 1);
-    mbar_init(done, 1);
+    for (int i = 0; i < RING; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (warp >= 8) producer_regs(); else consumer_regs();
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    if (warp == 8 && lane == 0) {
       mbar_arrive_expect_tx(r_full, 2 * kTile);
       tma_load_4d(sR1, &mapR1, r_full, c0, r0, b, 0);
       tma_load_4d(sR2, &mapR2, r_full, c0, r0, b, 0);
@@ -401,58 +324,13 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
         tma_load_4d(sC + s * 2 * kTile + kTile, &mapC2, &c_full[s], c0, j * 128, b, 0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idS = umma_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idA = umma_idesc_bf16(128, DH, 0, 1);
-      const uint32_t aR1 = smem_u32(sR1) + koff, aR2 = smem_u32(sR2) + koff;
-      mbar_wait(r_full, 0);
-      tc_fence_after();
-      for (int j = 0; j < nstep; ++j) {
-        const int s = j % RING;
-        mbar_wait(&c_full[s], (j / RING) & 1);
-        tc_fence_after();
-        const uint32_t aC1 = smem_u32(sC + s * 2 * kTile) + koff, aC2 = aC1 + kTile;
-        // the softmax warps must have finished reading the previous step's S / dP: implied by e_full(j-1),
-        // which this thread waited for before issuing the previous accumulation
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k) {
-          // S (or S^T) = R1 . C1^T ;  dP (or dP^T) = R2 . C2^T
-          umma_f16(tmem_base, umma_desc_sw128(aR1 + k * 32, 16, 1024), umma_desc_sw128(aC1 + k * 32, 16, 1024),
-                   idS, k != 0 ? 1u : 0u);
-          umma_f16(tmem_base + 128u, umma_desc_sw128(aR2 + k * 32, 16, 1024),
-                   umma_desc_sw128(aC2 + k * 32, 16, 1024), idS, k != 0 ? 1u : 0u);
-        }
-        umma_commit(s_full);
-        mbar_wait(e_full, j & 1);
-        tc_fence_after();
-        const uint32_t aE1 = smem_u32(sE1), aE2 = smem_u32(sE2);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint32_t eo = (uint32_t)((k >> 2) * kTile + (k & 3) * 32);
-          if constexpr (ROWS_ARE_KEYS) {
-            // dV += P^T . dO_i  (B = C2 = dO_i, MN-major) ;  dK += dS^T . Q_i  (B = C1 = Q_i)
-            umma_f16(tmem_base + 256u, umma_desc_sw128(aE1 + eo, 16, 1024),
-                     umma_desc_sw128(aC2 + k * 2048, 8192, 1024), idA, (j | k) != 0 ? 1u : 0u);
-            umma_f16(tmem_base + 320u, umma_desc_sw128(aE2 + eo, 16, 1024),
-                     umma_desc_sw128(aC1 + k * 2048, 8192, 1024), idA, (j | k) != 0 ? 1u : 0u);
-          } else {
-            // dQ += dS . K_j  (B = C1 = K_j, MN-major)
-            umma_f16(tmem_base + 256u, umma_desc_sw128(aE2 + eo, 16, 1024),
-                     umma_desc_sw128(aC1 + k * 2048, 8192, 1024), idA, (j | k) != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(e_free);
-        umma_commit(&c_empty[s]);
-      }
-      umma_commit(done);
-    }
   } else {
-    const int q = warp & 3;
-    const int wg = (warp - 2) >> 2;                    // element-wise warp group: columns [wg * 128 / EWG, ...)
-    constexpr int CW = 128 / EWG;                      // columns per thread and step
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
+    const int wg = warp >> 2;                          // columns [64 wg, 64 wg + 64) of S / dP
+    constexpr int CW = 64;
+    const int row = (warp & 3) * 32 + lane;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    float* xs = sX + wg * (kAccXchgBytes / 4);
+    const int xbar = 2 + wg;
     const long long stat_base = ((long long)b * p.heads + head) * p.L;
     // dQ kernel: this thread's query row statistics; dK/dV kernel: they belong to the COLUMNS (queries)
     float lse_r = 0.f, d_r = 0.f;
@@ -462,8 +340,13 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
         d_r = p.dvec[stat_base + r0 + row] * p.scale;
       }
     }
+    const uint32_t aR1 = smem_u32(sR1) + koff, aR2 = smem_u32(sR2) + koff;
     const uint32_t sE1a = smem_u32(sE1), sE2a = smem_u32(sE2);
+    WgAcc<DH> A;                                       // dQ | dV (warpgroup 0) or dK (warpgroup 1)
+    A.zero();
+    mbar_wait(r_full, 0);
     for (int j = 0; j < nstep; ++j) {
+      const int s = j % RING;
       const int cbase = j * 128;
       if constexpr (ROWS_ARE_KEYS) {
         // stage the query-side statistics of this step (parity buffer j & 1), 128 threads = 128 columns
@@ -473,11 +356,25 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
           st[row] = ok ? p.lse[stat_base + cbase + row] * kLog2e : 0.f;
           st[128 + row] = ok ? p.dvec[stat_base + cbase + row] * p.scale : 0.f;
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(128 * EWG) : "memory");
       }
-      if (j > 0) mbar_wait(e_free, (j - 1) & 1);      // previous step's accumulation has consumed E1 / E2
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
+      mbar_wait(&c_full[s], (j / RING) & 1);
+      const uint32_t aC1 = smem_u32(sC + s * 2 * kTile) + koff, aC2 = aC1 + kTile;
+      // S (or S^T) = R1 . C1^T ;  dP (or dP^T) = R2 . C2^T  - this warpgroup's 64 columns
+      WgAcc<64> Sa, Pa;
+      Sa.zero();
+      Pa.zero();
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < DH / 16; ++k) {
+        Sa.mma<0, 0>(gmma_desc_sw128(aR1 + k * 32, 16, 1024), gmma_desc_sw128(aR1 + 8192 + k * 32, 16, 1024),
+                     gmma_desc_sw128(aC1 + wg * 8192 + k * 32, 16, 1024));
+        Pa.mma<0, 0>(gmma_desc_sw128(aR2 + k * 32, 16, 1024), gmma_desc_sw128(aR2 + 8192 + k * 32, 16, 1024),
+                     gmma_desc_sw128(aC2 + wg * 8192 + k * 32, 16, 1024));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // the statistics are staged and the previous step's accumulation has consumed E1 / E2
+      named_bar_sync(1, 256);
       const float* st = sStat + (j & 1) * 256;
       const bool row_in = ROWS_ARE_KEYS ? (r0 + row < p.Lk) : (r0 + row < p.L);
       const int col_lim = (ROWS_ARE_KEYS ? p.L : p.Lk) - cbase;      // columns of this step inside the tensor
@@ -486,11 +383,12 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
       auto ewise = [&](auto mask_tag) {
         constexpr bool MASK = decltype(mask_tag)::value;
 #pragma unroll 1
-        for (int c = wg * CW; c < (wg + 1) * CW; c += 32) {
-          uint32_t vs[32], vp[32], w1[16], w2[16];
-          tmem_ld_32x32(lane_addr + (uint32_t)c, vs);
-          tmem_ld_32x32(lane_addr + 128u + (uint32_t)c, vp);
-          tmem_ld_wait();
+        for (int cl = 0; cl < CW; cl += 32) {
+          const int c = wg * CW + cl;
+          float vs[32], vp[32];
+          uint32_t w1[16], w2[16];
+          Sa.row32(xs, xbar, cl, vs);
+          Pa.row32(xs, xbar, cl, vp);
 #pragma unroll
           for (int i = 0; i < 32; i += 4) {
             float lq[4] = {lse_r, lse_r, lse_r, lse_r}, dq4[4] = {d_r, d_r, d_r, d_r};
@@ -503,10 +401,10 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
             float pr[4], ds[4];
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
-              float pv = ex2(fmaf(__uint_as_float(vs[i + u]), p.scale_log2, -lq[u]));
+              float pv = ex2(fmaf(vs[i + u], p.scale_log2, -lq[u]));
               if (MASK && !(row_in && (c + i + u < col_lim))) pv = 0.f;
               pr[u] = pv;
-              ds[u] = pv * fmaf(__uint_as_float(vp[i + u]), p.scale, -dq4[u]);
+              ds[u] = pv * fmaf(vp[i + u], p.scale, -dq4[u]);
             }
             w1[i >> 1] = pack_bf16x2(pr[0], pr[1]);
             w1[(i >> 1) + 1] = pack_bf16x2(pr[2], pr[3]);
@@ -517,52 +415,55 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
           store_p_chunk(sE2a, row, c, w2);
         }
       };
-      // warp-uniform choice (the TMEM loads inside are warp-collective)
-      const bool need_mask = __any_sync(0xffffffffu, !row_in) || col_lim < 128;
+      // warpgroup-uniform choice (row32 synchronises the warpgroup)
+      const bool need_mask = r0 + 128 > nrows || col_lim < 128;
       if (need_mask) ewise(std::true_type{}); else ewise(std::false_type{});
-      tc_fence_before();
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(e_full);
-    }
-    // epilogue: accumulators -> bf16 rows.  tcgen05.ld is warp-collective (.sync.aligned): EVERY lane executes
-    // it, only the global stores are predicated on the row being inside the tensor.
-    mbar_wait(done, 0);
-    tc_fence_after();
-    const bool row_ok = r0 + row < nrows;
-    constexpr int NOUT = ROWS_ARE_KEYS ? 2 : 1;
+      named_bar_sync(1, 256);                          // both halves of E1 / E2 are published
+      if (ROWS_ARE_KEYS || wg == 0) {
+        // dV += P^T . dO_i (B = C2, MN-major) | dK += dS^T . Q_i (B = C1) | dQ += dS . K_j (B = C1)
+        const uint32_t aE = (ROWS_ARE_KEYS && wg == 0) ? sE1a : sE2a;
+        const uint32_t aB = (ROWS_ARE_KEYS && wg == 0) ? aC2 : aC1;
+        wgmma_fence();
 #pragma unroll
-    for (int which = 0; which < NOUT; ++which) {
+        for (int k = 0; k < 8; ++k) {
+          const uint32_t eo = aE + (uint32_t)((k >> 2) * kTile + (k & 3) * 32);
+          A.mma<0, 1>(gmma_desc_sw128(eo, 16, 1024), gmma_desc_sw128(eo + 8192, 16, 1024),
+                      gmma_desc_sw128(aB + k * 2048, 8192, 1024));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+      }
+      if (wg_leader) mbar_arrive(&c_empty[s]);
+    }
+    // epilogue: accumulator rows -> bf16
+    if (ROWS_ARE_KEYS || wg == 0) {
+      const bool row_ok = r0 + row < nrows;
       __nv_bfloat16* base;
       if constexpr (ROWS_ARE_KEYS)
-        base = which == 0 ? p.dv + (long long)b * p.dv_bs + (long long)(r0 + row) * p.dv_ld
-                          : p.dk + (long long)b * p.dk_bs + (long long)(r0 + row) * p.dk_ld;
+        base = wg == 0 ? p.dv + (long long)b * p.dv_bs + (long long)(r0 + row) * p.dv_ld
+                       : p.dk + (long long)b * p.dk_bs + (long long)(r0 + row) * p.dk_ld;
       else
         base = p.dq + (long long)b * p.dq_bs + (long long)(r0 + row) * p.dq_ld;
       base += head * DH;
 #pragma unroll
       for (int c = 0; c < DH; c += 32) {
-        if (EWG == 2 && ((which * (DH / 32) + c / 32) & 1) != wg) continue;   // the 32-column pieces alternate
-        uint32_t v[32];
-        tmem_ld_32x32(lane_addr + 256u + (uint32_t)(which * 64 + c), v);
-        tmem_ld_wait();
+        float v[32];
+        A.row32(xs, xbar, c, v);
         if (row_ok) {
 #pragma unroll
           for (int i = 0; i < 32; i += 8) {
             uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(v[i]), __uint_as_float(v[i + 1]));
-            u.y = pack_bf16x2(__uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-            u.z = pack_bf16x2(__uint_as_float(v[i + 4]), __uint_as_float(v[i + 5]));
-            u.w = pack_bf16x2(__uint_as_float(v[i + 6]), __uint_as_float(v[i + 7]));
+            u.x = pack_bf16x2(v[i], v[i + 1]);
+            u.y = pack_bf16x2(v[i + 2], v[i + 3]);
+            u.z = pack_bf16x2(v[i + 4], v[i + 5]);
+            u.w = pack_bf16x2(v[i + 6], v[i + 7]);
             *reinterpret_cast<uint4*>(base + c + i) = u;
           }
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 int make_map(CUtensorMap* m, const void* ptr, int hd, int rows, int B, long long ld, long long bs) {
@@ -602,29 +503,24 @@ int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
   d.o = (__nv_bfloat16*)a->o; d.o_ld = a->o_ld; d.o_bs = a->o_bs;
   d.lse = a->lse;
   const bool short_keys = a->Lk <= 128 && !getenv("FDX_ATTN_NO_SHORT");
-  const bool dual = !short_keys && !getenv("FDX_ATTN_NO_DUAL");      // two CTAs per SM for the flash loop
-  const int smem = short_keys ? (1 + 2 + 2) * kTile + 1024 + 256
-                   : dual     ? (1 + 2 * 2 + 2) * kTile + 256
-                              : (1 + 2 * kKV + 4) * kTile + 1024 + 256;
+  const int smem = (1 + 2 * (short_keys ? 1 : kKV) + 2) * kTile + kAccXchgBytes + 1024 + 256;
   dim3 grid((a->L + 127) / 128, a->heads, a->B);
-  static bool attr[6] = {false, false, false, false, false, false};
-#define FDX_ATTN_FWD_LAUNCH(DHV, SH, DU, IDX)                                                                     \
+  static bool attr[4] = {false, false, false, false};
+#define FDX_ATTN_FWD_LAUNCH(DHV, SH, IDX)                                                                         \
   {                                                                                                               \
     if (!attr[IDX]) {                                                                                             \
-      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_fwd_kernel<DHV, SH, DU>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_fwd_kernel<DHV, SH>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
                                     smem));                                                                       \
       attr[IDX] = true;                                                                                           \
     }                                                                                                             \
-    fdx_attn_fwd_kernel<DHV, SH, DU><<<grid, kThreads, smem, (cudaStream_t)stream>>>(mQ, mK, mV, d);               \
+    fdx_attn_fwd_kernel<DHV, SH><<<grid, kThreads, smem, (cudaStream_t)stream>>>(mQ, mK, mV, d);                  \
   }
   if (a->dh == 64) {
-    if (short_keys) FDX_ATTN_FWD_LAUNCH(64, true, false, 0)
-    else if (dual) FDX_ATTN_FWD_LAUNCH(64, false, true, 4)
-    else FDX_ATTN_FWD_LAUNCH(64, false, false, 1)
+    if (short_keys) FDX_ATTN_FWD_LAUNCH(64, true, 0)
+    else FDX_ATTN_FWD_LAUNCH(64, false, 1)
   } else {
-    if (short_keys) FDX_ATTN_FWD_LAUNCH(32, true, false, 2)
-    else if (dual) FDX_ATTN_FWD_LAUNCH(32, false, true, 5)
-    else FDX_ATTN_FWD_LAUNCH(32, false, false, 3)
+    if (short_keys) FDX_ATTN_FWD_LAUNCH(32, true, 2)
+    else FDX_ATTN_FWD_LAUNCH(32, false, 3)
   }
 #undef FDX_ATTN_FWD_LAUNCH
   fdx_note_kernel(FDX_KERNEL_ATTN_FWD);
@@ -657,24 +553,20 @@ int fdx_attention_bwd(const fdx_attn_desc* a, void* stream) {
     attn_dvec_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d);
     FDX_LAUNCH_CHECK();
   }
-  const int smem = (2 + 2 * 2 + 4) * kTile + 2 * 256 * 4 + 1024 + 256;
-  static bool attr[8] = {false, false, false, false, false, false, false, false};
-  const bool one_group = getenv("FDX_ATTN_BWD_EWG1") != nullptr;   // round-2a arrangement: four element-wise warps
-#define FDX_ATTN_BWD_LAUNCH1(DHV, RK, EW, IDX, GRIDX, M1, M2, M3, M4)                                             \
+  const int smem = (2 + 2 * 2 + 4) * kTile + 2 * 256 * 4 + 2 * kAccXchgBytes + 1024 + 256;
+  static bool attr[4] = {false, false, false, false};
+#define FDX_ATTN_BWD_LAUNCH(DHV, RK, IDX, GRIDX, M1, M2, M3, M4)                                                  \
   {                                                                                                                \
     if (!attr[IDX]) {                                                                                              \
-      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_bwd_kernel<DHV, RK, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_bwd_kernel<DHV, RK>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
                                     smem));                                                                        \
       attr[IDX] = true;                                                                                            \
     }                                                                                                              \
     dim3 grid((GRIDX + 127) / 128, a->heads, a->B);                                                                \
-    fdx_attn_bwd_kernel<DHV, RK, EW><<<grid, 64 + 128 * EW, smem, st>>>(M1, M2, M3, M4, d);                        \
+    fdx_attn_bwd_kernel<DHV, RK><<<grid, kBwdThreads, smem, st>>>(M1, M2, M3, M4, d);                              \
     fdx_note_kernel(FDX_KERNEL_ATTN_BWD);                                                                          \
     FDX_LAUNCH_CHECK();                                                                                            \
   }
-#define FDX_ATTN_BWD_LAUNCH(DHV, RK, IDX, GRIDX, M1, M2, M3, M4)                                                  \
-  if (one_group) FDX_ATTN_BWD_LAUNCH1(DHV, RK, 1, IDX, GRIDX, M1, M2, M3, M4)                                      \
-  else FDX_ATTN_BWD_LAUNCH1(DHV, RK, 2, (IDX + 4), GRIDX, M1, M2, M3, M4)
   if (a->dh == 64) {
     FDX_ATTN_BWD_LAUNCH(64, false, 0, a->L, mQ, mDO, mK, mV)      // dQ: rows = queries (Q, dO), loop (K_j, V_j)
     FDX_ATTN_BWD_LAUNCH(64, true, 1, a->Lk, mK, mV, mQ, mDO)      // dK/dV: rows = keys (K, V), loop (Q_i, dO_i)
@@ -683,7 +575,6 @@ int fdx_attention_bwd(const fdx_attn_desc* a, void* stream) {
     FDX_ATTN_BWD_LAUNCH(32, true, 3, a->Lk, mK, mV, mQ, mDO)
   }
 #undef FDX_ATTN_BWD_LAUNCH
-#undef FDX_ATTN_BWD_LAUNCH1
   return FDX_OK;
 }
 

@@ -1,7 +1,7 @@
-// fdx_common.cuh -- shared device helpers for the libfdx sm_100a kernels.
+// fdx_common.cuh -- shared device helpers for the libfdx sm_90a kernels.
 //
-// Thin inline-PTX wrappers for the Blackwell primitives the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld),
+// Thin inline-PTX wrappers for the Hopper primitives the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors),
 // plus error plumbing for the C-ABI.  No torch, no CUTLASS types.
 #pragma once
 #include <cuda_runtime.h>
@@ -117,157 +117,194 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ----- tcgen05 ---------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 (bf16/f16 in, f32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread retire
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// ----- CTA pair (cta_group::2): two SMs of one TPC execute one M=256 MMA; each CTA stages its own 128
-//       rows of A and HALF of B's columns, halving B's shared-memory traffic per FLOP ---------------
+// ----- clusters ----------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ uint32_t cluster_id_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctaid_x() {   // number of clusters in the grid
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-  return r;
-}
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address -> CTA 0
-// TMA load issued by EITHER CTA of a pair; its bytes complete on the LEADER's mbarrier (same offset).
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                int c0, int c1, int c2, int c3) {
+
+// ----- wgmma ----------------------------------------------------------------------
+// One warpgroup (four consecutive warps, the first a multiple of four) computes D(64 x N, f32 registers)
+// += A(64 x 16) * B(16 x N), both operands read from shared memory through matrix descriptors.  TA / TB = 1
+// selects an MN-major (transposed) operand, 0 a K-major one.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uint64_t db) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %20, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1, %18, %19;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
 }
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %36, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, %34, %35;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
 }
-// arrive on the mbarrier at this offset in BOTH CTAs when the pair's previously issued MMAs retire
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-          "r"(smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %68, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, %66, %67;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
 }
-// arrive on the mbarrier at this offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n192k16(float (&d)[96], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets TMEM lane (base+i), 32 columns.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %100, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+      "}, %96, %97, p, 1, 1, %98, %99;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
 }
 
-// ----- UMMA descriptors -------------------------------------------------------
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//  [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [46,48) version=1
-//  [49,52) base_offset  [52] lbo_mode  [61,64) layout (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes) {
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N == 32 || N == 64 || N == 128 || N == 192, "wgmma_bf16: unsupported N");
+  if constexpr (N == 32) wgmma_m64n32k16<TA, TB>(d, da, db);
+  else if constexpr (N == 64) wgmma_m64n64k16<TA, TB>(d, da, db);
+  else if constexpr (N == 128) wgmma_m64n128k16<TA, TB>(d, da, db);
+  else wgmma_m64n192k16<TA, TB>(d, da, db);
+}
+
+// ----- GMMA shared-memory descriptors --------------------------------------------
+//  [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [49,52) base_offset  [62,64) layout (1 = SWIZZLE_128B)
+//  K-major, 128B swizzle: rows of 64 bf16 (128 B), SBO = 1024 (8 rows); K advances 16 elements = +32 B.
+//  MN-major, 128B swizzle: 64-element MN runs per K row; LBO = byte stride between 64-wide MN blocks,
+//  SBO = 1024 (8 K rows); K advances 16 rows = +2048 B.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor for kind::f16 with bf16 A/B, f32 D (cute::UMMA::InstrDescriptor):
-//  [4,6) c_format=1(F32) [7,10) a_format=1(BF16) [10,13) b_format=1(BF16)
-//  [15] a_major (0=K,1=MN) [16] b_major [17,23) N>>3 [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// Warp-specialised kernels with two consumer warpgroups and one producer warpgroup (384 threads): the
+// register file is budgeted per warpgroup, so the producer hands its registers to the consumers.
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory"); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory"); }
+
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+
+// ----- warpgroup accumulator ---------------------------------------------------------
+// A 128 x WN f32 tile held by one warpgroup as two m64 wgmma fragments (rows 0..63 and 64..127).
+// row32() hands each thread one accumulator row (by default row 32 w + l for warp w of the warpgroup, lane l),
+// columns [c, c + 32): the one-row-per-thread layout the epilogues work in.  The fragments cross through a 128 x 32 f32 tile
+// in shared memory (kAccXchgBytes per warpgroup, 16-byte aligned); every thread of the warpgroup must call
+// it with the same c.  Named barrier `bar` (one per warpgroup) orders the exchange.
+constexpr int kAccXchgLd = 36;                 // padded row: conflict-free 16-byte row reads
+constexpr int kAccXchgBytes = 128 * kAccXchgLd * 4;
+
+template <int WN>
+struct WgAcc {
+  static_assert(WN == 32 || WN == 64 || WN == 128, "WgAcc: N = 32, 64 or 128");
+  float d[2][WN / 2];
+
+  __device__ __forceinline__ void zero() {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < WN / 2; ++i) d[h][i] = 0.f;
+  }
+  // rows 0..63 from da_lo, rows 64..127 from da_hi, all WN columns from db (one K = 16 step)
+  template <int TA, int TB>
+  __device__ __forceinline__ void mma(uint64_t da_lo, uint64_t da_hi, uint64_t db) {
+    wgmma_bf16<WN, TA, TB>(d[0], da_lo, db);
+    wgmma_bf16<WN, TA, TB>(d[1], da_hi, db);
+  }
+  // one 64-row half only (h = 0: rows 0..63, 1: rows 64..127)
+  template <int TA, int TB>
+  __device__ __forceinline__ void mma_half(int h, uint64_t da, uint64_t db) {
+    if (h == 0) wgmma_bf16<WN, TA, TB>(d[0], da, db);
+    else wgmma_bf16<WN, TA, TB>(d[1], da, db);
+  }
+  // row < 0: row 32 w + l of the calling thread (warp w of the warpgroup, lane l)
+  __device__ __forceinline__ void row32(float* xs, int bar, int c, float (&f)[32], int row = -1) const {
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+    if (row < 0) row = w * 32 + l;
+    named_bar_sync(bar, 128);                  // the previous chunk's reads of xs are done
+#pragma unroll
+    for (int cc = 0; cc < WN / 32; ++cc) {
+      if (cc == (c >> 5)) {                     // compile-time register indices, run-time chunk
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int r = h * 64 + w * 16 + (l >> 2), col = j * 8 + 2 * (l & 3);
+            const float* s = &d[h][(cc * 4 + j) * 4];
+            *reinterpret_cast<float2*>(xs + r * kAccXchgLd + col) = make_float2(s[0], s[1]);
+            *reinterpret_cast<float2*>(xs + (r + 8) * kAccXchgLd + col) = make_float2(s[2], s[3]);
+          }
+      }
+    }
+    named_bar_sync(bar, 128);
+    const float4* src = reinterpret_cast<const float4*>(xs + row * kAccXchgLd);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float4 v = src[j];
+      f[4 * j] = v.x; f[4 * j + 1] = v.y; f[4 * j + 2] = v.z; f[4 * j + 3] = v.w;
+    }
+  }
+};
 
 // ----- misc ------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
@@ -292,53 +329,27 @@ __device__ __forceinline__ float sigmoid_fast(float z) {
 }
 __device__ __forceinline__ float silu_f(float z) { return z * sigmoid_fast(z); }
 
-// ---- packed f32x2 arithmetic (sm_100: FFMA2 / FADD2 - two f32 lanes per instruction) ---------------
-// The streaming GroupNorm kernels are instruction-issue limited, not HBM limited, when written with
-// scalar f32 ops (ncu: 20-24 instructions per element); the packed forms halve the FP instruction count.
-typedef unsigned long long f32x2_t;
-__device__ __forceinline__ f32x2_t f2_pack(float lo, float hi) {
-  f32x2_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(f32x2_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
+// ---- f32 pairs ---------------------------------------------------------------------------------------
+// The streaming GroupNorm kernels work on channel pairs; sm_90 has no packed f32x2 instructions, so each
+// pair operation is two scalar f32 operations.
+typedef float2 f32x2_t;
+__device__ __forceinline__ f32x2_t f2_pack(float lo, float hi) { return make_float2(lo, hi); }
+__device__ __forceinline__ void f2_unpack(f32x2_t v, float& lo, float& hi) { lo = v.x; hi = v.y; }
 __device__ __forceinline__ f32x2_t f2_fma(f32x2_t a, f32x2_t b, f32x2_t c) {
-  f32x2_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-__device__ __forceinline__ f32x2_t f2_mul(f32x2_t a, f32x2_t b) {
-  f32x2_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2_t f2_add(f32x2_t a, f32x2_t b) {
-  f32x2_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2_t f2_sub(f32x2_t a, f32x2_t b) {
-  f32x2_t d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// bf16x2 word -> (lo, hi) as f32x2: a shift and a mask
+__device__ __forceinline__ f32x2_t f2_mul(f32x2_t a, f32x2_t b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ f32x2_t f2_add(f32x2_t a, f32x2_t b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ f32x2_t f2_sub(f32x2_t a, f32x2_t b) { return make_float2(a.x - b.x, a.y - b.y); }
+// bf16x2 word -> (lo, hi): a shift and a mask
 __device__ __forceinline__ f32x2_t f2_from_bf16x2(uint32_t u) {
   return f2_pack(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
 }
-__device__ __forceinline__ uint32_t f2_to_bf16x2(f32x2_t v) {
-  float lo, hi;
-  f2_unpack(v, lo, hi);
-  return pack_bf16x2(lo, hi);
-}
+__device__ __forceinline__ uint32_t f2_to_bf16x2(f32x2_t v) { return pack_bf16x2(v.x, v.y); }
 __device__ __forceinline__ f32x2_t f2_tanh(f32x2_t v) {
-  float lo, hi;
-  f2_unpack(v, lo, hi);
-  asm("tanh.approx.f32 %0, %0;" : "+f"(lo));
-  asm("tanh.approx.f32 %0, %0;" : "+f"(hi));
-  return f2_pack(lo, hi);
+  asm("tanh.approx.f32 %0, %0;" : "+f"(v.x));
+  asm("tanh.approx.f32 %0, %0;" : "+f"(v.y));
+  return v;
 }
 
 #endif  // __CUDACC__

@@ -202,7 +202,7 @@ cout3_dgrad_kernel(const float* __restrict__ dF, const float* __restrict__ w, in
 }
 
 // ---- im2col of a 3-channel tensor: col[p][t*3+k] = S[p + sgn*d(t)][k] (0 outside), bf16 [P][32];
-//      column 27 optionally = 1 (bias row), columns 28..31 = 0.  Feeds the tcgen05 engine so the two
+//      column 27 optionally = 1 (bias row), columns 28..31 = 0.  Feeds the wgmma engine so the two
 //      3-channel weight gradients are (pixels x 32)^T (pixels x 64) GEMMs instead of CUDA-core loops.
 template <bool SMALL_F32>
 __global__ void __launch_bounds__(256)
@@ -287,7 +287,7 @@ int fdx_im2col3x3_c3(const void* src, int src_is_f32, int sgn, int N, int H, int
   FDX_REQUIRE(sgn == 1 || sgn == -1, "im2col3x3_c3: sgn must be +1 or -1");
   const long long npix = (long long)N * H * W;
   long long grid = (npix + 255) / 256;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > fdx_num_sms() * 16) grid = fdx_num_sms() * 16;
   if (src_is_f32)
     im2col3_kernel<true><<<(int)grid, 256, 0, (cudaStream_t)stream>>>(src, sgn, N, H, W, ones_col,
                                                                       (__nv_bfloat16*)col_bf16);
@@ -305,7 +305,7 @@ int fdx_conv_in_fwd(const void* x_bf16, int N, int H, int W, const float* w_hwio
               "conv_in_fwd: bad output shape");
   const long long total = (long long)N * H * W * (y->c / 8);
   long long grid = (total + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > fdx_num_sms() * 8) grid = fdx_num_sms() * 8;
   cin3_fwd_kernel<<<(int)grid, 256, sizeof(float) * 28 * y->c, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)x_bf16, w_hwio, bias, N, H, W, y->c, (__nv_bfloat16*)y->ptr,
       y->pix_stride);
@@ -317,7 +317,7 @@ int fdx_conv_in_wgrad(const void* x_bf16, const fdx_act* dy, float* dw_hwio, flo
                       void* stream) {
   FDX_REQUIRE(x_bf16 && dy && dy->ptr && dw_hwio, "conv_in_wgrad: null pointer");
   FDX_REQUIRE(dy->c == 64, "conv_in_wgrad: Cout must be 64 (got %d)", dy->c);
-  rank27_wgrad_kernel<false, +1><<<148 * 4, 256, 0, (cudaStream_t)stream>>>(
+  rank27_wgrad_kernel<false, +1><<<fdx_num_sms() * 4, 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)dy->ptr, dy->pix_stride, x_bf16, dy->n, dy->h, dy->w, dw_hwio, dbias);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
@@ -328,7 +328,7 @@ int fdx_col2im3x3_c3(const float* col_f32, const float* bias, int N, int H, int 
   FDX_REQUIRE(col_f32 && y_f32 && N > 0 && H > 0 && W > 0, "col2im3x3_c3: bad arguments");
   const long long npix = (long long)N * H * W;
   long long grid = (npix + 255) / 256;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > fdx_num_sms() * 16) grid = fdx_num_sms() * 16;
   col2im3_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(col_f32, bias, N, H, W, y_f32);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
@@ -340,7 +340,7 @@ int fdx_conv_out_fwd(const fdx_act* x, const float* w_hwio, const float* bias, f
   FDX_REQUIRE(x->c % 8 == 0 && x->c <= 256, "conv_out_fwd: bad Cin %d", x->c);
   const long long npix = (long long)x->n * x->h * x->w;
   long long grid = (npix + 127) / 128;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > fdx_num_sms() * 16) grid = fdx_num_sms() * 16;
   cout3_fwd_kernel<<<(int)grid, 128, sizeof(float) * 27 * x->c, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)x->ptr, x->pix_stride, w_hwio, bias, x->n, x->h, x->w, x->c, y_f32);
   FDX_LAUNCH_CHECK();
@@ -352,7 +352,7 @@ int fdx_conv_out_dgrad(const float* dF, const float* w_hwio, const fdx_act* dx, 
   FDX_REQUIRE(dx->c % 8 == 0 && dx->c <= 256, "conv_out_dgrad: bad Cin %d", dx->c);
   const long long total = (long long)dx->n * dx->h * dx->w * (dx->c / 8);
   long long grid = (total + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > fdx_num_sms() * 8) grid = fdx_num_sms() * 8;
   cout3_dgrad_kernel<<<(int)grid, 256, sizeof(float) * 27 * dx->c, (cudaStream_t)stream>>>(
       dF, w_hwio, dx->n, dx->h, dx->w, dx->c, (__nv_bfloat16*)dx->ptr, dx->pix_stride);
   FDX_LAUNCH_CHECK();
@@ -363,7 +363,7 @@ int fdx_conv_out_wgrad(const fdx_act* x, const float* dF, float* dw_hwio, float*
                        void* stream) {
   FDX_REQUIRE(x && x->ptr && dF && dw_hwio, "conv_out_wgrad: null pointer");
   FDX_REQUIRE(x->c == 64, "conv_out_wgrad: Cin must be 64 (got %d)", x->c);
-  rank27_wgrad_kernel<true, -1><<<148 * 4, 256, 0, (cudaStream_t)stream>>>(
+  rank27_wgrad_kernel<true, -1><<<fdx_num_sms() * 4, 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)x->ptr, x->pix_stride, dF, x->n, x->h, x->w, dw_hwio, dbias);
   FDX_LAUNCH_CHECK();
   return FDX_OK;

@@ -106,9 +106,7 @@ const char* fdx_kernel_kind_name(int kind) {
   switch (kind) {
     case FDX_KERNEL_TC: return "fdx_tc_kernel";
     case FDX_KERNEL_TCT: return "fdx_tct_kernel";
-    case FDX_KERNEL_WGRAD9K: return "fdx_wgrad9k_kernel";
     case FDX_KERNEL_WGRAD9: return "fdx_wgrad9_kernel";
-    case FDX_KERNEL_CONV3: return "fdx_conv3_kernel";
     case FDX_KERNEL_ATTN_FWD: return "fdx_attn_fwd_kernel";
     case FDX_KERNEL_ATTN_BWD: return "fdx_attn_bwd_kernel";
   }

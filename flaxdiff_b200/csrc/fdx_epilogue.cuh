@@ -1,20 +1,19 @@
-// fdx_epilogue.cuh -- coalesced bf16 epilogue for the tcgen05 kernels.
+// fdx_epilogue.cuh -- coalesced bf16 epilogue for the wgmma kernels.
 //
-// tcgen05.ld hands every thread of an epilogue warp one accumulator ROW (one output pixel).  Storing
+// WgAcc::row32 hands every thread of a consumer warp one accumulator ROW (one output pixel).  Storing
 // straight from that layout makes each 16-byte store instruction of a warp touch 32 different cache
-// lines; ncu showed the epilogue warps, not the tensor pipe, bounding the short-K (Cin = 64) tiles
-// (tensor pipe 22 % active, producer parked on a full ring, issuer never waiting for data).
-// Here each warp stages its 32 rows x 64 channels (4 KB, XOR-swizzled 16-byte pieces, conflict free)
+// lines.  Here each warp stages its 32 rows x 64 channels (4 KB, XOR-swizzled 16-byte pieces, conflict free)
 // in shared memory and moves it to / from global memory with 8 lanes per pixel: four complete
 // 128-byte lines per instruction, for the store and for the fused side-input read alike.  The side
 // input (residual, or the GroupNorm input below) of the first 64-column chunk is requested BEFORE the
 // warp waits for the accumulator, and that of chunk c+1 while chunk c is being converted, so its
-// global-memory latency never sits on the epilogue's critical path.
+// global-memory latency never sits on the epilogue's critical path; the first one is in flight while the
+// warpgroup runs its main loop.
 //
 // EPI = EPI_COLSTATS additionally accumulates, per (image, output channel), the sum and the sum of
 // squares of the bf16 values it stores: the statistics pass of the GroupNorm that consumes this tensor
 // (flaxdiff/models/common.py:273-288) then never reads it (2 B/element saved; two fused multiply-adds
-// per element in the coalesced store phase - cheap enough for the four epilogue warps, unlike silu').
+// per element in the coalesced store phase).
 //
 // EPI = EPI_GN_BWD fuses the first pass of GroupNorm(+SiLU) backward (flaxdiff/models/common.py:286-288,
 // 310-312 under jax.grad) into the data-gradient convolution that produces its input: with
@@ -49,20 +48,18 @@ __device__ __forceinline__ float epi_silu_grad_times(float dy, float z) {
   return dy * sg * (1.f + z * (1.f - sg));
 }
 
-// One warp, its 32 accumulator rows, all BN columns of the tile.
+// One warp of a consumer warpgroup, its 32 accumulator rows, the warpgroup's WN columns of the tile.
 //   stage   : this warp's 4 KB staging tile (shared memory, 128-byte aligned)
-//   t_addr  : TMEM address of (first lane of this warp's quarter, first column of the accumulator)
-//   col_base: first global output column of the tile (nt * BN)
+//   acc, xs, xbar : the warpgroup's accumulator, its exchange tile and named barrier (see WgAcc::row32)
+//   col_base: first global output column of the warpgroup's columns
 //   valid / obase / rbase / img : this LANE's row: in range?, element offsets into out / res, image index
-//   wait_acc: called once, after the first side-input loads are in flight, to wait for the accumulator
-//   GN only : q = warp quarter (0..3), xchg = 2 x 2 KB CTA-shared exchange area, par = running chunk
-//             parity (kept by the caller across tiles), slot = workspace slot of this tile; all rows
-//             of the tile belong to image `img` of lane 0.
-template <int BN, int EPI, int PARTS, class WaitFn>
-__device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_t* stage, uint32_t t_addr,
-                                                       int lane, int col_base, bool valid, long long obase,
-                                                       long long rbase, int img, WaitFn wait_acc, int q = 0,
-                                                       float* xchg = nullptr, int* par = nullptr,
+//   mainloop: called once, after the first side-input loads are in flight, to compute the accumulator
+//   GN only : par = running chunk parity (kept by the caller across tiles), slot = workspace slot of
+//             this tile; all rows of the tile belong to image `img` of lane 0.
+template <int WN, int EPI, class Acc, class MainFn>
+__device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_t* stage, const Acc& acc, float* xs,
+                                                       int xbar, int lane, int col_base, bool valid, long long obase,
+                                                       long long rbase, int img, MainFn mainloop, int* par = nullptr,
                                                        int slot = 0) {
   constexpr bool GN = (EPI == EPI_GN_BWD);
   constexpr bool SUMS = (EPI != EPI_PLAIN);
@@ -85,7 +82,7 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
 
   auto load_side = [&](int c0, uint4 (&dst)[8]) {
     const int col0 = col_base + c0;
-    const bool in = (c0 < BN) && (col0 < e.Ncols);
+    const bool in = (c0 < WN) && (col0 < e.Ncols);
     const bool half2 = (col0 + 32) < e.Ncols;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
@@ -97,10 +94,10 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
 
   uint4 xr[8];
   if (side) load_side(0, xr);
-  wait_acc();
+  mainloop();
 
 #pragma unroll 1
-  for (int c0 = 0; c0 < BN; c0 += 64) {
+  for (int c0 = 0; c0 < WN; c0 += 64) {
     const int col0 = col_base + c0;
     if (col0 >= e.Ncols) break;                      // uniform over the CTA
     const bool half2 = (col0 + 32) < e.Ncols;        // second 32-column half present (Ncols % 32 == 0)
@@ -119,19 +116,8 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (h == 1 && !half2) break;
-      uint32_t v[32];
-      tmem_ld_32x32(t_addr + c0 + h * 32, v);
-      tmem_ld_wait();
       float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-#pragma unroll
-      for (int pp = 1; pp < PARTS; ++pp) {             // partial accumulators (see TcCfg::kParts)
-        tmem_ld_32x32(t_addr + pp * BN + c0 + h * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] += __uint_as_float(v[j]);
-      }
+      acc.row32(xs, xbar, c0 + h * 32, f);
 #pragma unroll
       for (int j = 0; j < 32; ++j) f[j] *= e.alpha;
       if (e.bias) {
@@ -230,37 +216,7 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
         s0[i] += __shfl_xor_sync(0xffffffffu, s0[i], 16);
         s1[i] += __shfl_xor_sync(0xffffffffu, s1[i], 16);
       }
-      // Each warp adds its own 32-row partial (lanes 0..7 own 8 channels each) with 16-byte reductions.  Round 1
-      // exchanged the four warps' partials through shared memory behind a 128-thread barrier per 64-column
-      // chunk - that barrier serialised the epilogue warps (Upsample forward: 15 K cycles per 128 x 256 tile against
-      // 4.8 K of MMA time).  FDX_EPI_XCHG (compile-time) keeps the old exchange for comparison.
-#ifdef FDX_EPI_XCHG
-      float* xb = xchg + (*par) * 512 + q * 128;      // [par][warp][which][64]
-      if (lane < 8) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          xb[piece * 8 + i] = s0[i];
-          xb[64 + piece * 8 + i] = s1[i];
-        }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");   // the four epilogue warps
-      if (q == 0) {
-        const int which = lane >> 4, c4 = (lane & 15) * 4;
-        const float* xs = xchg + (*par) * 512 + which * 64 + c4;
-        float4 t = *reinterpret_cast<const float4*>(xs);
-#pragma unroll
-        for (int w = 1; w < 4; ++w) {
-          const float4 o = *reinterpret_cast<const float4*>(xs + w * 128);
-          t.x += o.x; t.y += o.y; t.z += o.z; t.w += o.w;
-        }
-        if (c4 < 32 || half2) {
-          float* dst = e.gn_ws + (((long long)slot * e.gn_N + img0) * 2 + which) * e.ws_ld + col0 + c4;
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(t.x), "f"(t.y),
-                       "f"(t.z), "f"(t.w)
-                       : "memory");
-        }
-      }
-#else
+      // each warp adds its own 32-row partial (lanes 0..7 own 8 channels each) with 16-byte reductions
       if (lane < 8 && (piece < 4 || half2)) {
         float* d0 = e.gn_ws + (((long long)slot * e.gn_N + img0) * 2) * e.ws_ld + col0 + piece * 8;
         float* d1 = d0 + e.ws_ld;
@@ -273,7 +229,6 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
         asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d1 + 4), "f"(s1[4]), "f"(s1[5]),
                      "f"(s1[6]), "f"(s1[7]) : "memory");
       }
-#endif
       *par ^= 1;
     }
     __syncwarp();

@@ -9,7 +9,7 @@ namespace {
 
 inline int stream_grid(long long work_items, int block) {
   long long g = (work_items + block - 1) / block;
-  const long long cap = 148LL * 8;
+  const long long cap = (long long)fdx_num_sms() * 8;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
   return (int)g;

@@ -175,7 +175,7 @@ int fdx_time_embed_bwd(const float* demb, const float* four, const float* h1, co
 int fdx_softmax_fwd(const float* S, long long rows, int L, int Lp, void* P_bf16, void* stream) {
   FDX_REQUIRE(S && P_bf16 && rows > 0 && L > 0 && Lp >= L, "softmax_fwd: bad arguments");
   long long grid = (rows + 7) / 8;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > fdx_num_sms() * 16) grid = fdx_num_sms() * 16;
   softmax_fwd_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(S, rows, L, Lp,
                                                                  (__nv_bfloat16*)P_bf16);
   FDX_LAUNCH_CHECK();
@@ -186,7 +186,7 @@ int fdx_softmax_bwd(const void* P_bf16, const float* dP, long long rows, int L, 
                     void* dS_bf16, void* stream) {
   FDX_REQUIRE(P_bf16 && dP && dS_bf16 && rows > 0 && L > 0 && Lp >= L, "softmax_bwd: bad arguments");
   long long grid = (rows + 7) / 8;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > fdx_num_sms() * 16) grid = fdx_num_sms() * 16;
   softmax_bwd_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)P_bf16, dP, rows, L, Lp, scale, (__nv_bfloat16*)dS_bf16);
   FDX_LAUNCH_CHECK();

@@ -9,7 +9,8 @@
 //
 // HBM-bound kernels: every thread owns one 16-byte (8 x bf16) channel vector of a pixel,
 // fully coalesced; per-(image,group) partial sums are reduced with warp shuffles,
-// then shared-memory atomics, then one global atomic per block.
+// then shared-memory atomics, then one global atomic per block - except the forward statistics
+// (gn_stats_kernel), which are reduced in a fixed order so that they do not change from run to run.
 #include "fdx_common.cuh"
 #include <stdlib.h>
 #include "../../include/fdx.h"
@@ -36,52 +37,44 @@ __device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&f)[8]) {
   *reinterpret_cast<uint4*>(p) = u;
 }
 
-// stats[n][g] = (sum, sumsq) accumulated with atomics (buffer zeroed by the caller)
 constexpr int kU = 4;   // pixels in flight per thread (memory-level parallelism)
 
+// stats[n][g] = (sum, sumsq).  One block per (group, image) reduces all of the group's elements in a fixed
+// order (strided per-thread sums, warp shuffles, then the warps in index order), so the statistics are the
+// same from run to run: with float atomics the summation order varies, and a one-ulp change of a mean flips
+// bf16 roundings in everything downstream.
 __global__ void __launch_bounds__(kNT)
 gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int C, int G,
                 float* __restrict__ stats) {
-  const int vpp = C >> 3, rows = kNT / vpp, cpg = C / G;
-  const int n = blockIdx.y;
-  const int tid = threadIdx.x;
-  __shared__ float sh[64];
-  if (tid < 2 * G) sh[tid] = 0.f;
-  __syncthreads();
-  if (tid < rows * vpp) {
-    const int cv = tid % vpp, r = tid / vpp;
-    const int g = (cv * 8) / cpg;
-    float s = 0.f, q = 0.f;
-    const __nv_bfloat16* base = x + (long long)n * HW * xps + cv * 8;
-    const int stride = gridDim.x * rows;
-    int p = blockIdx.x * rows + r;
-    for (; p + (kU - 1) * stride < HW; p += kU * stride) {
-      uint4 u[kU];
+  const int cpg = C / G, vpg = cpg >> 3;         // 16-byte vectors of one group per pixel
+  const int g = blockIdx.x, n = blockIdx.y;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const __nv_bfloat16* base = x + (long long)n * HW * xps + g * cpg;
+  const long long items = (long long)HW * vpg;
+  float s = 0.f, q = 0.f;
+#pragma unroll 4
+  for (long long i = tid; i < items; i += kNT) {
+    const long long p = i / vpg;
+    float f[8];
+    load8(base + p * xps + (i - p * vpg) * 8, f);
 #pragma unroll
-      for (int k = 0; k < kU; ++k)
-        u[k] = *reinterpret_cast<const uint4*>(base + (long long)(p + k * stride) * xps);
-#pragma unroll
-      for (int k = 0; k < kU; ++k) {
-        const float2 a = unpack_bf16x2(u[k].x), b = unpack_bf16x2(u[k].y), c = unpack_bf16x2(u[k].z),
-                     d = unpack_bf16x2(u[k].w);
-        s += (a.x + a.y) + (b.x + b.y) + (c.x + c.y) + (d.x + d.y);
-        q += a.x * a.x + a.y * a.y + b.x * b.x + b.y * b.y + c.x * c.x + c.y * c.y + d.x * d.x + d.y * d.y;
-      }
-    }
-    for (; p < HW; p += stride) {
-      float f[8];
-      load8(base + (long long)p * xps, f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { s += f[j]; q += f[j] * f[j]; }
-    }
-    atomicAdd(&sh[2 * g], s);
-    atomicAdd(&sh[2 * g + 1], q);
+    for (int j = 0; j < 8; ++j) { s += f[j]; q = fmaf(f[j], f[j], q); }
   }
+  s = warp_sum(s);
+  q = warp_sum(q);
+  __shared__ float sh[2][kNT / 32];
+  if (lane == 0) { sh[0][warp] = s; sh[1][warp] = q; }
   __syncthreads();
-  if (tid < 2 * G) atomicAdd(&stats[(long long)n * 2 * G + tid], sh[tid]);
+  if (tid == 0) {
+    float a = 0.f, b = 0.f;
+#pragma unroll
+    for (int w = 0; w < kNT / 32; ++w) { a += sh[0][w]; b += sh[1][w]; }
+    stats[((long long)n * G + g) * 2] = a;
+    stats[((long long)n * G + g) * 2 + 1] = b;
+  }
 }
 
-// y = silu?(a x + b) per channel pair with packed f32x2 ops: h = x*(a/2) + b/2, silu(z) = h*(1 + tanh(h))
+// y = silu?(a x + b) per channel pair: h = x*(a/2) + b/2, silu(z) = h*(1 + tanh(h))
 template <bool SILU>
 __global__ void __launch_bounds__(kNT)
 gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int C, int G,
@@ -170,11 +163,10 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int 
 // and pass 2 is  dx = dz*a_c - x*c2 + c3  with per-group c2 = rstd^2*m2, c3 = mean*c2 - rstd*m1.
 // Both passes are instruction-issue sensitive (two MUFU per element), hence the reduced algebra.
 
-// The two streaming passes of the backward are written with packed f32x2 arithmetic (FFMA2): with
-// scalar ops ncu counted 20-24 instructions per element and an issue-slot utilisation that capped both
-// passes at 56-63 % of the HBM rate.  Per channel PAIR: h = x*(a/2) + b/2, t = tanh(h),
+// The two streaming passes of the backward work on channel pairs (f32x2_t, fdx_common.cuh) with reduced
+// algebra, because they are instruction-issue sensitive.  Per channel PAIR: h = x*(a/2) + b/2, t = tanh(h),
 //   sigmoid(z) = (1+t)/2,  silu'(z) = sigmoid(z) * (1 + h*(1-t)),  dz = dy * silu'(z)
-// = 6 packed ops + 2 MUFU.  Every thread owns 8 channels (16-byte vectors) of kBU pixels per iteration.
+// = 6 pair ops + 2 MUFU.  Every thread owns 8 channels (16-byte vectors) of kBU pixels per iteration.
 constexpr int kBU = 3;   // pixels in flight per thread
 
 struct GnPair4 { f32x2_t v[4]; };
@@ -576,8 +568,8 @@ gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps,
 // statistics it needs are per IMAGE, so here a cluster of CL CTAs owns one image: every CTA runs pass 1 on
 // its slice of the pixels, the per-channel sums are exchanged through distributed shared memory
 // (mapa + ld.shared::cluster), every CTA derives the per-group constants, and pass 2 re-reads the SAME
-// slice - a few hundred microseconds later at most, while the lines are still in the 126 MB L2 (the launch
-// keeps the images in flight, 148 / CL clusters, below ~48 MB of x + dy).  HBM traffic: 4 B read + 2 B
+// slice - a few hundred microseconds later at most, while the lines are still in the 50 MB L2 (the launch
+// keeps the images in flight, SMs / CL clusters, below ~20 MB of x + dy).  HBM traffic: 4 B read + 2 B
 // written per element.  ws[n][c] = (S0, S1) is still written (rank 0) for the dgamma / dbeta finalize.
 __device__ __forceinline__ uint32_t cluster_nctarank() {
   uint32_t r;
@@ -1173,14 +1165,14 @@ int gn_check(const fdx_act* x, int groups, const char* what) {
 
 // Two waves of co-resident blocks (`resident` per SM for the kernel in question): every block then
 // amortises its prologue (statistics / gamma / beta loads) and epilogue (partial-sum reduction, atomics)
-// over many pixel rows.  Sizing for ~16 blocks per SM made the small deep-level tensors pure launch /
-// prologue latency (ncu: 8 MB in 8 us).
+// over many pixel rows.  Sizing for ~16 blocks per SM makes the small deep-level tensors pure launch /
+// prologue latency.
 dim3 gn_grid(const fdx_act* x, int unroll, int resident) {
   const int HW = x->h * x->w;
   const int rows = kNT / (x->c / 8);
   int bx = (HW + rows * unroll - 1) / (rows * unroll);
   static const int waves = getenv("FDX_GN_WAVES") ? atoi(getenv("FDX_GN_WAVES")) : 2;
-  int target = (waves * resident * 148) / x->n;
+  int target = (waves * resident * fdx_num_sms()) / x->n;
   if (target < 1) target = 1;
   if (bx > target) bx = target;
   if (bx < 1) bx = 1;
@@ -1228,10 +1220,10 @@ extern "C" {
 int fdx_groupnorm_stats(const fdx_act* x, int groups, float* stats, void* stream) {
   int s = gn_check(x, groups, "groupnorm_stats");
   if (s != FDX_OK) return s;
-  cudaStream_t st = (cudaStream_t)stream;
-  FDX_CUDA(cudaMemsetAsync(stats, 0, sizeof(float) * 2 * groups * x->n, st));
-  gn_stats_kernel<<<gn_grid(x, kU, 5), kNT, 0, st>>>((const __nv_bfloat16*)x->ptr, x->pix_stride,
-                                              x->h * x->w, x->c, groups, stats);
+  FDX_REQUIRE((x->c / groups) % 8 == 0, "groupnorm_stats: channels per group (%d) must be a multiple of 8",
+              x->c / groups);
+  gn_stats_kernel<<<dim3(groups, x->n), kNT, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x->ptr, x->pix_stride,
+                                                                       x->h * x->w, x->c, groups, stats);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
 }
@@ -1312,8 +1304,9 @@ static int groupnorm_bwd_impl(const fdx_act* x, const fdx_act* dy, int groups, c
   const double img_bytes = 4.0 * HW * C;                      // x + dy of one image, bf16
   int CL = 8;
   while (CL > 1 && (HW / CL) < 4 * (kNT / (C / 8))) CL >>= 1;  // keep >= 4 row iterations per CTA
-  // images in flight with one CTA per SM = 148 / CL; beyond ~64 MB the second pass would miss in L2 anyway
-  const bool fits_l2 = (148.0 / CL) * img_bytes <= 64.0 * 1024 * 1024;
+  // images in flight with one CTA per SM = SMs / CL; beyond ~half the 50 MB L2 the second pass would miss anyway
+  const double sms = (double)fdx_num_sms();
+  const bool fits_l2 = (sms / CL) * img_bytes <= 24.0 * 1024 * 1024;
   // FDX_GN_PIPE=1: the persistent pipelined kernel for the shapes the cluster path cannot take (large images);
   // FDX_GN_PIPE=2: for every shape.  Its stage counters live behind `red` in the caller's workspace
   // (2*N*groups floats >= the <= 2*N stages ever needed... capped to that many stages).
@@ -1348,8 +1341,8 @@ static int groupnorm_bwd_impl(const fdx_act* x, const fdx_act* dy, int groups, c
     return FDX_OK;
   }
   if (!two_pass && HW >= 1024 && fits_l2) {
-    // CTAs per SM so that (148 * per_sm / CL) images * img_bytes <= 48 MB, at least 1
-    int per_sm = (int)((48.0 * 1024 * 1024 * CL) / (148.0 * img_bytes));
+    // CTAs per SM so that (SMs * per_sm / CL) images * img_bytes <= 20 MB, at least 1
+    int per_sm = (int)((20.0 * 1024 * 1024 * CL) / (sms * img_bytes));
     if (per_sm > 2) per_sm = 2;
     if (per_sm < 1) per_sm = 1;
     const size_t need = sizeof(float) * (2 * (size_t)(kNT / (C / 8)) * C + 2 * C + 2 * groups);
@@ -1443,7 +1436,7 @@ int fdx_groupnorm_coeffs(const float* stats, const float* gamma, const float* be
   FDX_REQUIRE(stats && gamma && beta && ab && N > 0 && HW > 0 && C > 0 && groups > 0 && C % groups == 0,
               "groupnorm_coeffs: bad arguments");
   long long grid = ((long long)N * C + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > fdx_num_sms() * 8) grid = fdx_num_sms() * 8;
   gn_coeffs_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(stats, gamma, beta, N, HW, C, groups, eps, ab);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
@@ -1479,7 +1472,7 @@ static int groupnorm_bwd_dz_impl(const fdx_act* x, const fdx_act* dz, int groups
   float* sums = ws;                         // [N][C][2]
   float* red = ws + 2LL * N * C;            // [N][G][2]
   long long cg = ((long long)N * C + 255) / 256;
-  if (cg > 148 * 8) cg = 148 * 8;
+  if (cg > fdx_num_sms() * 8) cg = fdx_num_sms() * 8;
   gn_collapse_slots_kernel<<<(int)cg, 256, 0, st>>>(ws_slots, slots, N, C, sums);
   FDX_LAUNCH_CHECK();
   const int cb = (C + kFinC - 1) / kFinC, gb = (N * groups + 7) / 8;
@@ -1522,7 +1515,7 @@ int fdx_rmsnorm_fwd(const fdx_act* x, const float* scale, float eps, const fdx_a
   FDX_REQUIRE(x->c % 8 == 0 && x->c <= 1024, "rmsnorm_fwd: C=%d must be a multiple of 8, <= 1024", x->c);
   const long long npix = (long long)x->n * x->h * x->w;
   int grid = (int)((npix + 7) / 8);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > fdx_num_sms() * 8) grid = fdx_num_sms() * 8;
   rms_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x->ptr, x->pix_stride, npix,
                                                          x->c, scale, eps, (__nv_bfloat16*)y->ptr,
                                                          y->pix_stride);
@@ -1536,7 +1529,7 @@ int fdx_rmsnorm_bwd(const fdx_act* x, const fdx_act* dy, const float* scale, flo
   FDX_REQUIRE(x->c % 8 == 0 && x->c <= 1024, "rmsnorm_bwd: C=%d must be a multiple of 8, <= 1024", x->c);
   const long long npix = (long long)x->n * x->h * x->w;
   int grid = (int)((npix + 7) / 8);
-  if (grid > 148 * 2) grid = 148 * 2;
+  if (grid > fdx_num_sms() * 2) grid = fdx_num_sms() * 2;
   rms_bwd_kernel<<<grid, 256, sizeof(float) * x->c, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)x->ptr, x->pix_stride, (const __nv_bfloat16*)dy->ptr, dy->pix_stride, npix, x->c,
       scale, eps, (__nv_bfloat16*)dx->ptr, dx->pix_stride, accumulate, dscale);

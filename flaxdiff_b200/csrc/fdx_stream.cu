@@ -18,7 +18,7 @@ namespace {
 
 inline int stream_grid(long long work_items, int block) {
   long long g = (work_items + block - 1) / block;
-  const long long cap = 148LL * 8;
+  const long long cap = (long long)fdx_num_sms() * 8;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
   return (int)g;
@@ -420,7 +420,7 @@ int fdx_colsum(const fdx_act* x, float* out, int per_image, void* stream) {
   const int HW = x->h * x->w;
   const int rows = 256 / (x->c / 8);
   int bx = (HW + 4 * rows - 1) / (4 * rows);
-  int target = (16 * 148 + x->n - 1) / x->n;
+  int target = (16 * fdx_num_sms() + x->n - 1) / x->n;
   if (bx > target) bx = target;
   if (bx < 1) bx = 1;
   cudaStream_t st = (cudaStream_t)stream;

@@ -1,4 +1,4 @@
-// fdx_tc.cu -- the tcgen05 / TMA / TMEM "tap-GEMM" engine for sm_100a.
+// fdx_tc.cu -- the wgmma / TMA "tap-GEMM" engine for sm_90a.
 //
 // Replaces what the reference delegates to XLA for every dense contraction on the
 // UNet hot path: flax nn.Conv 3x3 / 1x1 (flaxdiff/models/common.py:166-172,
@@ -6,46 +6,39 @@
 // and the QK^T / PV products of nn.dot_product_attention (attention.py:170-174),
 // forward and backward.
 //
-// Design (one CTA per SM, persistent over output tiles, 6 warps):
-//   warp 0      TMA producer: per K-chunk one 128B-swizzled A box (64 channels x
+// Design (one CTA per SM, persistent over 128 x BN output tiles):
+//   last WG     TMA producer (one thread): per K-chunk one 128B-swizzled A box (64 channels x
 //               128 pixels, shifted by the tap offset; out-of-image = zero fill
 //               = SAME padding) and the matching B box, into a ring of stages.
-//   warp 1      MMA issuer: one elected thread issues tcgen05.mma (M=128, N=BN,
-//               K=16, bf16 -> f32) into a double-buffered TMEM accumulator and
-//               tcgen05.commit's the stage back to the producer.
-//   warps 2..5  epilogue: tcgen05.ld the accumulator (one pixel row per thread),
-//               fuse bias + per-image timestep vector + residual, store bf16/f32
-//               (or f32 atomics for the split-K weight gradient).
+//   warpgroups  consumers (one per 128 output columns): wgmma m64 x {64,128} x 16
+//               (bf16 -> f32 registers) over all 128 rows, release each stage once
+//               its MMAs retire, then run the epilogue on their own columns: fuse
+//               bias + per-image timestep vector + residual, store bf16/f32 (or f32
+//               atomics for the split-K weight gradient).
 #include "fdx_tc.cuh"
 #include "fdx_epilogue.cuh"
 #include <stdlib.h>
 
 namespace {
 
-constexpr int kThreads = 192;
 constexpr int kBK = 64;                 // K elements (or K rows) per pipeline stage
 constexpr int kABytes = 128 * kBK * 2;  // 16 KB per stage for A in every mode
 
 template <int BN>
 struct TcCfg {
-  // K chunks (64 deep) per pipeline stage.  At BN = 64 one chunk is only 4 MMAs = 128 tensor
-  // cycles, less than the ~150-200 cycles the single producer / issuer threads spend per stage
-  // on mbarrier try_wait + TMA / MMA issue (ncu: tensor pipe 22 % active), so two chunks share
-  // a stage there.  Not used by the MN-major-A (weight-gradient) mode.
+  static constexpr int kWG = (BN == 256) ? 2 : 1;   // consumer warpgroups; each owns BN / kWG columns
+  static constexpr int kWN = BN / kWG;              // wgmma N
+  static constexpr int kThreads = 128 * (kWG + 1);  // + the producer warpgroup (one thread issues TMA)
+  // K chunks (64 deep) per pipeline stage: at BN = 64 one chunk is only 8 wgmma (two row halves x 4 K
+  // steps), too little work per mbarrier round trip, so two chunks share a stage there.  Not used by the
+  // MN-major-A (weight-gradient) mode.
   static constexpr int kSub = (BN == 64) ? 2 : 1;
-  static constexpr int kStages = (BN == 64) ? 4 : (BN == 128) ? 6 : 4;
+  static constexpr int kStages = (BN == 128) ? 5 : 3;   // as many as fit in 227 KB
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kSub * (kABytes + kBBytes);
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/ +
-                                    16384 /*epilogue staging: 4 warps x 4 KB*/ +
-                                    4096 /*GroupNorm-backward column-sum exchange*/;
-  // Every M=128,K=16 MMA with a K-major A operand costs ~150 cycles whatever N is (tensor pipe 21 %
-  // active at N=64, 43 % at 128, 85 % at 256).  Cycling through kParts independent partial accumulators
-  // (summed by the epilogue) was measured NOT to help (4 / 2 parts at BN = 64 / 128: 26.4 vs 25.9 ms per
-  // step), so the cost is not an accumulator dependency chain; neither is it B's shared-memory traffic
-  // (CTA pairs, below).  The mechanism is kept for experiments.
-  static constexpr int kParts = 1;
-  static constexpr int kTmemCols = 512;     // 2 buffers x kParts x BN columns
+                                    kWG * (16384 /*epilogue staging: 4 warps x 4 KB*/ + kAccXchgBytes);
+  static_assert(kSmemBytes <= 227 * 1024, "tc: shared memory");
 };
 
 struct TcDev {
@@ -68,7 +61,6 @@ struct TcDev {
   int ntp;               // TC_MNMN: number of tap groups = ceil(ntaps / tpp)
   int splits;
   int ntiles;
-  int npairs;            // PAIR kernels: ceil(row tiles / 2) * nblks tile pairs
   // epilogue
   void* out;
   int out_f32, out_atomic;
@@ -106,31 +98,16 @@ __device__ __forceinline__ MnTile decode_mn(const TcDev& p, int tile) {
   return m;
 }
 
-// PAIR = true: the kernel runs as clusters of two CTAs (one TPC).  Each CTA owns one 128-row tile and
-// stages its own A box plus HALF of the B tile's columns; the leader CTA (cluster rank 0) issues
-// tcgen05.mma.cta_group::2 (M = 256) that reads both CTAs' shared memory and writes both CTAs' TMEM.
-// B's TMA writes and UMMA reads per CTA are halved - the engine's measured bound is shared-memory
-// bandwidth.  Barrier topology: every TMA of either CTA completes on the LEADER's full[stage]; the
-// leader's commits multicast to empty[stage] / tfull[acc] of both CTAs; both CTAs' epilogue warps
-// arrive on the leader's tempty[acc].
-template <int BN, int MODE, int EPI, bool PAIR>
-__global__ void __launch_bounds__(kThreads, 1)
+template <int BN, int MODE, int EPI>
+__global__ void __launch_bounds__(TcCfg<BN>::kThreads, 1)
 fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
               const TcDev p) {
   using Cfg = TcCfg<BN>;
-  static_assert(!PAIR || MODE != TC_MNMN, "CTA pairs: K-major A only");
-  constexpr int BNL = PAIR ? BN / 2 : BN;           // B columns staged by THIS CTA
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const bool leader = (rank == 0);
-  // tile loop of this CTA: index t -> (column block nt, row tile mt)
-  const int t_begin = PAIR ? (int)cluster_id_x() : (int)blockIdx.x;
-  const int t_step = PAIR ? (int)cluster_nctaid_x() : (int)gridDim.x;
-  const int t_end = PAIR ? p.npairs : p.ntiles;
   constexpr int S = Cfg::kStages;
+  constexpr int WN = Cfg::kWN;
   constexpr bool A_MN = (MODE == TC_MNMN);
   constexpr bool B_MN = (MODE != TC_KK);
-  constexpr int SUB = A_MN ? 1 : Cfg::kSub;    // K chunks per stage (producer view)
-  constexpr int SUBK = SUB;                     // same, issuer view
+  constexpr int SUB = A_MN ? 1 : Cfg::kSub;    // K chunks per stage
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -138,50 +115,40 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * Cfg::kStageBytes);
   uint64_t* full = bars;            // [S]
   uint64_t* empty = bars + S;       // [S]
-  uint64_t* tfull = bars + 2 * S;   // [2]
-  uint64_t* tempty = bars + 2 * S + 2;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 4);
-  uint8_t* epi_stage = smem + S * Cfg::kStageBytes + 256;   // 16 KB, 128-byte aligned
-  float* epi_xchg = reinterpret_cast<float*>(epi_stage + 16384);   // 4 KB (GN only)
+  uint8_t* epi_stage = smem + S * Cfg::kStageBytes + 256;   // kWG x 16 KB, 128-byte aligned
+  float* acc_xchg = reinterpret_cast<float*>(epi_stage + Cfg::kWG * 16384);   // kWG x kAccXchgBytes
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  constexpr int kProducer = 4 * Cfg::kWG;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducer && lane == 0) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
     for (int i = 0; i < S; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
+      mbar_init(&empty[i], Cfg::kWG);
     }
-    mbar_init(&tfull[0], 1);
-    mbar_init(&tfull[1], 1);
-    mbar_init(&tempty[0], PAIR ? 8 : 4);
-    mbar_init(&tempty[1], PAIR ? 8 : 4);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if constexpr (PAIR) { tmem_alloc_2sm(tmem_slot, Cfg::kTmemCols); tmem_relinquish_2sm(); }
-    else { tmem_alloc(tmem_slot, Cfg::kTmemCols); tmem_relinquish(); }
+  __syncthreads();
+  if constexpr (Cfg::kWG == 2) {
+    if (warp >= kProducer) producer_regs(); else consumer_regs();
   }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // ---- tile decode helpers ------------------------------------------------
   // TC_KK / TC_KMN : tile -> (nt, xb, yb, nb);  nk = ntaps * kchunks
   // TC_MNMN        : tile -> (split, nt, mb, tap); nk = pixel blocks of this split
 
-  if (warp == 0) {
+  if (warp >= kProducer) {
     // =========================== TMA producer ==============================
-    if (lane == 0) {
+    if (warp == kProducer && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = t_begin; tile < t_end; tile += t_step) {
+      for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
         if constexpr (!A_MN) {
           const int nt = tile % p.nblks;
-          const int mt = PAIR ? 2 * (tile / p.nblks) + (int)rank : tile / p.nblks;
+          const int mt = tile / p.nblks;
           const int xb = mt % p.nxb;
           const int yb = (mt / p.nxb) % p.nyb;
           const int nb = mt / (p.nxb * p.nyb);
@@ -193,28 +160,11 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
             mbar_wait(&empty[stage], phase ^ 1);
             uint8_t* sa0 = smem + stage * Cfg::kStageBytes;
             uint8_t* sb0 = sa0 + SUB * kABytes;
-            if constexpr (PAIR) {
-              // the leader posts the bytes of BOTH CTAs; the peer's loads complete on the same barrier
-              if (leader) mbar_arrive_expect_tx(&full[stage], nsub * (2 * kABytes + Cfg::kBBytes));
-            } else {
-              mbar_arrive_expect_tx(&full[stage], nsub * (kABytes + Cfg::kBBytes));
-            }
+            mbar_arrive_expect_tx(&full[stage], nsub * (kABytes + Cfg::kBBytes));
             for (int u = 0; u < nsub; ++u) {
               const int t = (q + u) / p.kchunks, kc = (q + u) % p.kchunks;
               uint8_t* sa = sa0 + u * kABytes;
               uint8_t* sb = sb0 + u * Cfg::kBBytes;
-              const int ncol0 = nt * BN + (int)rank * BNL;      // first B column staged by this CTA
-              if constexpr (PAIR) {
-                tma_load_4d_2sm(sa, &mapA, &full[stage], kc * kBK, x0 + p.tap_dx[t], y0 + p.tap_dy[t], n0);
-                if constexpr (!B_MN) {
-                  tma_load_4d_2sm(sb, &mapB, &full[stage], kc * kBK, ncol0, p.b_batched ? zb1 : p.tap_b[t], zb2);
-                } else {
-#pragma unroll
-                  for (int j = 0; j < BNL / 64; ++j)
-                    tma_load_4d_2sm(sb + j * (kBK * 128), &mapB, &full[stage], ncol0 + j * 64,
-                                    p.tap_b[t] + kc * kBK, zb1, zb2);
-                }
-              } else {
               tma_load_4d(sa, &mapA, &full[stage], kc * kBK, x0 + p.tap_dx[t], y0 + p.tap_dy[t], n0);
               if constexpr (!B_MN) {
                 // B K-major: box (64 k, BN rows); tap selects z1 (or batched z1/z2)
@@ -226,7 +176,6 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
                 for (int j = 0; j < BN / 64; ++j)
                   tma_load_4d(sb + j * (kBK * 128), &mapB, &full[stage], nt * BN + j * 64,
                               p.tap_b[t] + kc * kBK, zb1, zb2);
-              }
               }
             }
             if (++stage == S) { stage = 0; phase ^= 1; }
@@ -266,78 +215,28 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================ MMA issuer ===============================
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = umma_idesc_bf16(PAIR ? 256 : 128, BN, A_MN ? 1 : 0, B_MN ? 1 : 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = t_begin; tile < t_end; tile += t_step) {
-        int nk;
-        if constexpr (!A_MN) {
-          nk = p.ntaps * p.kchunks;
-        } else {
-          const MnTile mt_ = decode_mn(p, tile);
-          nk = mt_.pb1 - mt_.pb0;
-        }
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * Cfg::kParts * BN);
-        for (int q = 0; q < nk; q += SUBK) {
-          const int nsub = (nk - q) < SUBK ? (nk - q) : SUBK;
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa0 = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb0 = sa0 + SUBK * kABytes;
-          for (int u = 0; u < nsub; ++u) {
-            const uint32_t sa = sa0 + u * kABytes;
-            const uint32_t sb = sb0 + u * Cfg::kBBytes;
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k) {
-              // K-major: advance 16 elements (32 B) inside the 128B swizzle row; SBO = 8 rows.
-              // MN-major: advance 16 k-rows (2048 B); LBO = next 64-wide block, SBO = 8 rows.
-              const uint64_t da = A_MN ? umma_desc_sw128(sa + k * 2048, kBK * 128, 1024)
-                                       : umma_desc_sw128(sa + k * 32, 16, 1024);
-              const uint64_t db = B_MN ? umma_desc_sw128(sb + k * 2048, kBK * 128, 1024)
-                                       : umma_desc_sw128(sb + k * 32, 16, 1024);
-              // MMA number (q+u)*4 + k of this tile goes to partial accumulator (number % kParts);
-              // the first MMA of every partial overwrites it
-              const int mi = (q + u) * (kBK / 16) + k;
-              const uint32_t dpart = d_tmem + (uint32_t)((mi % Cfg::kParts) * BN);
-              const uint32_t accf = mi >= Cfg::kParts ? 1u : 0u;
-              if constexpr (PAIR) umma_f16_2sm(dpart, da, db, idesc, accf);
-              else umma_f16(dpart, da, db, idesc, accf);
-            }
-          }
-          // frees the smem stage (of both CTAs of a pair) when these MMAs retire
-          if constexpr (PAIR) umma_commit_2sm(&empty[stage]); else umma_commit(&empty[stage]);
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-        if (nk == 0) {
-          // nothing accumulated for this tile: epilogue must not read garbage
-        }
-        if constexpr (PAIR) umma_commit_2sm(&tfull[acc]); else umma_commit(&tfull[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // ============================= epilogue =================================
-    const int q = warp & 3;              // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;       // accumulator row owned by this thread
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ========================= consumer warpgroups ==========================
+    const int wg = warp >> 2;            // columns [wg * WN, wg * WN + WN) of the tile
+    const int q = warp & 3;
+    const int row = q * 32 + lane;       // accumulator row this thread stores in the epilogue
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    float* xs = acc_xchg + wg * (kAccXchgBytes / 4);
+    const int xbar = 1 + wg;             // named barrier of this warpgroup's accumulator exchange
+    WgAcc<WN> acc;
+    int stage = 0;
+    uint32_t phase = 0;
     int gn_par = 0;
-    for (int tile = t_begin; tile < t_end; tile += t_step) {
+    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
       int nt;
       bool valid;
       long long obase, rbase = 0;
       int img = 0;
       bool has_acc = true;
+      int nk;
       if constexpr (!A_MN) {
         nt = tile % p.nblks;
-        const int mt = PAIR ? 2 * (tile / p.nblks) + (int)rank : tile / p.nblks;
+        const int mt = tile / p.nblks;
         const int xb = mt % p.nxb;
         const int yb = (mt / p.nxb) % p.nyb;
         const int nb = mt / (p.nxb * p.nyb);
@@ -346,13 +245,14 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         valid = (x < p.W) && (y < p.H) && (n < p.N);
         img = n;
         obase = (long long)n * p.os_n + (long long)y * p.os_y + (long long)x * p.os_x;
+        nk = p.ntaps * p.kchunks;
         if (p.res) {
           rbase = (long long)n * p.rs_n + (long long)y * p.rs_y + (long long)x * p.rs_x;
-          // the side input of this row: request all of its lines now (L2 prefetch), before the accumulator
-          // wait - the epilogue's own register prefetch runs only one 64-column chunk ahead
+          // the side input of this row: request all of its lines now (L2 prefetch), before the main loop -
+          // the epilogue's own register prefetch runs only one 64-column chunk ahead
           if (valid && !p.out_f32 && !p.out_atomic) {
-            const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(p.res) + rbase + nt * BN;
-            const int ncol = min(BN, p.Ncols - nt * BN);
+            const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(p.res) + rbase + nt * BN + wg * WN;
+            const int ncol = min(WN, p.Ncols - nt * BN - wg * WN);
             for (int c = 0; c < ncol; c += 64) asm volatile("prefetch.global.L2 [%0];" ::"l"(a + c));
           }
         }
@@ -366,37 +266,58 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         obase = (long long)p.tap_b[valid ? tap : 0] * p.os_tap + (long long)m * p.os_m;
         if (p.mn_batched)
           obase += (long long)(mt_.bz % p.nyb) * p.os_y + (long long)(mt_.bz / p.nyb) * p.os_n;
-        has_acc = (mt_.pb1 - mt_.pb0) > 0;
+        nk = mt_.pb1 - mt_.pb0;
+        has_acc = nk > 0;
       }
-      auto wait_acc = [&]() {
-        mbar_wait(&tfull[acc], acc_phase);
-        tc_fence_after();
+      // main loop: the MMAs of stage s are retired (and s released to the producer) while those of s+1 run
+      auto mainloop = [&]() {
+        acc.zero();
+        int prev = -1;
+        for (int qk = 0; qk < nk; qk += SUB) {
+          const int nsub = (nk - qk) < SUB ? (nk - qk) : SUB;
+          mbar_wait(&full[stage], phase);
+          wgmma_fence();
+          const uint32_t sa0 = smem_u32(smem + stage * Cfg::kStageBytes);
+          const uint32_t sb0 = sa0 + SUB * kABytes + wg * WN * 128;   // this warpgroup's B columns
+          for (int u = 0; u < nsub; ++u) {
+            const uint32_t sa = sa0 + u * kABytes;
+            const uint32_t sb = sb0 + u * Cfg::kBBytes;
+#pragma unroll
+            for (int k = 0; k < kBK / 16; ++k) {
+              // K-major: advance 16 elements (32 B) inside the 128B swizzle row; SBO = 8 rows.
+              // MN-major: advance 16 k-rows (2048 B); LBO = next 64-wide block, SBO = 8 rows.
+              // Rows 64..127 of A start 8 KB further in both layouts.
+              const uint32_t ao = A_MN ? sa + k * 2048 : sa + k * 32;
+              const uint64_t da0 = A_MN ? gmma_desc_sw128(ao, kBK * 128, 1024) : gmma_desc_sw128(ao, 16, 1024);
+              const uint64_t da1 = A_MN ? gmma_desc_sw128(ao + 8192, kBK * 128, 1024)
+                                        : gmma_desc_sw128(ao + 8192, 16, 1024);
+              const uint64_t db = B_MN ? gmma_desc_sw128(sb + k * 2048, kBK * 128, 1024)
+                                       : gmma_desc_sw128(sb + k * 32, 16, 1024);
+              acc.template mma<A_MN ? 1 : 0, B_MN ? 1 : 0>(da0, da1, db);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && wg_leader) mbar_arrive(&empty[prev]);
+          prev = stage;
+          if (++stage == S) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        if (prev >= 0 && wg_leader) mbar_arrive(&empty[prev]);
       };
-      const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * Cfg::kParts * BN);
       if (!A_MN && !p.out_f32 && !p.out_atomic) {
         // bf16 output: stage through shared memory so global stores / side-input loads are coalesced
         EpiArgs ea{p.out, p.bias, p.rowvec, p.res, p.Ncols, p.alpha, p.gn_ab, p.gn_ws, p.N, p.ws_ld};
-        epilogue_bf16_coalesced<BN, EPI, Cfg::kParts>(ea, epi_stage + q * 4096, t_addr, lane, nt * BN, valid && has_acc,
-                                         obase, rbase, img, wait_acc, q, epi_xchg, &gn_par,
-                                         EPI != EPI_PLAIN ? tile % p.gn_slots : 0);
+        epilogue_bf16_coalesced<WN, EPI>(ea, epi_stage + (wg * 4 + q) * 4096, acc, xs, xbar, lane,
+                                         nt * BN + wg * WN, valid && has_acc, obase, rbase, img, mainloop,
+                                         &gn_par, EPI != EPI_PLAIN ? tile % p.gn_slots : 0);
       } else {
-      wait_acc();
+      mainloop();
 #pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_addr + c0, v);
-        tmem_ld_wait();
+      for (int c0 = 0; c0 < WN; c0 += 32) {
         float f[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-#pragma unroll
-        for (int pp = 1; pp < Cfg::kParts; ++pp) {        // sum the partial accumulators
-          tmem_ld_32x32(t_addr + pp * BN + c0, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] += __uint_as_float(v[j]);
-        }
-        const int col0 = nt * BN + c0;
+        acc.row32(xs, xbar, c0, f);
+        const int col0 = nt * BN + wg * WN + c0;
         if (valid && has_acc && col0 < p.Ncols) {
 #pragma unroll
           for (int j = 0; j < 32; ++j) f[j] *= p.alpha;
@@ -446,21 +367,7 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         }
       }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_cluster(&tempty[acc], 0); else mbar_arrive(&tempty[acc]);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();   // the leader's MMAs read the peer's smem
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
-    else tmem_dealloc(tmem_base, Cfg::kTmemCols);
   }
 }
 
@@ -469,48 +376,16 @@ int launch_cfg(const CUtensorMap& mA, const CUtensorMap& mB, const TcDev& d, cud
   using Cfg = TcCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    FDX_CUDA(cudaFuncSetAttribute(fdx_tc_kernel<BN, MODE, EPI, false>,
+    FDX_CUDA(cudaFuncSetAttribute(fdx_tc_kernel<BN, MODE, EPI>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
   }
   int grid = fdx_num_sms();
   if (grid <= 0) return FDX_ERR_NO_DEVICE;
   if (d.ntiles < grid) grid = d.ntiles;
-  fdx_tc_kernel<BN, MODE, EPI, false><<<grid, kThreads, Cfg::kSmemBytes, stream>>>(mA, mB, d);
+  fdx_tc_kernel<BN, MODE, EPI><<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mA, mB, d);
   fdx_note_kernel(FDX_KERNEL_TC);
   FDX_LAUNCH_CHECK();
-  return FDX_OK;
-}
-
-// CTA-pair launch: clusters of two CTAs, an even grid
-template <int BN, int MODE>
-int launch_pair(const CUtensorMap& mA, const CUtensorMap& mB, const TcDev& d, cudaStream_t stream) {
-  using Cfg = TcCfg<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    FDX_CUDA(cudaFuncSetAttribute(fdx_tc_kernel<BN, MODE, EPI_PLAIN, true>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  int sms = fdx_num_sms();
-  if (sms <= 0) return FDX_ERR_NO_DEVICE;
-  int clusters = sms / 2;
-  if (d.npairs < clusters) clusters = d.npairs;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  FDX_CUDA(cudaLaunchKernelEx(&cfg, fdx_tc_kernel<BN, MODE, EPI_PLAIN, true>, mA, mB, d));
-  fdx_note_kernel(FDX_KERNEL_TC);
-  fdx_count_launch();
   return FDX_OK;
 }
 
@@ -522,9 +397,6 @@ int launch_gn(const CUtensorMap& mA, const CUtensorMap& mB, const TcDev& d, cuda
   if constexpr (MODE == TC_KMN) {
     if (d.gn_ws && !d.gn_ab) return launch_cfg<BN, MODE, EPI_COLSTATS>(mA, mB, d, stream);
   }
-  if constexpr (MODE != TC_MNMN && BN >= 128 && !(MODE == TC_KMN && BN == 192)) {
-    if (d.npairs > 0) return launch_pair<BN, MODE>(mA, mB, d, stream);
-  }
   return launch_cfg<BN, MODE, EPI_PLAIN>(mA, mB, d, stream);
 }
 
@@ -534,7 +406,6 @@ int launch_mode(int BN, const CUtensorMap& mA, const CUtensorMap& mB, const TcDe
   switch (BN) {
     case 64: return launch_gn<64, MODE>(mA, mB, d, stream);
     case 128: return launch_gn<128, MODE>(mA, mB, d, stream);
-    case 192: return launch_gn<192, MODE>(mA, mB, d, stream);
     case 256: return launch_gn<256, MODE>(mA, mB, d, stream);
   }
   fdx_set_error("tc: unsupported BN %d", BN);
@@ -596,8 +467,8 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
   int BN = 64;
   {
     long long best = -1;
-    const int cands[4] = {256, 192, 128, 64};
-    for (int i = 0; i < 4; ++i) {
+    const int cands[3] = {256, 128, 64};
+    for (int i = 0; i < 3; ++i) {
       const int bn = cands[i];
       const long long nt = (L.Ncols + bn - 1) / bn;
       const long long cost = nt * (bn + 64);
@@ -630,28 +501,15 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
   d.nnb = (L.N + TN - 1) / TN;
   const long long pix_blocks = (long long)d.nxb * d.nyb * d.nnb;
 
-  // halo-sharing variant: fewer TMA writes, but measured slower than the generic kernel on B200
-  // (both are shared-memory-bandwidth bound); kept as an opt-in experiment.
-  if (L.mode != TC_MNMN && !L.gn_ws && getenv("FDX_CONV3")) {
-    const int r3 = fdx_conv3_launch(L, BN, stream);
-    if (r3 != FDX_ERR_UNSUPPORTED) return r3;
-  }
   if (L.mode != TC_MNMN) {
-    // Round 1 narrowed the column tile until the launch had two waves of tiles.  But a K = 16 MMA of this
-    // (pixels-as-M) engine costs ~150 cycles whatever its N (DESIGN 3.1), so a tile's duration does not shrink
-    // with BN and more, narrower tiles only add rounds: 8x8 images (128 pixel tiles at B = 256) ran 256 -> 256 at
-    // BN = 64 in four rounds instead of one (47 us; 407 TF/s).  FDX_TC_BN_V1=1 restores the old rule.
+    // Round 1 narrowed the column tile until the launch had two waves of tiles; narrower tiles re-read the A
+    // operand once per column block and add rounds.  FDX_TC_BN_V1=1 restores the old rule.
     static const bool bn_v1 = getenv("FDX_TC_BN_V1") != nullptr;
     while (bn_v1 && BN > 64 && pix_blocks * ((L.Ncols + BN - 1) / BN) < 2LL * fdx_num_sms())
-      BN = (BN == 192) ? 64 : BN / 2;
+      BN /= 2;
     d.nblks = (L.Ncols + BN - 1) / BN;
     d.kchunks = (L.K + kBK - 1) / kBK;
     d.ntiles = (int)(pix_blocks * d.nblks);
-    // CTA pairs (cta_group::2): plain bf16 epilogue, BN >= 128 (MN-major B needs whole 64-column blocks
-    // per CTA: not BN = 192); opt-in while it is being measured
-    d.npairs = 0;
-    if (getenv("FDX_PAIR") && !L.gn_ws && BN >= 128 && !(L.mode == TC_KMN && BN == 192) && pix_blocks >= 2)
-      d.npairs = (int)(((pix_blocks + 1) / 2) * d.nblks);
     d.splits = 1;
     d.mblks = 1;
     d.tpp = 1;
@@ -708,7 +566,7 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
     uint32_t box[4];
     uint32_t est[4] = {1, 1, 1, 1};
     if (L.mode == TC_KK) {
-      box[0] = 64; box[1] = (uint32_t)(d.npairs > 0 ? BN / 2 : BN); box[2] = 1; box[3] = 1;
+      box[0] = 64; box[1] = (uint32_t)BN; box[2] = 1; box[3] = 1;
     } else if (L.mode == TC_KMN) {
       box[0] = 64; box[1] = 64; box[2] = 1; box[3] = 1;
     } else {

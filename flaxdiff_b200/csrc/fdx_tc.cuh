@@ -1,4 +1,4 @@
-// fdx_tc.cuh -- launch descriptor of the tcgen05 "tap-GEMM" engine (fdx_tc.cu).
+// fdx_tc.cuh -- launch descriptor of the wgmma "tap-GEMM" engine (fdx_tc.cu).
 //
 // One persistent, warp-specialised kernel computes
 //     D[m, n] = alpha * sum_{tap t} sum_{k} A_t[m, k] * B_t[n, k]   (+ epilogue)
@@ -75,6 +75,3 @@ int fdx_wgrad9_launch(const fdx_act* x, const fdx_act* dy, float* dw, cudaStream
 // Transposed formulation (weights as A, 256 pixels as N) for Ncols = 64 / 128 (fdx_tct.cu);
 // FDX_ERR_UNSUPPORTED = geometry not covered.
 int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream);
-
-// Halo-sharing 3x3 stride-1 kernel (fdx_conv3.cu); FDX_ERR_UNSUPPORTED = geometry not covered.
-int fdx_conv3_launch(const TcLaunch& L, int BN, cudaStream_t stream);

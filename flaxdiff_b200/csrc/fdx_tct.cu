@@ -1,32 +1,29 @@
 // fdx_tct.cu -- the TRANSPOSED formulation of the 3x3 convolution (forward and data gradient) for
 // layers with few output channels (Cout = 64 / 128 forward, Cin = 64 / 128 in the data gradient).
 //
-// fdx_tc.cu puts the pixels in the M dimension, so a Cout = 64 layer can only issue 128 x 64 x 16 MMAs, and
-// every M = 128, K = 16 MMA costs ~150 cycles whatever N is (DESIGN.md 3.1): the tensor pipe is 21 % active
-// at N = 64 and 43 % at N = 128.  Here the roles are swapped,
+// fdx_tc.cu puts the pixels in the M dimension, so a Cout = 64 layer can only issue N = 64 MMAs, whose
+// shared-memory operand traffic per FLOP is twice that of N = 128.  Here the roles are swapped,
 //     D^T[co, px] = sum_tap sum_ci  W_tap[ci, co]  *  X[px + tap, ci]
 // A = the weight tile (M = 64 or 128 output channels x 64 k; MN-major straight from HWIO in the forward,
 // K-major from the (Cout, Cin, tap) view in the data gradient), B = 256 pixels (two 16 x 8 TMA boxes of
-// 64 channels, K-major, N = 256), so every MMA is M x 256 x 16.  The accumulator is D^T: TMEM lane = output
-// channel, column = pixel; the epilogue warps therefore own whole channels (bias and the fused per-channel
-// GroupNorm sums are per-thread scalars) and write 64-byte channel runs per pixel.
+// 64 channels, K-major).  The accumulator is D^T: row = output channel, column = pixel.  Two consumer
+// warpgroups each own 128 of the pixel columns and issue m64 n128 k16 wgmma (two per K step at M = 128).
 //
-// M = 64 (64 output channels): an M = 64 accumulator occupies lanes 0-15 of every TMEM sub-partition only,
-// so TWO pixel halves (2 x 256 pixels, 16 wide x 32 tall) are interleaved into the same 256 columns - half
-// 0 in lanes 0-15, half 1 in lanes 16-31 (TMEM lane offset 16 of the MMA's D address) - and the epilogue
-// warps again work with all 32 lanes.  K steps alternate between the halves; the 8 KB weight tile is
-// simply fetched for both.
+// M = 64 (64 output channels): TWO pixel halves (2 x 256 pixels, 16 wide x 32 tall) share a tile - half 0
+// in accumulator rows 0-63, half 1 in rows 64-127 - so a warpgroup again holds a 128-row accumulator.  K
+// steps alternate between the halves; the 8 KB weight tile is simply fetched for both.
 //
-// Same barrier topology as fdx_tc.cu: warp 0 = TMA producer, warp 1 = MMA issuer, warps 2..5 = epilogue,
-// double-buffered 2 x 256-column TMEM accumulator.  Geometry: stride 1, W and H multiples of 16.
+// Warps 8..11 = producer (one thread issues TMA), warps 0..7 = the two consumer warpgroups (main loop, then epilogue on their own
+// columns).  Geometry: stride 1, W and H multiples of 16.
 #include "fdx_tc.cuh"
 #include "fdx_epilogue.cuh"
 #include <stdlib.h>
 
 namespace {
 
-constexpr int kEpiWarps = 8;                 // two groups of four: the tile's pixel columns are split between them
-constexpr int kThreads = 64 + 32 * kEpiWarps;
+constexpr int kEpiWarps = 8;                 // two warpgroups: the tile's pixel columns are split between them
+constexpr int kThreads = 32 * kEpiWarps + 128;  // + the producer warpgroup (one thread issues TMA)
+constexpr int kLdT = 128 + 4;                // row of the transposed exchange tile [32 px][128 channel rows]
 constexpr int kPixBytes = 2 * 128 * 128;     // two boxes of 128 pixels x 64 channels bf16
 
 struct TctDev {
@@ -45,17 +42,15 @@ struct TctDev {
   const float* gn_ab;      // GNB kernels: [N][2][Ncols] GroupNorm coefficients a, b of the tensor `res` (= x)
 };
 
-// HALO = true (round 2, 3x3 stride-1 only): the 64- and 128-output-channel layers were L2 -> shared-memory
-// bandwidth bound, not MMA bound: every (tap, K chunk) re-loaded its 256 pixels, 40 KB of TMA per 2.1 MFLOP at
-// M = 64 = 52 FLOP per byte, and the L2 delivers ~15 TB/s (780 TF/s measured on 64 -> 64).  Here ONE tall box of
+// HALO = true (3x3 stride-1 only): with per-tap loads every (tap, K chunk) re-loads its 256 pixels, 40 KB of TMA
+// per 2.1 MFLOP at M = 64 = 52 FLOP per byte, so the layers are L2 -> shared-memory bandwidth bound.  ONE tall box of
 // 16 x 18 pixels (rows y0-1 .. y0+16) is loaded per (kx, K chunk); the three ky taps are 2048-byte row offsets
 // into it (swizzle-aligned views, exactly as in the nine-tap weight gradient), so a stage carries three weight
 // tiles + 36 KB of pixels and feeds twelve MMAs: 96 -> 36 KB of pixel traffic per three taps.
 // GNB = true (data gradient only): the first pass of the GroupNorm(+SiLU) backward in the epilogue - with x = the
 // GroupNorm input (side input `res`) and z = a_c x + b_c the kernel stores dz = dy * silu'(z) instead of dy and
 // accumulates S0 = sum dz, S1 = sum dz * x per (image, channel) into the column-sum workspace, exactly as the
-// pixels-as-M engine's EPI_GN_BWD (fdx_epilogue.cuh).  There the silu' arithmetic sat in four epilogue warps and
-// lost to the separate statistics pass; with eight epilogue warps it fits under the tile's MMA time.
+// pixels-as-M engine's EPI_GN_BWD (fdx_epilogue.cuh).
 template <int MT, bool A_MN, bool HALO, bool GNB>
 __global__ void __launch_bounds__(kThreads, 1)
 fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapX,
@@ -73,28 +68,20 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * kStageBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + S;
-  uint64_t* tfull = bars + 2 * S;
-  uint64_t* tempty = bars + 2 * S + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 4);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == kEpiWarps && lane == 0) {
     tma_prefetch_desc(&mapW);
     tma_prefetch_desc(&mapX);
-    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(&tfull[0], 1); mbar_init(&tfull[1], 1);
-    mbar_init(&tempty[0], kEpiWarps); mbar_init(&tempty[1], kEpiWarps);
+    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (warp >= kEpiWarps) producer_regs(); else consumer_regs();
   const int nk = p.ntaps * p.kchunks;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= kEpiWarps) {
+    if (warp == kEpiWarps && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
         const int cb = tile % p.cblks;
@@ -150,89 +137,31 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(MT, 256, A_MN ? 1 : 0, 0);
-      int stage = 0, acc = 0; uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 256);
-        const int yb_i = ((tile / p.cblks) / p.nxb) % p.nyb;
-        if constexpr (HALO) {
-          for (int qq = 0; qq < 3 * p.kchunks * NH; ++qq) {
-            if (IL && yb_i * TH + 16 * (qq % NH) >= p.H) continue;   // same skip as the producer
-            const uint32_t dh = d_tmem + ((uint32_t)((qq % NH) * 16) << 16);
-            mbar_wait(&full[stage], phase);
-            tc_fence_after();
-            const uint32_t sw = smem_u32(smem + stage * kStageBytes);
-            const uint32_t sx = sw + 3 * kWBytes;
-#pragma unroll
-            for (int ky = 0; ky < 3; ++ky) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint64_t da = A_MN ? umma_desc_sw128(sw + ky * kWBytes + k * 2048, 8192, 1024)
-                                         : umma_desc_sw128(sw + ky * kWBytes + k * 32, 16, 1024);
-                const uint64_t db = umma_desc_sw128(sx + ky * 2048 + k * 32, 16, 1024);   // rows ky .. ky+15 of the box
-                umma_f16(dh, da, db, idesc, (qq >= NH || ky != 0 || k != 0) ? 1u : 0u);
-              }
-            }
-            umma_commit(&empty[stage]);
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
-        } else
-        for (int qq = 0; qq < nk * NH; ++qq) {
-          const int q = qq / NH;
-          if (IL && yb_i * TH + 16 * (qq % NH) >= p.H) continue;     // same skip as the producer
-          const uint32_t dh = d_tmem + ((uint32_t)((qq % NH) * 16) << 16);   // half 1 -> TMEM lanes 16..31
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sw = smem_u32(smem + stage * kStageBytes);
-          const uint32_t sx = sw + kWBytes;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = A_MN ? umma_desc_sw128(sw + k * 2048, 8192, 1024)
-                                     : umma_desc_sw128(sw + k * 32, 16, 1024);
-            const uint64_t db = umma_desc_sw128(sx + k * 32, 16, 1024);
-            umma_f16(dh, da, db, idesc, (q | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // ============ epilogue ===============================================================
-    // TMEM gives this thread ONE output channel (lane) and 32 pixels (columns) per load.  The f32 values
-    // (+ bias + timestep row) are transposed through a per-warp shared-memory tile [32 px][CW channels]
-    // (CW = channels per warp: 32 at M=128, 16 at M=64) and leave as 16-byte channel pieces: lane ->
-    // (pixel l / PPX + k * (32 / PPX), piece l % PPX).  A lane always owns the same 8 channels, so the
-    // fused GroupNorm sums are per-lane registers, reduced once per tile.
-    // Eight epilogue warps (round 2): the 64- and 128-channel layers were EPILOGUE bound (64 -> 64 at 64x64:
-    // 110 us against 67 us of MMA time; per 32-pixel chunk one tcgen05.ld -> staging -> 16-byte pieces chain per
-    // warp with nothing to overlap it).  Warps 2..5 take the pixel columns 0..127 of the accumulator, warps 6..9
-    // the columns 128..255 - same TMEM lanes (warp % 4), own staging tile, own GroupNorm partial sums.
+    // ============ consumers: main loop, then epilogue ====================================================
+    // The f32 values of a 32-pixel chunk are transposed through the warpgroup's shared-memory tile
+    // [32 px][128 channel rows] and leave as 16-byte channel pieces: lane -> (pixel l / PPX + k * (32 / PPX),
+    // piece l % PPX).  A lane always owns the same 8 channels, so bias, timestep row and the fused GroupNorm
+    // sums are per-lane registers, reduced once per tile.
     const int q = warp & 3;
-    const int ew = warp - 2;                             // 0 .. kEpiWarps-1: staging tile of this warp
-    const int c_begin = (ew >> 2) * (256 / (kEpiWarps / 4)), c_end = c_begin + 256 / (kEpiWarps / 4);
-    constexpr int CW = 32;                               // staging slots per pixel column = lanes of the warp:
-                                                         // M=128: 32 channels; M=64: 16 channels x 2 halves
+    const int wg = warp >> 2;
+    const int ew = warp;                                 // 0 .. kEpiWarps-1
+    const int c_begin = wg * 128, c_end = c_begin + 128;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const int xbar = 1 + wg;
     constexpr int PPX = 4;                               // 16-byte pieces per staged pixel column
     constexpr int CPW = IL ? 16 : 32;                    // channels owned by one warp
-    const int crow = IL ? q * 16 + (lane & 15) : q * 32 + lane;
-    constexpr int RS = CW + 4;                           // padded row (floats): conflict-free 16-byte reads
-    float* stg = reinterpret_cast<float*>(smem + S * kStageBytes + 256) + ew * (32 * RS);  // [32 px][RS] f32
+    float* xsT = reinterpret_cast<float*>(smem + S * kStageBytes + 256) + wg * (32 * kLdT);
     const int piece = lane % PPX, prow = lane / PPX;     // read phase: this lane's piece and first pixel
-    int acc = 0; uint32_t acc_phase = 0;
+    // accumulator row of this lane's first channel: M = 128: channel; M = 64: half * 64 + channel
+    const int srow = IL ? (piece >> 1) * 64 + q * 16 + (piece & 1) * 8 : q * 32 + piece * 8;
     __nv_bfloat16* outp = static_cast<__nv_bfloat16*>(p.out);
     const __nv_bfloat16* resp = static_cast<const __nv_bfloat16*>(p.res);
+    WgAcc<128> acc;
+    int stage = 0; uint32_t phase = 0;
     // Side input (residual / accumulate source): the register prefetch below runs one 32-pixel chunk ahead,
-    // a few hundred cycles - enough for an L2 hit, not for HBM (measured: 64 -> 64 at 64x64 took 190 us with a
-    // residual against 110 us without; every chunk waited a full DRAM round trip).  So the 128 epilogue threads
-    // pull the side input of the NEXT tile into L2 while they work on the current one (one line per pixel and
-    // 64 channels; <= 64 KB per CTA in flight).
+    // enough for an L2 hit, not for HBM.  So the consumer threads pull the side input of the NEXT tile into L2
+    // while they work on the current one (one line per pixel and 64 channels; <= 64 KB per CTA in flight).
     auto prefetch_res = [&](int t) {
       if (resp == nullptr || t >= p.ntiles) return;
       const int cb_ = t % p.cblks, mt_ = t / p.cblks;
@@ -252,21 +181,24 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
       const int cb = tile % p.cblks;
       const int mt = tile / p.cblks;
       const int xb = mt % p.nxb, yb = (mt / p.nxb) % p.nyb, nb = mt / (p.nxb * p.nyb);
-      const int co = cb * MT + crow;                      // write phase: this thread's channel
       const int cw0 = cb * MT + q * CPW;                  // first channel of this warp
-      const bool live = co < p.Ncols;
       // read phase: piece -> (pixel half, 8-channel group); half 1 lies 16 pixel rows below half 0
       const int yh = yb * TH + (IL ? 16 * (piece >> 1) : 0);
       const long long obase = (long long)nb * p.os_n + (long long)yh * p.os_y + (long long)(xb * 16) * p.os_x;
       const long long rbase = (long long)nb * p.rs_n + (long long)yh * p.rs_y + (long long)(xb * 16) * p.rs_x;
-      float add = 0.f;
-      if (live) {
-        if (p.bias) add += __ldg(p.bias + co);
-        if (p.rowvec) add += __ldg(p.rowvec + (long long)nb * p.Ncols + co);
-      }
-      // residual pieces are requested one 32-pixel chunk ahead (the first before the accumulator wait)
+      // residual pieces are requested one 32-pixel chunk ahead (the first before the main loop)
       const int ch = cw0 + (IL ? (piece & 1) : piece) * 8;   // read phase: this lane's first channel
       const bool ch_ok = ch < p.Ncols && yh < p.H;           // (H % 32 == 16: the last tile has no half 1)
+      float add[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) add[i] = 0.f;
+      if (ch_ok) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          if (p.bias) add[i] += __ldg(p.bias + ch + i);
+          if (p.rowvec) add[i] += __ldg(p.rowvec + (long long)nb * p.Ncols + ch + i);
+        }
+      }
       float ga[8], gb[8];
       if constexpr (GNB) {
 #pragma unroll
@@ -291,30 +223,106 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
       };
       uint4 rcur[PPX], rnxt[PPX];
       load_res(c_begin, rcur);
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 256);
+      // ---- main loop: this warpgroup's 128 pixel columns ----
+      const int yb_i = yb;
+      acc.zero();
+      int prev = -1;
+      auto release = [&]() {
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && wg_leader) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      };
+      if constexpr (HALO) {
+        for (int qq = 0; qq < 3 * p.kchunks * NH; ++qq) {
+          if (IL && yb_i * TH + 16 * (qq % NH) >= p.H) continue;   // same skip as the producer
+          const int hh = qq % NH;
+          mbar_wait(&full[stage], phase);
+          wgmma_fence();
+          const uint32_t sw = smem_u32(smem + stage * kStageBytes);
+          const uint32_t sx = sw + 3 * kWBytes + wg * 16384;     // pixel rows 8 wg .. 8 wg + 7 of the view
+#pragma unroll
+          for (int ky = 0; ky < 3; ++ky) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const uint32_t aw = A_MN ? sw + ky * kWBytes + k * 2048 : sw + ky * kWBytes + k * 32;
+              const uint64_t db = gmma_desc_sw128(sx + ky * 2048 + k * 32, 16, 1024);   // rows ky .. ky+15 of the box
+              if constexpr (IL) {
+                acc.mma_half<A_MN ? 1 : 0, 0>(hh, A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024), db);
+              } else {
+                acc.mma<A_MN ? 1 : 0, 0>(A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024),
+                                         A_MN ? gmma_desc_sw128(aw + 8192, 8192, 1024)
+                                              : gmma_desc_sw128(aw + 8192, 16, 1024),
+                                         db);
+              }
+            }
+          }
+          release();
+        }
+      } else
+      for (int qq = 0; qq < nk * NH; ++qq) {
+        if (IL && yb_i * TH + 16 * (qq % NH) >= p.H) continue;     // same skip as the producer
+        const int hh = qq % NH;
+        mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        const uint32_t sw = smem_u32(smem + stage * kStageBytes);
+        const uint32_t sx = sw + kWBytes + wg * 16384;             // this warpgroup's 128-pixel box
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint32_t aw = A_MN ? sw + k * 2048 : sw + k * 32;
+          const uint64_t db = gmma_desc_sw128(sx + k * 32, 16, 1024);
+          if constexpr (IL) {
+            acc.mma_half<A_MN ? 1 : 0, 0>(hh, A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024), db);
+          } else {
+            acc.mma<A_MN ? 1 : 0, 0>(A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024),
+                                     A_MN ? gmma_desc_sw128(aw + 8192, 8192, 1024) : gmma_desc_sw128(aw + 8192, 16, 1024),
+                                     db);
+          }
+        }
+        release();
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty[prev]);
+
       float s0[8], s1[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) { s0[i] = 0.f; s1[i] = 0.f; }
 #pragma unroll 1
       for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_addr + c0, v);
-        tmem_ld_wait();
-        // ---- write phase: stg[px j][channel (lane within the warp's CW)] ----
+        // ---- write phase: accumulator fragments of columns c0 .. c0+31 -> xsT[px][channel row] ----
+        named_bar_sync(xbar, 128);                       // the previous chunk's reads are done
+        {
+          const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+          const int cc = (c0 - c_begin) >> 5;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) stg[j * RS + lane] = __uint_as_float(v[j]) * p.alpha + add;
-        __syncwarp();
+          for (int ci = 0; ci < 4; ++ci) {
+            if (ci != cc) continue;                      // compile-time register indices, run-time chunk
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const int r = h * 64 + w * 16 + (l >> 2), n = jj * 8 + 2 * (l & 3);
+                const float* d = &acc.d[h][(ci * 4 + jj) * 4];
+                xsT[n * kLdT + r] = d[0];
+                xsT[(n + 1) * kLdT + r] = d[1];
+                xsT[n * kLdT + r + 8] = d[2];
+                xsT[(n + 1) * kLdT + r + 8] = d[3];
+              }
+          }
+        }
+        named_bar_sync(xbar, 128);
         load_res(c0 + 32, rnxt);
         // ---- read phase: 16-byte channel pieces; columns c0 .. c0+31 = pixel rows c0/16, c0/16 + 1 ----
 #pragma unroll
         for (int k = 0; k < PPX; ++k) {
           const int j = prow + k * (32 / PPX);            // pixel (column) within the chunk
           const int ty = c0 / 16 + (j >> 4), tx = j & 15;
-          const float4 a = *reinterpret_cast<const float4*>(stg + j * RS + piece * 8);
-          const float4 b = *reinterpret_cast<const float4*>(stg + j * RS + piece * 8 + 4);
+          const float4 a = *reinterpret_cast<const float4*>(xsT + j * kLdT + srow);
+          const float4 b = *reinterpret_cast<const float4*>(xsT + j * kLdT + srow + 4);
           float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+          for (int i = 0; i < 8; ++i) f[i] = f[i] * p.alpha + add[i];
           if (ch_ok) {
             float xv[8];
             if (resp) {
@@ -345,7 +353,6 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
             }
           }
         }
-        __syncwarp();
 #pragma unroll
         for (int k = 0; k < PPX; ++k) rcur[k] = rnxt[k];
       }
@@ -365,22 +372,15 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
           for (int i = 0; i < 8; ++i) { atomicAdd(w + i, s0[i]); atomicAdd(w + p.cs_ld + i, s1[i]); }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 template <int MT, bool A_MN, bool HALO, bool GNB = false>
 int launch_tct(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& d, cudaStream_t stream) {
   constexpr int S = HALO ? ((MT == 128) ? 2 : 3) : ((MT == 128) ? 3 : 4);
   constexpr int stage = HALO ? (3 * MT * 128 + 18 * 16 * 128) : (MT * 128 + kPixBytes);
-  constexpr int smem = S * stage + 1024 + 256 + kEpiWarps * 32 * 36 * 4 /* epilogue transpose tiles */;
+  constexpr int smem = S * stage + 1024 + 256 + 2 * 32 * kLdT * 4 /* epilogue transpose tiles */;
   static_assert(smem <= 227 * 1024, "tct: shared memory");
   static bool attr_set = false;
   if (!attr_set) {

@@ -96,7 +96,7 @@ int fdx_upconv3x3_pack(const float* w_hwio, int cin, int cout, void* weff_bf16, 
   FDX_REQUIRE(w_hwio && weff_bf16 && cin > 0 && cout > 0, "upconv3x3_pack: bad arguments");
   const long long slab = (long long)cin * cout;
   long long grid = (slab + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > fdx_num_sms() * 8) grid = fdx_num_sms() * 8;
   upconv_pack_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(w_hwio, slab, (__nv_bfloat16*)weff_bf16);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
@@ -232,7 +232,7 @@ int fdx_upconv3x3_wgrad(const fdx_act* x, const fdx_act* dy, float* dweff_ws, fl
   s = fdx_tc_launch(L, st);
   if (s != FDX_OK) return s;
   long long grid = (slab + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > fdx_num_sms() * 8) grid = fdx_num_sms() * 8;
   upconv_fold_kernel<<<(int)grid, 256, 0, st>>>(dweff_ws, slab, dw_hwio);
   FDX_LAUNCH_CHECK();
   return FDX_OK;

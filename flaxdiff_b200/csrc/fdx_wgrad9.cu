@@ -5,30 +5,23 @@
 //  trainer/general_diffusion_trainer.py:321-322).
 //
 // The generic split-K engine (fdx_tc.cu, TC_MNMN) re-reads X and dY from L2 once per (tap, row block,
-// column block): 43-85 FLOP per L2 byte, which is L2-bandwidth-bound on B200 (measured 200-750 TF/s).
-// Here one CTA owns a 64(ci) x 64(co) block of ALL nine taps for its slice of the pixels:
-//   * per 64-pixel block (16x4 or 8x8 patch) TMA brings ONE dY box and THREE X boxes - one per kx
-//     shift, each (TH+2) rows tall - so the three ky shifts of a box are plain row offsets of
-//     ky*TW*128 B: multiples of 1024 B, i.e. swizzle-aligned views of the same shared memory;
-//   * the nine taps are five tcgen05.mma groups of M=128 (two taps x 64 channels: the MN-major
-//     descriptor's leading-dimension offset jumps from one tap's view to the next), N=64, into
-//     five TMEM accumulators (320 columns);
-//   * X traffic drops from 9 to 3*(TH+2)/TH boxes per block: 107 FLOP per L2 byte.
-// Tiles = (ci block, co block, pixel split); split-K partial sums are combined with f32 atomics.
-//
-// TRANSPOSED = true computes the same tile as D^T: M = 64 output channels (A = the dY box, MN-major), and
-// N = 192 = the three ky views x 64 input channels of ONE kx box (B, MN-major; the views are TW*128 B
-// apart = the descriptor's leading-dimension offset): three 64 x 192 x 16 MMAs per K step instead of five
-// 128 x 64 x 16 ones.  An M = 64 accumulator fills lanes 0-15 of each TMEM sub-partition, so kx = 0 and
-// kx = 1 are interleaved into columns 0..191 (lane offsets 0 / 16) and kx = 2 uses columns 192..383.
+// column block).  Here one CTA owns a 64(ci) x 64(co) block of ALL nine taps for its slice of the pixels, and
+// the SHIFTS ARE SPLIT between the operands:  dW[ky][kx][ci][co] = sum_px X[y+ky-1, x'][ci] * dY[y, x'-kx+1][co]
+//   * A (M) = the ky views of ONE X box (TH+2 rows, no x halo): rows of TW pixels are TW*128 B apart
+//             (1024-aligned), so each ky is a 64-channel MN-major operand at a plain byte offset;
+//   * B (N) = THREE dY boxes shifted by kx-1 pixels (TMA zero-fills outside the image), contiguous in shared
+//             memory: N = 3 kx x 64 co = 192 (descriptor leading-dimension offset 8192).
+// Consumer warpgroup ky issues one m64 n192 k16 wgmma per 16 pixels; its accumulator row is (ky, ci) and its
+// columns (kx, co) are contiguous in HWIO, so the split-K partial sums leave the registers as 8-byte
+// red.global.add.v2.f32.  36 KB of TMA per 64-pixel block.
+// Tiles = (ci block, co block, pixel split).
 #include "fdx_common.cuh"
 #include "../../include/fdx.h"
-#include <stdlib.h>
 
 namespace {
 
-constexpr int kThreads = 192;
-constexpr int kStages = 4;
+constexpr int kStages = 5;
+constexpr int kThreads = 3 * 128 + 32;   // three consumer warpgroups (ky) + the producer warp
 
 struct W9Dev {
   int TW, TH;              // pixel patch (TW*TH == 64)
@@ -38,201 +31,10 @@ struct W9Dev {
   float* dw;               // [9][Cin][Cout] f32, accumulated
 };
 
-// tap order sorted by shared-memory address of its view: (kx, ky) lexicographic
-__device__ __forceinline__ int tap_of_slot(int slot) {   // slot 0..8 -> tap index ky*3+kx
-  const int kx = slot / 3, ky = slot % 3;
-  return ky * 3 + kx;
-}
-
-template <bool TRANSPOSED>
 __global__ void __launch_bounds__(kThreads, 1)
 fdx_wgrad9_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapY,
                   const W9Dev p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  const int xbuf_bytes = (p.TH + 2) * p.TW * 128;      // one kx box (rows of 64 bf16 channels)
-  const int ybuf_bytes = 64 * 128;
-  const int stage_bytes = 3 * xbuf_bytes + ybuf_bytes; // multiple of 1024
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * stage_bytes);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + kStages;
-  uint64_t* tfull = bars + 2 * kStages;
-  uint64_t* tempty = bars + 2 * kStages + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapX);
-    tma_prefetch_desc(&mapY);
-    for (int i = 0; i < kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 4);
-    fence_barrier_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const long long kblocks = (long long)p.nxb * p.nyb * p.nimg;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-        int r = tile;
-        const int cb = r % p.cib; r /= p.cib;
-        const int ob = r % p.cob; r /= p.cob;
-        const int sp = r;
-        const int pb0 = (int)((kblocks * sp) / p.splits), pb1 = (int)((kblocks * (sp + 1)) / p.splits);
-        for (int pb = pb0; pb < pb1; ++pb) {
-          const int xb = pb % p.nxb, yb = (pb / p.nxb) % p.nyb, nb = pb / (p.nxb * p.nyb);
-          mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sx = smem + stage * stage_bytes;
-          uint8_t* sy = sx + 3 * xbuf_bytes;
-          mbar_arrive_expect_tx(&full[stage], stage_bytes);
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx)
-            tma_load_4d(sx + kx * xbuf_bytes, &mapX, &full[stage], cb * 64, xb * p.TW + kx - 1,
-                        yb * p.TH - 1, nb);
-          tma_load_4d(sy, &mapY, &full[stage], ob * 64, xb * p.TW, yb * p.TH, nb);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = TRANSPOSED ? umma_idesc_bf16(64, 192, 1, 1) : umma_idesc_bf16(128, 64, 1, 1);
-      int stage = 0; uint32_t phase = 0, tphase = 0;
-      for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-        const int sp = tile / (p.cib * p.cob);
-        const int nk = (int)((kblocks * (sp + 1)) / p.splits) - (int)((kblocks * sp) / p.splits);
-        mbar_wait(tempty, tphase ^ 1);
-        tc_fence_after();
-        for (int i = 0; i < nk; ++i) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sx = smem_u32(smem + stage * stage_bytes);
-          const uint32_t sy = sx + 3 * xbuf_bytes;
-          if constexpr (TRANSPOSED) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t da = umma_desc_sw128(sy + k * 2048, 8192, 1024);            // dY: 64 co x 16 px
-#pragma unroll
-              for (int kx = 0; kx < 3; ++kx) {
-                // B = (ky, ci) columns of box kx: three 64-channel blocks, p.TW * 128 B apart
-                const uint64_t db = umma_desc_sw128(sx + kx * xbuf_bytes + k * 2048, p.TW * 128, 1024);
-                const uint32_t d = tmem_base + (kx == 2 ? 192u : 0u) + (kx == 1 ? (16u << 16) : 0u);
-                umma_f16(d, da, db, idesc, (i | k) != 0 ? 1u : 0u);
-              }
-            }
-          } else
-#pragma unroll
-          for (int g = 0; g < 5; ++g) {
-            // slots 2g, 2g+1 (slot 9 does not exist: its rows are computed on slot 8's view and dropped)
-            const int s0 = 2 * g, s1 = (2 * g + 1 < 9) ? 2 * g + 1 : 2 * g;
-            const uint32_t v0 = sx + (s0 / 3) * xbuf_bytes + (s0 % 3) * p.TW * 128;
-            const uint32_t v1 = sx + (s1 / 3) * xbuf_bytes + (s1 % 3) * p.TW * 128;
-            const uint32_t lbo = (v1 > v0) ? (v1 - v0) : 1024;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t da = umma_desc_sw128(v0 + k * 2048, lbo, 1024);
-              const uint64_t db = umma_desc_sw128(sy + k * 2048, 8192, 1024);
-              umma_f16(tmem_base + g * 64, da, db, idesc, (i | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull);
-        tphase ^= 1;
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    uint32_t tphase = 0;
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-      int r = tile;
-      const int cb = r % p.cib; r /= p.cib;
-      const int ob = r % p.cob;
-      const int ci = cb * 64 + (row & 63);
-      mbar_wait(tfull, tphase);
-      tc_fence_after();
-      if constexpr (TRANSPOSED) {
-        // lane = output channel: rows 16 q + (lane & 15); lanes 0-15 hold kx = 0 (columns 0..191) and
-        // kx = 2 (columns 192..383), lanes 16-31 hold kx = 1 (columns 0..191); column = ky * 64 + ci
-        const int co = ob * 64 + q * 16 + (lane & 15);
-#pragma unroll 1
-        for (int c0 = 0; c0 < 384; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-          tmem_ld_wait();
-          const int kx = c0 < 192 ? (lane >> 4) : 2;
-          const bool live = (c0 < 192 || lane < 16) && co < p.Cout;
-          if (live) {
-            const int cc = c0 < 192 ? c0 : c0 - 192;
-            const int ky = cc >> 6, ci0 = cb * 64 + (cc & 63);
-            float* out = p.dw + ((long long)(ky * 3 + kx) * p.Cin + ci0) * p.Cout + co;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (ci0 + j < p.Cin) atomicAdd(out + (long long)j * p.Cout, __uint_as_float(v[j]));
-          }
-        }
-      } else
-#pragma unroll 1
-      for (int g = 0; g < 5; ++g) {
-        const int slot = 2 * g + (row >> 6);
-        const bool valid = (slot < 9) && (ci < p.Cin);
-        const int tap = valid ? tap_of_slot(slot) : 0;
-        float* out = p.dw + ((long long)tap * p.Cin + ci) * p.Cout + ob * 64;
-#pragma unroll 1
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(g * 64 + c0), v);
-          tmem_ld_wait();
-          if (valid && ob * 64 + c0 < p.Cout) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(out + c0 + j),
-                           "f"(__uint_as_float(v[j])), "f"(__uint_as_float(v[j + 1])),
-                           "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
-                           : "memory");
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);
-      tphase ^= 1;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
-}
-
-
-// ---------------------------------------------------------------------------------------------------
-// Round-2 arrangement ("ky pairs in M, kx in N").  The kernels above are bounded by the MMA SHAPE, not by
-// data movement: tcgen05 floor = max(M,128) * N / 256 cycles per K=16 step, so the transposed variant's three
-// M=64 x N=192 MMAs cost 3 * 96 = 288 cycles for work worth 144 (50 %), and the tap-pair variant's five
-// M=128 x N=64 MMAs are operand-read bound ((4 KB + 2 KB) / 128 B per cycle = 48 > 32).  Here the SHIFTS ARE
-// SPLIT between the operands:  dW[ky][kx][ci][co] = sum_px X[y+ky-1, x'][ci] * dY[y, x'-kx+1][co]
-//   * A (M) = the ky views of ONE X box (TH+2 rows, no x halo): rows of TW pixels are TW*128 B apart
-//             (1024-aligned), so (ky=0, ky=1) x 64 ci is one M=128 operand (descriptor LBO = TW*128) and
-//             ky=2 an M=64 one;
-//   * B (N) = THREE dY boxes shifted by kx-1 pixels (TMA zero-fills outside the image), contiguous in shared
-//             memory: N = 3 kx x 64 co = 192 (descriptor LBO = 8192).
-// Two MMAs per K=16 step, 96 + 96 = 192 cycles for 144 cycles' worth of work (75 % floor instead of 50 %),
-// 36 KB of TMA per 64-pixel block instead of 44 KB, and every accumulator row is (ky, ci) with the columns
-// (kx, co) contiguous in HWIO, so the split-K reduction is 16-byte red.global.add.v4.f32.
-// TMEM: columns [0,192) = ky 0/1 (128 lanes), [192,384) = ky 2 (lanes 0-15 of each sub-partition).
-__global__ void __launch_bounds__(kThreads, 1)
-fdx_wgrad9k_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapY,
-                   const W9Dev p) {
-  constexpr int S = 5;
+  constexpr int S = kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -243,27 +45,18 @@ fdx_wgrad9k_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_consta
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + S;
-  uint64_t* tfull = bars + 2 * S;
-  uint64_t* tempty = bars + 2 * S + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 12 && lane == 0) {
     tma_prefetch_desc(&mapX);
     tma_prefetch_desc(&mapY);
-    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 4);
+    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 3); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const long long kblocks = (long long)p.nxb * p.nyb * p.nimg;
 
-  if (warp == 0) {
+  if (warp == 12) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
@@ -286,80 +79,59 @@ fdx_wgrad9k_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc01 = umma_idesc_bf16(128, 192, 1, 1);
-      constexpr uint32_t idesc2 = umma_idesc_bf16(64, 192, 1, 1);
-      int stage = 0; uint32_t phase = 0, tphase = 0;
-      for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-        const int sp = tile / (p.cib * p.cob);
-        const int nk = (int)((kblocks * (sp + 1)) / p.splits) - (int)((kblocks * sp) / p.splits);
-        mbar_wait(tempty, tphase ^ 1);
-        tc_fence_after();
-        for (int i = 0; i < nk; ++i) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sx = smem_u32(smem + stage * stage_bytes);
-          const uint32_t sy = sx + xbuf_bytes;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t db = umma_desc_sw128(sy + k * 2048, 8192, 1024);              // 3 kx x 64 co
-            const uint64_t da01 = umma_desc_sw128(sx + k * 2048, row_bytes, 1024);       // ky 0 | ky 1
-            const uint64_t da2 = umma_desc_sw128(sx + 2 * row_bytes + k * 2048, 1024, 1024);
-            umma_f16(tmem_base, da01, db, idesc01, (i | k) != 0 ? 1u : 0u);
-            umma_f16(tmem_base + 192u, da2, db, idesc2, (i | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull);
-        tphase ^= 1;
-      }
-    }
   } else {
-    const int q = warp & 3;
-    uint32_t tphase = 0;
+    const int ky = warp >> 2;                            // this warpgroup's row of taps
+    const int w = warp & 3;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    float acc[96];
+    int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
       int r = tile;
       const int cb = r % p.cib; r /= p.cib;
       const int ob = r % p.cob; r /= p.cob;
       const int sp = r;
-      const bool has = ((int)((kblocks * (sp + 1)) / p.splits) - (int)((kblocks * sp) / p.splits)) > 0;
-      mbar_wait(tfull, tphase);
-      tc_fence_after();
-      // columns [0,192): row = 32 q + lane = (ky = row >> 6, ci = row & 63); columns [192,384): ky = 2,
-      // lanes 0-15 of this sub-partition = ci 16 q + lane
-#pragma unroll 1
-      for (int c0 = 0; c0 < 384; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-        tmem_ld_wait();
-        const bool first = c0 < 192;
-        const int row = q * 32 + lane;
-        const int ky = first ? (row >> 6) : 2;
-        const int ci = cb * 64 + (first ? (row & 63) : (q * 16 + (lane & 15)));
-        const int cc = first ? c0 : c0 - 192;
-        const int kx = cc >> 6, co0 = ob * 64 + (cc & 63);
-        const bool live = has && (first || lane < 16) && ci < p.Cin && co0 < p.Cout;
-        if (live) {
-          float* out = p.dw + ((long long)(ky * 3 + kx) * p.Cin + ci) * p.Cout + co0;
+      const int nk = (int)((kblocks * (sp + 1)) / p.splits) - (int)((kblocks * sp) / p.splits);
 #pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(out + j),
-                         "f"(__uint_as_float(v[j])), "f"(__uint_as_float(v[j + 1])),
-                         "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
+      for (int i = 0; i < 96; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int i = 0; i < nk; ++i) {
+        mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        const uint32_t sx = smem_u32(smem + stage * stage_bytes);
+        const uint32_t sy = sx + xbuf_bytes;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t da = gmma_desc_sw128(sx + ky * row_bytes + k * 2048, 1024, 1024);   // 64 ci x 16 px
+          const uint64_t db = gmma_desc_sw128(sy + k * 2048, 8192, 1024);                    // 3 kx x 64 co
+          wgmma_bf16<192, 1, 1>(acc, da, db);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && wg_leader) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty[prev]);
+      if (nk > 0) {
+        // fragment: rows ci = 16 w + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1) = (kx, co)
+        const int ci = cb * 64 + w * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < 24; ++j) {
+          const int kx = j >> 3, co = ob * 64 + (j & 7) * 8 + 2 * (lane & 3);
+          if (co >= p.Cout) continue;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (ci + 8 * h >= p.Cin) continue;
+            float* out = p.dw + ((long long)(ky * 3 + kx) * p.Cin + ci + 8 * h) * p.Cout + co;
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(out), "f"(acc[4 * j + 2 * h]),
+                         "f"(acc[4 * j + 2 * h + 1])
                          : "memory");
+          }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);
-      tphase ^= 1;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 }  // namespace
@@ -413,39 +185,18 @@ int fdx_wgrad9_launch(const fdx_act* x, const fdx_act* dy, float* dw, cudaStream
     int s = fdx_make_tmap_bf16(&mY, dy->ptr, 4, dims, str, box, est, 1);
     if (s != FDX_OK) return s;
   }
-  // default: the round-2 "ky pairs in M, kx in N" kernel; FDX_WGRAD9_V1=1 selects the round-1 kernels
-  // (transposed arrangement, or the tap-pair one with FDX_NO_WGRAD9T=1).  Cout must be a multiple of 32 for
-  // the 16-byte reductions (it is a multiple of 64 on every UNet layer).
-  if (!getenv("FDX_WGRAD9_V1")) {
-    const int stage_k = (d.TH + 2) * d.TW * 128 + 3 * 64 * 128;
-    const int smem_k = 5 * stage_k + 1024 + 256;
-    static bool attr_k = false;
-    if (!attr_k) {
-      FDX_CUDA(cudaFuncSetAttribute(fdx_wgrad9k_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    5 * (6 * 16 * 128 + 3 * 64 * 128) + 1024 + 256));
-      attr_k = true;
-    }
-    const int gridk = sms < d.ntiles ? sms : d.ntiles;
-    fdx_wgrad9k_kernel<<<gridk, kThreads, smem_k, stream>>>(mX, mY, d);
-    fdx_note_kernel(FDX_KERNEL_WGRAD9K);
-    FDX_LAUNCH_CHECK();
-    return FDX_OK;
-  }
-  const int stage_bytes = 3 * (d.TH + 2) * d.TW * 128 + 64 * 128;
+  // Cout must be even for the 8-byte reductions (it is a multiple of 64 on every UNet layer).
+  if (d.Cout % 2 != 0) return FDX_ERR_UNSUPPORTED;
+  const int stage_bytes = (d.TH + 2) * d.TW * 128 + 3 * 64 * 128;
   const int smem_bytes = kStages * stage_bytes + 1024 + 256;
   static bool attr_set = false;
   if (!attr_set) {
-    const int max_smem = kStages * (3 * 6 * 16 * 128 + 64 * 128) + 1024 + 256;
-    FDX_CUDA(cudaFuncSetAttribute(fdx_wgrad9_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    FDX_CUDA(cudaFuncSetAttribute(fdx_wgrad9_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    FDX_CUDA(cudaFuncSetAttribute(fdx_wgrad9_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  kStages * (6 * 16 * 128 + 3 * 64 * 128) + 1024 + 256));
     attr_set = true;
   }
-  int grid = sms < d.ntiles ? sms : d.ntiles;
-  // transposed arrangement by default (22.5 vs 23.1 ms/step at C2); FDX_NO_WGRAD9T=1 selects the tap-pair one
-  if (!getenv("FDX_NO_WGRAD9T"))
-    fdx_wgrad9_kernel<true><<<grid, kThreads, smem_bytes, stream>>>(mX, mY, d);
-  else
-    fdx_wgrad9_kernel<false><<<grid, kThreads, smem_bytes, stream>>>(mX, mY, d);
+  const int grid = sms < d.ntiles ? sms : d.ntiles;
+  fdx_wgrad9_kernel<<<grid, kThreads, smem_bytes, stream>>>(mX, mY, d);
   fdx_note_kernel(FDX_KERNEL_WGRAD9);
   FDX_LAUNCH_CHECK();
   return FDX_OK;

@@ -10,14 +10,14 @@ API kept from the reference (flax.linen module surface):
 Parameter names / layouts are flax's (HWIO conv kernels, (in,out) dense kernels, names as in
 pretrained/*/_METADATA): `ConvLayer_0/conv/kernel`, `down_0_residual_0/norm1/scale`, ...
 
-Execution design (B200-first, not a translation of the flax module tree):
+Execution design (GPU-first, not a translation of the flax module tree):
   * activations are NHWC bf16; every skip concatenation (simple_unet.py:145,196) is a
     channel *slot* of a pre-allocated buffer, so producers write it in place and the
     concat is free; TMA reads the strided views directly;
   * each ResidualBlock (models/common.py:284-338) is: GN stats -> GN apply+SiLU ->
-    conv3x3 [tcgen05] with bias + timestep row-vector fused in the epilogue -> GN stats ->
+    conv3x3 [wgmma] with bias + timestep row-vector fused in the epilogue -> GN stats ->
     apply+SiLU -> conv3x3 with bias + residual fused; the 1x1 residual conv is a GEMM;
-  * backward is an explicit tape (no autograd engine): dgrad / wgrad on the same tcgen05
+  * backward is an explicit tape (no autograd engine): dgrad / wgrad on the same wgmma
     engine, GroupNorm backward in two streaming passes, gradients accumulated at forks by
     the consumer kernels' accumulate flags;
   * reference quirks kept: res-blocks of a down level keep the incoming width, Upsample
@@ -51,9 +51,8 @@ def _attn_width(d: int) -> int:
     return 32 if d <= 32 else 64
 
 
-# 1x1 residual convolutions (ResidualBlock.residual_conv): conv-geometry launches by default - since the transposed
-# engine got eight epilogue warps they beat the flat GEMM launch on the HBM-bound shapes
-# (profiles/layers_r02_res1x1.txt); FDX_RES1X1_GEMM=1 restores the flat launch.
+# 1x1 residual convolutions (ResidualBlock.residual_conv): conv-geometry launches by default, so the layers with
+# 64 / 128 output channels run on the transposed engine; FDX_RES1X1_GEMM=1 restores the flat GEMM launch.
 _RES1X1_GEMM = bool(os.environ.get("FDX_RES1X1_GEMM"))
 _GN_APPLY_V1 = bool(os.environ.get("FDX_GN_APPLY_V1"))
 
@@ -562,8 +561,8 @@ class Unet:
     def _attn_fwd(self, name, xin: Node, dst: Node, heads, W, W16, ctx16=None):
         """TransformerBlock(only_pure_attention) (models/attention.py:321-380): xn = RMSNorm(x);
         out = xn + to_out(softmax(q k^T / sqrt(d)) v), keys / values from `textcontext` (cross-attention,
-        77 x 768) or from xn itself.  q / k / v / out projections are tcgen05 GEMMs; the attention core is ONE
-        fused kernel (fdx_attention_fwd: logits and probabilities stay in TMEM / shared memory).  Heads
+        77 x 768) or from xn itself.  q / k / v / out projections are tensor-core GEMMs; the attention core is ONE
+        fused kernel (fdx_attention_fwd: logits and probabilities stay in registers / shared memory).  Heads
         narrower than 32 are zero-padded to 32 (the kernel stores heads 32 or 64 wide).
         FDX_ATTN_UNFUSED=1 selects the round-1 path (separate QK^T / softmax / PV launches)."""
         if os.environ.get("FDX_ATTN_UNFUSED"):

@@ -117,7 +117,7 @@ def gemm(mode: int, A: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N
          a_s=(0, 0), b_s=(0, 0), d_s=(0, 0), alpha: float = 1.0,
          bias: Optional[torch.Tensor] = None, res: Optional[torch.Tensor] = None,
          r_ld: int = 0, r_s=(0, 0), atomic: bool = False, reduce_batch: bool = False) -> torch.Tensor:
-    """Generic (batched) bf16 GEMM on the tcgen05 engine; see include/fdx.h fdx_gemm_desc."""
+    """Generic (batched) bf16 GEMM on the tensor-core engine; see include/fdx.h fdx_gemm_desc."""
     g = _lib.fdx_gemm_desc()
     g.mode = mode
     g.M, g.N, g.K = M, N, K
@@ -266,7 +266,7 @@ def conv_dgrad_groupnorm_bwd(dy, w_hwio, x, groups, stats, gamma, beta, eps, dga
     of the GroupNorm backward in its epilogue (dz = dy * silu'(z), sum dz, sum dz*x) where that convolution runs
     on the transposed engine, then ONE pass over x and dz; elsewhere data gradient + the two-pass GroupNorm
     backward.  FDX_GN_FUSE=0: never fused; FDX_GN_FUSE=1: fused wherever an image has >= 128 pixels (also on the
-    pixels-as-M engine, where four epilogue warps make it slower - profiles/layers_r01_gn_fusion.txt)."""
+    pixels-as-M engine)."""
     da = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
     if fused is None:
         env = os.environ.get("FDX_GN_FUSE")
@@ -543,7 +543,7 @@ def upconv3x3_wgrad(x: torch.Tensor, dy: torch.Tensor, dw_hwio: torch.Tensor) ->
 # --------------------------------------------------------------------------- 3-channel convs
 def conv_in_fwd(x_bf16: torch.Tensor, w: torch.Tensor, bias, out: torch.Tensor,
                 w_bf16: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """conv_in 3->Cout as im2col (K = 27 padded to 32) + one tcgen05 GEMM with the bias fused."""
+    """conv_in 3->Cout as im2col (K = 27 padded to 32) + one tensor-core GEMM with the bias fused."""
     n, h, w_, c = x_bf16.shape
     assert c == 3 and x_bf16.dtype == torch.bfloat16 and x_bf16.is_contiguous()
     cout = out.shape[-1]
@@ -593,7 +593,7 @@ def conv_in_wgrad_direct(x_bf16, dy, dw, dbias):
 
 
 def conv_out_fwd(x: torch.Tensor, w: torch.Tensor, bias) -> torch.Tensor:
-    """conv_out Cin->3: one tcgen05 GEMM (pixels x Cin)(Cin x 27, padded to 32) with f32 output, then the
+    """conv_out Cin->3: one tensor-core GEMM (pixels x Cin)(Cin x 27, padded to 32) with f32 output, then the
     col2im scatter that adds the nine taps' partial sums and the bias."""
     n, h, w_, cin = x.shape
     wr = torch.zeros((cin, 32), dtype=torch.float32, device=x.device)

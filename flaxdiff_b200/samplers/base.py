@@ -5,7 +5,7 @@ What is kept from the reference: constructor and `generate_samples` / `sample_st
 bit-exact), classifier-free-guidance batching, the "last step returns x0" rule, the initial-noise
 scaling and the final clip.
 
-What is different (B200-first): the reference jits only `sample_model` and runs every update
+What is different (GPU-first): the reference jits only `sample_model` and runs every update
 rule as dozens of un-jitted XLA dispatches (SURVEY.md $3.2).  Here one denoise evaluation
 (rates -> c_in scaling -> UNet -> x0/eps recovery) is captured ONCE in a CUDA graph per
 (shape, params) and replayed per step, and every update rule is a single `fdx_affine_combine`

@@ -1,4 +1,4 @@
-/* fdx.h -- C-ABI of libfdx.so, the B200 (sm_100a) kernel library under the
+/* fdx.h -- C-ABI of libfdx.so, the H100 (sm_90a) kernel library under the
  * flaxdiff_b200 Python surface.
  *
  * The reference (AshishKumar4/FlaxDiff) has no FFI / plugin interface: every device
@@ -43,15 +43,14 @@ unsigned long long fdx_launch_count(void);
  * profiler attribute a CUDA-event interval around one C-ABI call to the kernel that ran (bench.py roofline). */
 #define FDX_KERNEL_TC 0       /* fdx_tc_kernel: pixels-as-M tap-GEMM engine */
 #define FDX_KERNEL_TCT 1      /* fdx_tct_kernel: transposed (weights-as-M) engine */
-#define FDX_KERNEL_WGRAD9K 2  /* fdx_wgrad9k_kernel: nine-tap weight gradient, ky pairs in M / kx in N */
-#define FDX_KERNEL_WGRAD9 3   /* fdx_wgrad9_kernel: round-1 nine-tap weight gradient */
-#define FDX_KERNEL_CONV3 4    /* fdx_conv3_kernel: halo-sharing forward (opt-in) */
+/* 2 and 4: retired kernel families */
+#define FDX_KERNEL_WGRAD9 3   /* fdx_wgrad9_kernel: nine-tap weight gradient, ky in M / kx in N */
 #define FDX_KERNEL_ATTN_FWD 5 /* fdx_attn_fwd_kernel: fused attention forward */
 #define FDX_KERNEL_ATTN_BWD 6 /* fdx_attn_bwd_kernel: fused attention backward */
 int fdx_last_kernel_kind(void);
 const char* fdx_kernel_kind_name(int kind);
 
-/* ---- tensor-core contractions (tcgen05 + TMA + TMEM) ------------------------- */
+/* ---- tensor-core contractions (wgmma + TMA) ----------------------------------- */
 /* flax nn.Conv 3x3 SAME, stride 1 or 2 (models/common.py:166-172, 237-244).
  * y = conv(x, w) + bias + rowvec[n] + res ; bias [Cout] f32, rowvec [N][Cout] f32 (the
  * ResidualBlock's `out + temb` add, common.py:300-308), res = residual add (common.py:334).
@@ -312,7 +311,7 @@ int fdx_geglu_bwd(const void* u_bf16, const void* dg_bf16, long long rows, int i
  * nn.dot_product_attention inside NormalAttention (models/attention.py:156-177): o = softmax(q k^T * scale) v
  * per (image, head), self-attention (Lk = L) or cross-attention to the text context (Lk = 77), and its
  * backward under jax.value_and_grad (trainer/general_diffusion_trainer.py:321).  The logits and probabilities
- * never reach HBM: flash-style tcgen05 kernels with S / P in TMEM / shared memory; the backward recomputes
+ * never reach HBM: flash-style wgmma kernels with S in registers and P in shared memory; the backward recomputes
  * them from `lse` (two kernels: dQ per query tile, dK + dV per key block; deterministic, no atomics).
  * Tensors: bf16 [B][rows][heads*dh], `*_ld` = elements between rows, `*_bs` = elements between images;
  * dh (as STORED) is 32 or 64 - narrower heads are zero-padded by the caller, `scale` = 1/sqrt(true width).

@@ -23,7 +23,7 @@ def _usable_cores() -> int:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
     try:
         import torch
         torch.set_num_threads(_usable_cores())   # os.cpu_count() over-reports inside a cgroup

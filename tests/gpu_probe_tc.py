@@ -1,4 +1,4 @@
-"""GPU probe for the tcgen05 tap-GEMM engine (run under gpurun; not a pytest file).
+"""GPU probe for the wgmma tap-GEMM engine (run directly on a GPU machine; not a pytest file).
 
 Runs every mode (conv fwd / dgrad / wgrad, stride 1 and 2, GEMM KK / KMN / MNMN, batched)
 against a torch fp32 reference on the same bf16-rounded inputs and prints one line per

@@ -93,16 +93,15 @@ def test_attention_strided_views_and_determinism():
 
 @pytest.mark.parametrize("B,heads,L,Lk,dh", [(2, 8, 1024, 1024, 64), (1, 4, 200, 300, 32), (2, 8, 384, 77, 64)])
 def test_attention_kernel_arrangements_agree(B, heads, L, Lk, dh, monkeypatch):
-    """The default arrangements (forward: two CTAs per SM with single S / P / O buffers for long key sequences;
-    backward: two element-wise warp groups) against their predecessors (FDX_ATTN_NO_DUAL / FDX_ATTN_BWD_EWG1,
-    read per launch).  Same arithmetic in the same order per element, so the results are bit-identical."""
+    """The forward's single-stage arrangement for key sequences that fit one 128-key block against the K/V ring
+    (FDX_ATTN_NO_SHORT, read per launch).  Same arithmetic in the same order per element, so the results are
+    bit-identical."""
     torch.manual_seed(2)
     HD = heads * dh
     q, k, v, d_o = (torch.randn(B, n, HD, device=dev).bfloat16() for n in (L, Lk, Lk, L))
     o, lse = ops.attention_fwd(q, k, v, heads, dh, dh ** -0.5)
     g = ops.attention_bwd(q, k, v, o, lse, d_o, heads, dh, dh ** -0.5)
-    monkeypatch.setenv("FDX_ATTN_NO_DUAL", "1")
-    monkeypatch.setenv("FDX_ATTN_BWD_EWG1", "1")
+    monkeypatch.setenv("FDX_ATTN_NO_SHORT", "1")
     o1, lse1 = ops.attention_fwd(q, k, v, heads, dh, dh ** -0.5)
     g1 = ops.attention_bwd(q, k, v, o, lse, d_o, heads, dh, dh ** -0.5)
     torch.cuda.synchronize()

@@ -222,7 +222,7 @@ def test_conv_in_out_and_grads():
     w_in = torch.randn(3, 3, 3, 64, device=dev) * 0.2
     b_in = torch.randn(64, device=dev) * 0.1
     y = torch.empty(B, H, H, 64, device=dev, dtype=torch.bfloat16)
-    ops.conv_in_fwd(x, w_in, b_in, y)             # im2col + tcgen05 GEMM (bf16 weights)
+    ops.conv_in_fwd(x, w_in, b_in, y)             # im2col + tensor-core GEMM (bf16 weights)
     wr, br = w_in.cpu().requires_grad_(True), b_in.cpu().requires_grad_(True)
     yr = U.conv_same(x.float().cpu(), wr, br)
     assert rel(y, yr) < 6e-3
@@ -240,18 +240,18 @@ def test_conv_in_out_and_grads():
     Fo = ops.conv_out_fwd(a, w_out, b_out)
     ar, wo, bo = a.float().cpu().requires_grad_(True), w_out.cpu().requires_grad_(True), b_out.cpu().requires_grad_(True)
     Fr = U.conv_same(ar, wo, bo)
-    assert rel(Fo, Fr) < 5e-3                     # tcgen05 GEMM (bf16 weights) + col2im scatter
+    assert rel(Fo, Fr) < 5e-3                     # tensor-core GEMM (bf16 weights) + col2im scatter
     assert rel(ops.conv_out_fwd_direct(a, w_out, b_out), Fr) < 1e-5   # CUDA-core variant, f32 weights
     dF = torch.randn(B, H, H, 3, device=dev)
     Fr.backward(dF.cpu())
     da = torch.empty_like(a)
-    ops.conv_out_dgrad(dF, w_out, da)             # im2col + tcgen05 GEMM (dF and weights in bf16)
+    ops.conv_out_dgrad(dF, w_out, da)             # im2col + tensor-core GEMM (dF and weights in bf16)
     assert rel(da, ar.grad) < 8e-3
     da2 = torch.empty_like(a)
     ops.conv_out_dgrad_direct(dF, w_out, da2)
     assert rel(da2, ar.grad) < 5e-3
     dwo, dbo = torch.zeros_like(w_out), torch.zeros_like(b_out)
-    ops.conv_out_wgrad(a, dF, dwo, dbo)          # im2col + tcgen05 GEMM (dF rounded to bf16)
+    ops.conv_out_wgrad(a, dF, dwo, dbo)          # im2col + tensor-core GEMM (dF rounded to bf16)
     assert rel(dwo, wo.grad) < 5e-3 and rel(dbo, bo.grad) < 5e-3
     dwo2, dbo2 = torch.zeros_like(w_out), torch.zeros_like(b_out)
     ops.conv_out_wgrad_direct(a, dF, dwo2, dbo2)  # CUDA-core variant, f32 dF

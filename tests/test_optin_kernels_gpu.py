@@ -1,10 +1,8 @@
 """The opt-in / alternative kernel arrangements (DESIGN.md $6 environment switches) under `-m gpu`:
 each is compared with the default arrangement AND with a plain fp32 torch convolution on the same inputs.
-  FDX_PAIR=1        CTA-pair (cta_group::2) tcgen05 kernels           fdx_tc.cu PAIR path
-  FDX_CONV3=1       halo-sharing forward kernel                        fdx_conv3.cu
+  FDX_TC_BN_V1=1    round-1 column-tile rule of the pixels-as-M engine  fdx_tc.cu
+  FDX_TCT_HALO=1    per-tap loads in the transposed engine (no M tile is 1 wide, so the halo variant is off)
   FDX_NO_TCT=1      pixels-as-M engine instead of the transposed one   fdx_tc.cu vs fdx_tct.cu
-  FDX_NO_WGRAD9T=1  tap-pair arrangement of the nine-tap weight gradient
-  FDX_WGRAD9_V1=1   round-1 nine-tap weight-gradient kernel instead of the kx-in-N one
   FDX_GN_FUSE=1     GroupNorm-backward first pass fused into the dgrad epilogue
   FDX_GN_2PASS=0    one-launch CLUSTER GroupNorm backward (measured slower than the two-pass default; kept tested)
   FDX_GN_PIPE=2     persistent software-pipelined GroupNorm backward (same)
@@ -80,7 +78,7 @@ def test_transposed_engine_halo_sharing_vs_per_tap_loads(B, H, W, cin, cout):
     assert rel(outs[1][0], outs[0][0]) < 2e-3 and rel(outs[1][1], outs[0][1]) < 2e-3
 
 
-@pytest.mark.parametrize("flag", ["FDX_PAIR", "FDX_CONV3", "FDX_NO_TCT"])
+@pytest.mark.parametrize("flag", ["FDX_TC_BN_V1", "FDX_TCT_HALO", "FDX_NO_TCT"])
 @pytest.mark.parametrize("B,H,W,cin,cout", SHAPES)
 def test_forward_and_dgrad_variants(flag, B, H, W, cin, cout):
     torch.manual_seed(0)
@@ -102,23 +100,6 @@ def test_forward_and_dgrad_variants(flag, B, H, W, cin, cout):
         assert rel(y, want) < 5e-3 and rel(dx, xr.grad) < 5e-3, (flag, on)
         outs.append((y, dx))
     assert rel(outs[1][0], outs[0][0]) < 2e-3 and rel(outs[1][1], outs[0][1]) < 2e-3
-
-
-@pytest.mark.parametrize("flag", ["FDX_NO_WGRAD9T", "FDX_WGRAD9_V1"])
-@pytest.mark.parametrize("B,H,W,cin,cout", SHAPES)
-def test_weight_gradient_variants(flag, B, H, W, cin, cout):
-    torch.manual_seed(0)
-    x = torch.randn(B, H, W, cin, device=dev).bfloat16()
-    dy = torch.randn(B, H, W, cout, device=dev).bfloat16()
-    wr = torch.zeros(3, 3, cin, cout, requires_grad=True, device=dev)
-    _conv_ref(x, wr).backward(dy.float())
-    for on in (False, True):
-        extra = {"FDX_WGRAD9_V1": "1"} if (flag == "FDX_NO_WGRAD9T" and on) else {}
-        with env(**{flag: "1" if on else None, **extra}):
-            dw = torch.zeros(3, 3, cin, cout, device=dev)
-            ops.conv3x3_wgrad(x, dy, dw)
-            torch.cuda.synchronize()
-        assert rel(dw, wr.grad) < 2e-3, (flag, on, rel(dw, wr.grad))
 
 
 @pytest.mark.parametrize("B,H,W,cin,cout", [(2, 32, 32, 128, 256), (2, 16, 16, 64, 64), (1, 64, 64, 192, 64)])

@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 tap-GEMM engine through the C-ABI (fdx_conv3x3_{fwd,dgrad,wgrad}, fdx_gemm)
+"""Parity of the wgmma tap-GEMM engine through the C-ABI (fdx_conv3x3_{fwd,dgrad,wgrad}, fdx_gemm)
 against fp32 references on the same bf16-rounded inputs.  Tolerance: relative L2 error <= 5e-3 for bf16
 outputs (one bf16 rounding of an f32 accumulator: 2^-9 ~ 2e-3), <= 1e-4 for f32 outputs."""
 import os
