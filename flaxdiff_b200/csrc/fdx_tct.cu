@@ -92,7 +92,6 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
           // stages: (kx, K chunk, half); taps t = ky * 3 + kx (fdx_conv3x3_fwd / dgrad fill order)
           for (int qq = 0; qq < 3 * p.kchunks * NH; ++qq) {
             const int q = qq / NH, y0 = yb * TH + 16 * (qq % NH);
-            if (IL && y0 >= p.H) continue;          // H % 32 == 16: the last tile has no second half
             const int kx = q / p.kchunks, kc = q % p.kchunks;
             mbar_wait(&empty[stage], phase ^ 1);
             uint8_t* sw = smem + stage * kStageBytes;
@@ -116,7 +115,6 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
         } else
         for (int qq = 0; qq < nk * NH; ++qq) {
           const int q = qq / NH, y0 = yb * TH + 16 * (qq % NH);
-          if (IL && y0 >= p.H) continue;            // H % 32 == 16: the last tile has no second half
           const int t = q / p.kchunks, kc = q % p.kchunks;
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sw = smem + stage * kStageBytes;
@@ -159,9 +157,9 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
     const __nv_bfloat16* resp = static_cast<const __nv_bfloat16*>(p.res);
     WgAcc<128> acc;
     int stage = 0; uint32_t phase = 0;
-    // Side input (residual / accumulate source): the register prefetch below runs one 32-pixel chunk ahead,
-    // enough for an L2 hit, not for HBM.  So the consumer threads pull the side input of the NEXT tile into L2
-    // while they work on the current one (one line per pixel and 64 channels; <= 64 KB per CTA in flight).
+    // Side input (residual / accumulate source): each epilogue chunk loads its own pieces, which hides an L2
+    // hit, not HBM.  So the consumer threads pull the side input of the NEXT tile into L2 while they work on
+    // the current one (one line per pixel and 64 channels; <= 64 KB per CTA in flight).
     auto prefetch_res = [&](int t) {
       if (resp == nullptr || t >= p.ntiles) return;
       const int cb_ = t % p.cblks, mt_ = t / p.cblks;
@@ -186,7 +184,6 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
       const int yh = yb * TH + (IL ? 16 * (piece >> 1) : 0);
       const long long obase = (long long)nb * p.os_n + (long long)yh * p.os_y + (long long)(xb * 16) * p.os_x;
       const long long rbase = (long long)nb * p.rs_n + (long long)yh * p.rs_y + (long long)(xb * 16) * p.rs_x;
-      // residual pieces are requested one 32-pixel chunk ahead (the first before the main loop)
       const int ch = cw0 + (IL ? (piece & 1) : piece) * 8;   // read phase: this lane's first channel
       const bool ch_ok = ch < p.Ncols && yh < p.H;           // (H % 32 == 16: the last tile has no half 1)
       float add[8];
@@ -221,10 +218,8 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
                                                    (long long)(j & 15) * p.rs_x + ch);
         }
       };
-      uint4 rcur[PPX], rnxt[PPX];
-      load_res(c_begin, rcur);
+      uint4 rcur[PPX];
       // ---- main loop: this warpgroup's 128 pixel columns ----
-      const int yb_i = yb;
       acc.zero();
       int prev = -1;
       auto release = [&]() {
@@ -234,53 +229,36 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
         prev = stage;
         if (++stage == S) { stage = 0; phase ^= 1; }
       };
-      if constexpr (HALO) {
-        for (int qq = 0; qq < 3 * p.kchunks * NH; ++qq) {
-          if (IL && yb_i * TH + 16 * (qq % NH) >= p.H) continue;   // same skip as the producer
-          const int hh = qq % NH;
+      // The half index is a compile-time constant (the halves are an unrolled inner loop): with a run-time
+      // choice of accumulator, or with the two halves' wgmma on different control paths, ptxas serialises
+      // every wgmma of the kernel.  For the same reason a tile without half 1 (H % 32 == 16) still runs it,
+      // on the zero rows TMA fills in below the image; the epilogue stores none of it.
+      const int nq = HALO ? 3 * p.kchunks : nk;
+      for (int kq = 0; kq < nq; ++kq) {
+#pragma unroll
+        for (int hh = 0; hh < NH; ++hh) {
           mbar_wait(&full[stage], phase);
           wgmma_fence();
           const uint32_t sw = smem_u32(smem + stage * kStageBytes);
-          const uint32_t sx = sw + 3 * kWBytes + wg * 16384;     // pixel rows 8 wg .. 8 wg + 7 of the view
+          // HALO: pixel rows 8 wg .. 8 wg + 7 of the box view; per-tap: this warpgroup's 128-pixel box
+          const uint32_t sx = sw + (HALO ? 3 : 1) * kWBytes + wg * 16384;
 #pragma unroll
-          for (int ky = 0; ky < 3; ++ky) {
+          for (int ky = 0; ky < (HALO ? 3 : 1); ++ky) {
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
               const uint32_t aw = A_MN ? sw + ky * kWBytes + k * 2048 : sw + ky * kWBytes + k * 32;
-              const uint64_t db = gmma_desc_sw128(sx + ky * 2048 + k * 32, 16, 1024);   // rows ky .. ky+15 of the box
+              const uint64_t db = gmma_desc_sw128(sx + ky * 2048 + k * 32, 16, 1024);   // HALO: rows ky .. ky+15
+              const uint64_t da = A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024);
               if constexpr (IL) {
-                acc.mma_half<A_MN ? 1 : 0, 0>(hh, A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024), db);
+                acc.mma_half<A_MN ? 1 : 0, 0>(hh, da, db);
               } else {
-                acc.mma<A_MN ? 1 : 0, 0>(A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024),
-                                         A_MN ? gmma_desc_sw128(aw + 8192, 8192, 1024)
-                                              : gmma_desc_sw128(aw + 8192, 16, 1024),
-                                         db);
+                acc.mma<A_MN ? 1 : 0, 0>(da, A_MN ? gmma_desc_sw128(aw + 8192, 8192, 1024)
+                                                  : gmma_desc_sw128(aw + 8192, 16, 1024), db);
               }
             }
           }
           release();
         }
-      } else
-      for (int qq = 0; qq < nk * NH; ++qq) {
-        if (IL && yb_i * TH + 16 * (qq % NH) >= p.H) continue;     // same skip as the producer
-        const int hh = qq % NH;
-        mbar_wait(&full[stage], phase);
-        wgmma_fence();
-        const uint32_t sw = smem_u32(smem + stage * kStageBytes);
-        const uint32_t sx = sw + kWBytes + wg * 16384;             // this warpgroup's 128-pixel box
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint32_t aw = A_MN ? sw + k * 2048 : sw + k * 32;
-          const uint64_t db = gmma_desc_sw128(sx + k * 32, 16, 1024);
-          if constexpr (IL) {
-            acc.mma_half<A_MN ? 1 : 0, 0>(hh, A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024), db);
-          } else {
-            acc.mma<A_MN ? 1 : 0, 0>(A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024),
-                                     A_MN ? gmma_desc_sw128(aw + 8192, 8192, 1024) : gmma_desc_sw128(aw + 8192, 16, 1024),
-                                     db);
-          }
-        }
-        release();
       }
       wgmma_wait<0>();
       if (prev >= 0 && wg_leader) mbar_arrive(&empty[prev]);
@@ -288,31 +266,31 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
       float s0[8], s1[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) { s0[i] = 0.f; s1[i] = 0.f; }
-#pragma unroll 1
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
+      // Unrolled: the chunk index is a compile-time register index, and the 32 accumulator registers of a
+      // chunk die once it is written out, which keeps the epilogue within the consumer register budget.
+#pragma unroll
+      for (int ci = 0; ci < 4; ++ci) {
+        const int c0 = c_begin + 32 * ci;
+        // The side input of this chunk is requested before the exchange so its latency overlaps it.  (A
+        // register prefetch one chunk ahead would keep 16 more registers live and push the epilogue into spills.)
+        load_res(c0, rcur);
         // ---- write phase: accumulator fragments of columns c0 .. c0+31 -> xsT[px][channel row] ----
         named_bar_sync(xbar, 128);                       // the previous chunk's reads are done
         {
           const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
-          const int cc = (c0 - c_begin) >> 5;
 #pragma unroll
-          for (int ci = 0; ci < 4; ++ci) {
-            if (ci != cc) continue;                      // compile-time register indices, run-time chunk
+          for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj) {
-                const int r = h * 64 + w * 16 + (l >> 2), n = jj * 8 + 2 * (l & 3);
-                const float* d = &acc.d[h][(ci * 4 + jj) * 4];
-                xsT[n * kLdT + r] = d[0];
-                xsT[(n + 1) * kLdT + r] = d[1];
-                xsT[n * kLdT + r + 8] = d[2];
-                xsT[(n + 1) * kLdT + r + 8] = d[3];
-              }
-          }
+            for (int jj = 0; jj < 4; ++jj) {
+              const int r = h * 64 + w * 16 + (l >> 2), n = jj * 8 + 2 * (l & 3);
+              const float* d = &acc.d[h][(ci * 4 + jj) * 4];
+              xsT[n * kLdT + r] = d[0];
+              xsT[(n + 1) * kLdT + r] = d[1];
+              xsT[n * kLdT + r + 8] = d[2];
+              xsT[(n + 1) * kLdT + r + 8] = d[3];
+            }
         }
         named_bar_sync(xbar, 128);
-        load_res(c0 + 32, rnxt);
         // ---- read phase: 16-byte channel pieces; columns c0 .. c0+31 = pixel rows c0/16, c0/16 + 1 ----
 #pragma unroll
         for (int k = 0; k < PPX; ++k) {
@@ -353,8 +331,6 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
             }
           }
         }
-#pragma unroll
-        for (int k = 0; k < PPX; ++k) rcur[k] = rnxt[k];
       }
       if (p.cs_ws) {
         // lanes with the same piece (l % PPX) hold the same 8 channels: combine them
