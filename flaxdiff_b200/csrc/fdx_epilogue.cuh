@@ -4,11 +4,10 @@
 // straight from that layout makes each 16-byte store instruction of a warp touch 32 different cache
 // lines.  Here each warp stages its 32 rows x 64 channels (4 KB, XOR-swizzled 16-byte pieces, conflict free)
 // in shared memory and moves it to / from global memory with 8 lanes per pixel: four complete
-// 128-byte lines per instruction, for the store and for the fused side-input read alike.  The side
-// input (residual, or the GroupNorm input below) of the first 64-column chunk is requested BEFORE the
-// warp waits for the accumulator, and that of chunk c+1 while chunk c is being converted, so its
-// global-memory latency never sits on the epilogue's critical path; the first one is in flight while the
-// warpgroup runs its main loop.
+// 128-byte lines per instruction, for the store and for the fused side-input read alike.  Each 64-column
+// chunk loads its own side input (residual, or the GroupNorm input below) just before its accumulator
+// exchange; the caller requests those lines into L2 before the main loop, so the load is an L2 hit.  Holding
+// the next chunk's side input in registers instead would not fit beside a 128 x 128 accumulator.
 //
 // EPI = EPI_COLSTATS additionally accumulates, per (image, output channel), the sum and the sum of
 // squares of the bf16 values it stores: the statistics pass of the GroupNorm that consumes this tensor
@@ -53,9 +52,13 @@ __device__ __forceinline__ float epi_silu_grad_times(float dy, float z) {
 //   acc, xs, xbar : the warpgroup's accumulator, its exchange tile and named barrier (see WgAcc::row32)
 //   col_base: first global output column of the warpgroup's columns
 //   valid / obase / rbase / img : this LANE's row: in range?, element offsets into out / res, image index
-//   mainloop: called once, after the first side-input loads are in flight, to compute the accumulator
+//   mainloop: called once to compute the accumulator
 //   GN only : par = running chunk parity (kept by the caller across tiles), slot = workspace slot of
 //             this tile; all rows of the tile belong to image `img` of lane 0.
+// Row offsets are kept as 32-bit distances from lane 0's row (the host checks that a tile's rows span less than
+// 2^31 elements).  The chunk loop is unrolled, so every WgAcc::row32 reads fixed registers and a chunk's
+// accumulator registers are free once it is written: the accumulator never leaves the register file, and ptxas
+// does not serialise the main loop's wgmma.
 template <int WN, int EPI, class Acc, class MainFn>
 __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_t* stage, const Acc& acc, float* xs,
                                                        int xbar, int lane, int col_base, bool valid, long long obase,
@@ -66,51 +69,49 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
   const uint32_t sbase = smem_u32(stage);
   const int sub = lane >> 3, piece = lane & 7;       // coalesced phase: 4 rows x 8 pieces per instruction
   const bool side = (e.res != nullptr);
-  const __nv_bfloat16* resp = static_cast<const __nv_bfloat16*>(e.res);
+  const long long rbase0 = __shfl_sync(0xffffffffu, rbase, 0), obase0 = __shfl_sync(0xffffffffu, obase, 0);
+  const __nv_bfloat16* resp = side ? static_cast<const __nv_bfloat16*>(e.res) + rbase0 : nullptr;
+  __nv_bfloat16* outp = static_cast<__nv_bfloat16*>(e.out) + obase0;
 
   // per-lane coalesced coordinates: rows 4k + sub, k = 0..7
-  long long rb_k[8], ob_k[8];
+  int rb_k[8], ob_k[8];
   uint32_t ok_mask = 0;
+  {
+    const int rd = (int)(rbase - rbase0), od = (int)(obase - obase0);
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int r = 4 * k + sub;
-    rb_k[k] = __shfl_sync(0xffffffffu, rbase, r);
-    ob_k[k] = __shfl_sync(0xffffffffu, obase, r);
-    if (__shfl_sync(0xffffffffu, (int)valid, r)) ok_mask |= 1u << k;
+    for (int k = 0; k < 8; ++k) {
+      const int r = 4 * k + sub;
+      rb_k[k] = __shfl_sync(0xffffffffu, rd, r);
+      ob_k[k] = __shfl_sync(0xffffffffu, od, r);
+      if (__shfl_sync(0xffffffffu, (int)valid, r)) ok_mask |= 1u << k;
+    }
   }
   const int img0 = __shfl_sync(0xffffffffu, img, 0);
 
-  auto load_side = [&](int c0, uint4 (&dst)[8]) {
-    const int col0 = col_base + c0;
-    const bool in = (c0 < WN) && (col0 < e.Ncols);
-    const bool half2 = (col0 + 32) < e.Ncols;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      dst[k] = make_uint4(0, 0, 0, 0);
-      if (in && ((ok_mask >> k) & 1u) && (piece < 4 || half2))
-        dst[k] = *reinterpret_cast<const uint4*>(resp + rb_k[k] + col0 + piece * 8);
-    }
-  };
-
-  uint4 xr[8];
-  if (side) load_side(0, xr);
   mainloop();
 
-#pragma unroll 1
+#pragma unroll
   for (int c0 = 0; c0 < WN; c0 += 64) {
     const int col0 = col_base + c0;
     if (col0 >= e.Ncols) break;                      // uniform over the CTA
     const bool half2 = (col0 + 32) < e.Ncols;        // second 32-column half present (Ncols % 32 == 0)
-    uint4 xn[8];
-    // ---- side input: registers -> shared (coalesced layout), then request the next chunk's ---------
+    // ---- side input of this chunk: global -> registers -> shared (coalesced layout) -----------------
+    // Loaded before the accumulator exchange so that its latency overlaps it; the lines were requested
+    // into L2 before the main loop.
+    uint4 xr[8];
     if (side) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        xr[k] = make_uint4(0, 0, 0, 0);
+        if (((ok_mask >> k) & 1u) && (piece < 4 || half2))
+          xr[k] = *reinterpret_cast<const uint4*>(resp + rb_k[k] + col0 + piece * 8);
+      }
 #pragma unroll
       for (int k = 0; k < 8; ++k)
         asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + epi_swz(4 * k + sub, piece)),
                      "r"(xr[k].x), "r"(xr[k].y), "r"(xr[k].z), "r"(xr[k].w)
                      : "memory");
       __syncwarp();
-      load_side(c0 + 64, xn);
     }
     // ---- accumulator rows -> bf16 in shared -----------------------------------------------------
 #pragma unroll
@@ -189,13 +190,14 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
                    : "r"(sbase + epi_swz(4 * k + sub, piece))
                    : "memory");
       const bool live = ((ok_mask >> k) & 1u) && (piece < 4 || half2);
-      if (live) *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(e.out) + ob_k[k] + col0 + piece * 8) = u;
+      if (live) *reinterpret_cast<uint4*>(outp + ob_k[k] + col0 + piece * 8) = u;
       if constexpr (SUMS) {
         if (live) {
           const float2 d0 = unpack_bf16x2(u.x), d1 = unpack_bf16x2(u.y), d2 = unpack_bf16x2(u.z),
                        d3 = unpack_bf16x2(u.w);
-          // second factor: the GroupNorm input x (EPI_GN_BWD) or the stored value itself (EPI_COLSTATS)
-          const uint4 xq = GN ? xr[k] : u;
+          // second factor: the GroupNorm input x (EPI_GN_BWD; read again, an L1 hit, rather than held in
+          // registers through the accumulator exchange) or the stored value itself (EPI_COLSTATS)
+          const uint4 xq = GN ? *reinterpret_cast<const uint4*>(resp + rb_k[k] + col0 + piece * 8) : u;
           const float2 x0 = unpack_bf16x2(xq.x), x1 = unpack_bf16x2(xq.y), x2 = unpack_bf16x2(xq.z),
                        x3 = unpack_bf16x2(xq.w);
           s0[0] += d0.x; s0[1] += d0.y; s0[2] += d1.x; s0[3] += d1.y;
@@ -232,9 +234,5 @@ __device__ __forceinline__ void epilogue_bf16_coalesced(const EpiArgs& e, uint8_
       *par ^= 1;
     }
     __syncwarp();
-    if (side) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) xr[k] = xn[k];
-    }
   }
 }

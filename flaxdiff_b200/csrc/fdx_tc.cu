@@ -30,13 +30,15 @@ struct TcCfg {
   static constexpr int kWN = BN / kWG;              // wgmma N
   static constexpr int kThreads = 128 * (kWG + 1);  // + the producer warpgroup (one thread issues TMA)
   // K chunks (64 deep) per pipeline stage: at BN = 64 one chunk is only 8 wgmma (two row halves x 4 K
-  // steps), too little work per mbarrier round trip, so two chunks share a stage there.  Not used by the
-  // MN-major-A (weight-gradient) mode.
+  // steps), too little work per mbarrier round trip, so two chunks share a stage there.  The consumers always
+  // issue the MMAs of kSub chunks: the missing tail chunk of an odd chunk count reads a zeroed shared-memory
+  // block instead, so the MMA loop has one control path.  Not used by the MN-major-A (weight-gradient) mode.
   static constexpr int kSub = (BN == 64) ? 2 : 1;
   static constexpr int kStages = (BN == 128) ? 5 : 3;   // as many as fit in 227 KB
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kSub * (kABytes + kBBytes);
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/ +
+  static constexpr int kZeroBytes = (kSub > 1) ? kABytes : 0;   // zero operand block of the tail chunk
+  static constexpr int kSmemBytes = kStages * kStageBytes + kZeroBytes + 1024 /*align*/ + 256 /*barriers*/ +
                                     kWG * (16384 /*epilogue staging: 4 warps x 4 KB*/ + kAccXchgBytes);
   static_assert(kSmemBytes <= 227 * 1024, "tc: shared memory");
 };
@@ -112,10 +114,11 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * Cfg::kStageBytes);
+  uint8_t* zero_blk = smem + S * Cfg::kStageBytes;                   // kZeroBytes, 1024-byte aligned
+  uint64_t* bars = reinterpret_cast<uint64_t*>(zero_blk + Cfg::kZeroBytes);
   uint64_t* full = bars;            // [S]
   uint64_t* empty = bars + S;       // [S]
-  uint8_t* epi_stage = smem + S * Cfg::kStageBytes + 256;   // kWG x 16 KB, 128-byte aligned
+  uint8_t* epi_stage = zero_blk + Cfg::kZeroBytes + 256;   // kWG x 16 KB, 128-byte aligned
   float* acc_xchg = reinterpret_cast<float*>(epi_stage + Cfg::kWG * 16384);   // kWG x kAccXchgBytes
 
   const int warp = threadIdx.x >> 5;
@@ -130,6 +133,11 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
       mbar_init(&empty[i], Cfg::kWG);
     }
     fence_barrier_init();
+  }
+  if constexpr (Cfg::kZeroBytes > 0) {
+    for (int i = threadIdx.x; i < Cfg::kZeroBytes / 16; i += blockDim.x)
+      reinterpret_cast<uint4*>(zero_blk)[i] = make_uint4(0, 0, 0, 0);
+    fence_proxy_async_smem();       // the zeros are read by wgmma (async proxy)
   }
   __syncthreads();
   if constexpr (Cfg::kWG == 2) {
@@ -248,8 +256,8 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         nk = p.ntaps * p.kchunks;
         if (p.res) {
           rbase = (long long)n * p.rs_n + (long long)y * p.rs_y + (long long)x * p.rs_x;
-          // the side input of this row: request all of its lines now (L2 prefetch), before the main loop -
-          // the epilogue's own register prefetch runs only one 64-column chunk ahead
+          // the side input of this row: request all of its lines now (L2 prefetch), before the main loop, so
+          // that the epilogue's per-chunk loads of it hit L2
           if (valid && !p.out_f32 && !p.out_atomic) {
             const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(p.res) + rbase + nt * BN + wg * WN;
             const int ncol = min(WN, p.Ncols - nt * BN - wg * WN);
@@ -274,14 +282,16 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         acc.zero();
         int prev = -1;
         for (int qk = 0; qk < nk; qk += SUB) {
-          const int nsub = (nk - qk) < SUB ? (nk - qk) : SUB;
           mbar_wait(&full[stage], phase);
           wgmma_fence();
           const uint32_t sa0 = smem_u32(smem + stage * Cfg::kStageBytes);
           const uint32_t sb0 = sa0 + SUB * kABytes + wg * WN * 128;   // this warpgroup's B columns
-          for (int u = 0; u < nsub; ++u) {
-            const uint32_t sa = sa0 + u * kABytes;
-            const uint32_t sb = sb0 + u * Cfg::kBBytes;
+#pragma unroll
+          for (int u = 0; u < SUB; ++u) {
+            // an odd chunk count's missing tail chunk: both operands read the zero block, adding exact zeros
+            const bool live = qk + u < nk;
+            const uint32_t sa = live ? sa0 + u * kABytes : smem_u32(zero_blk);
+            const uint32_t sb = live ? sb0 + u * Cfg::kBBytes : smem_u32(zero_blk);
 #pragma unroll
             for (int k = 0; k < kBK / 16; ++k) {
               // K-major: advance 16 elements (32 B) inside the 128B swizzle row; SBO = 8 rows.
@@ -313,7 +323,8 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
                                          &gn_par, EPI != EPI_PLAIN ? tile % p.gn_slots : 0);
       } else {
       mainloop();
-#pragma unroll 1
+      // Unrolled for the same reason as epilogue_bf16_coalesced: row32 then reads fixed accumulator registers.
+#pragma unroll
       for (int c0 = 0; c0 < WN; c0 += 32) {
         float f[32];
         acc.row32(xs, xbar, c0, f);
@@ -345,7 +356,10 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
           if (p.out_atomic) {
             float* op = static_cast<float*>(p.out) + obase + col0;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) atomicAdd(op + j, f[j]);
+            for (int j = 0; j < 8; ++j)
+              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(op + 4 * j), "f"(f[4 * j]),
+                           "f"(f[4 * j + 1]), "f"(f[4 * j + 2]), "f"(f[4 * j + 3])
+                           : "memory");
           } else if (p.out_f32) {
             float4* op = reinterpret_cast<float4*>(static_cast<float*>(p.out) + obase + col0);
 #pragma unroll
@@ -452,6 +466,12 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
   d.rs_x = L.rs_x; d.rs_y = L.rs_y; d.rs_n = L.rs_n;
   d.gn_ab = L.gn_ab; d.gn_ws = L.gn_ws; d.gn_slots = L.gn_slots > 0 ? L.gn_slots : 1;
   d.ws_ld = L.ws_ld > 0 ? L.ws_ld : L.Ncols;
+  if (L.out_f32) {
+    // float4 stores and 16-byte vector reductions
+    FDX_REQUIRE(reinterpret_cast<uintptr_t>(L.out) % 16 == 0 && L.os_x % 4 == 0 && L.os_y % 4 == 0 &&
+                    L.os_n % 4 == 0 && L.os_tap % 4 == 0 && L.os_m % 4 == 0,
+                "tc: f32 output must be 16-byte aligned with strides that are multiples of 4");
+  }
   if (L.gn_ws && !L.gn_ab) {
     FDX_REQUIRE(L.mode == TC_KMN && !L.gemm_like && !L.out_f32 && !L.out_atomic,
                 "tc: output column statistics need a bf16 convolution-forward launch");
@@ -492,6 +512,14 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
     TN = 1;
   }
   d.TW = TW; d.TH = TH; d.TN = TN;
+  if (L.mode != TC_MNMN && !L.out_f32 && !L.out_atomic) {
+    // the bf16 epilogue holds each row's offsets as 32-bit distances from the tile's first row
+    auto span = [&](long long sx, long long sy, long long sn) {
+      return (TW - 1) * llabs(sx) + (TH - 1) * llabs(sy) + (TN - 1) * llabs(sn);
+    };
+    FDX_REQUIRE(span(L.os_x, L.os_y, L.os_n) < (1LL << 31) && span(L.rs_x, L.rs_y, L.rs_n) < (1LL << 31),
+                "tc: the rows of one output tile span 2^31 elements or more");
+  }
   if (L.gn_ws && TN != 1) {
     fdx_set_error("tc: fused per-image column sums need at least 128 pixels per image (got %dx%d)", L.W, L.H);
     return FDX_ERR_UNSUPPORTED;
