@@ -19,8 +19,10 @@
 //       fdx_attn_bwd_dkv  per 128-key block, loop over query tiles (transposed tiles, tile row = key):
 //                         dV += P^T dO ;  dK += dS^T Q
 //     with P = exp2(s * scale*log2e - lse*log2e), D = rowsum(dO o O), dS including the 1/sqrt(d) factor.
-// Tensors are bf16 [B][L][heads * dh] (row stride and batch stride given), dh in {32, 64}; keys beyond Lk and
-// query rows beyond L are handled by TMA zero fill + masking, so 77-key cross-attention needs no padded copies.
+// Tensors are bf16 [B][L][heads * dh] (row stride and batch stride given), dh in {32, 64, 128}; keys beyond Lk
+// and query rows beyond L are handled by TMA zero fill + masking, so 77-key cross-attention needs no padded copies.
+// dh = 128 has kernels of its own (fdx_attn_fwd128_kernel, fdx_attn_bwd128_kernel: two consumer warpgroups of 64
+// rows that keep every product in its wgmma fragment, 64-row backward tiles), described above them.
 #include "fdx_common.cuh"
 #include "../../include/fdx.h"
 #include <math.h>
@@ -466,10 +468,384 @@ fdx_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_cons
   }
 }
 
-int make_map(CUtensorMap* m, const void* ptr, int hd, int rows, int B, long long ld, long long bs) {
+// ======================================================================================================
+// head width 128.  The kernels above hold 128-row products per warpgroup and hand their rows out through the
+// exchange tile; at 128 channels those products no longer fit the register file next to the accumulators.
+// These kernels keep every product in its wgmma fragment: thread l of warp w of a warpgroup owns rows
+// 16 w + l/4 (h = 0) and 16 w + l/4 + 8 (h = 1) of the 64-row fragment and, for g = 0 .. N/8 - 1, columns
+// 8 g + 2 (l % 4) + e (e = 0, 1) in element 4 g + 2 h + e.  Row reductions run over the four lanes of a quad.
+// A 128-channel tile is two 64-channel chunks (two TMA boxes); 128 channels start on a chunk boundary, so the
+// in-row byte offset of the narrower kernels is always 0 here.
+// ======================================================================================================
+constexpr int kWTile = 2 * kTile;                // [128 rows][128 ch] bf16: two [128][64] chunks
+constexpr int kFwd128Threads = 2 * 128 + 32;     // two consumer warpgroups + the producer warp
+
+// one bf16 pair (row r, columns col, col + 1) into a [rows][64 col] K-major 128B-swizzled chunk; a quad's four
+// lanes fill one 16-byte piece and the eight quads of a warp hit eight different pieces: no bank conflicts
+__device__ __forceinline__ void st_frag_pair(uint32_t chunk, int r, int col, uint32_t w) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(chunk + swz(r, col >> 3) + (col & 7) * 2), "r"(w) : "memory");
+}
+
+// forward, 128 queries per CTA: warpgroup wg owns query rows [64 wg, 64 wg + 64).  Per key block S = Q K_j^T
+// is one m64n128 fragment (64 registers), O one more; P_j goes through the warpgroup's own [64][128] bf16 tile.
+// Shared memory: Q 32 KB, NKV x (K, V) 64 KB, P 2 x 16 KB.
+template <bool SHORT>
+__global__ void __launch_bounds__(kFwd128Threads, 1)
+fdx_attn_fwd128_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                       const __grid_constant__ CUtensorMap mapV, const AttnDev p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  constexpr int NKV = SHORT ? 1 : 2;
+  uint8_t* sQ = smem;                                 // [2 chunks][128 queries][64 ch]
+  uint8_t* sKV = smem + kWTile;                       // NKV x (K, V), each [2 chunks][128 keys][64 ch]
+  uint8_t* sP = sKV + NKV * 2 * kWTile;               // per warpgroup [2 chunks][64 queries][64 keys]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + kWTile);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;          // [NKV]
+  uint64_t* kv_empty = bars + 3;         // [NKV]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int head = blockIdx.y, b = blockIdx.z;
+  const int q0 = blockIdx.x * 128;
+  const int nblk = (p.Lk + 127) / 128;
+  const int c0 = head * 128;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&mapQ); tma_prefetch_desc(&mapK); tma_prefetch_desc(&mapV);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < NKV; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 2); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    if (lane == 0) {
+      mbar_arrive_expect_tx(q_full, kWTile);
+      tma_load_4d(sQ, &mapQ, q_full, c0, q0, b, 0);
+      tma_load_4d(sQ + kTile, &mapQ, q_full, c0 + 64, q0, b, 0);
+      for (int j = 0; j < nblk; ++j) {
+        const int s = j % NKV;
+        uint8_t* kv = sKV + s * 2 * kWTile;
+        mbar_wait(&kv_empty[s], ((j / NKV) & 1) ^ 1);
+        mbar_arrive_expect_tx(&kv_full[s], 2 * kWTile);
+        tma_load_4d(kv, &mapK, &kv_full[s], c0, j * 128, b, 0);
+        tma_load_4d(kv + kTile, &mapK, &kv_full[s], c0 + 64, j * 128, b, 0);
+        tma_load_4d(kv + kWTile, &mapV, &kv_full[s], c0, j * 128, b, 0);
+        tma_load_4d(kv + kWTile + kTile, &mapV, &kv_full[s], c0 + 64, j * 128, b, 0);
+      }
+    }
+  } else {
+    const int wg = warp >> 2;
+    const int rq = (warp & 3) * 16 + (lane >> 2);      // fragment rows rq, rq + 8 of this warpgroup's 64
+    const int cq = 2 * (lane & 3);                     // fragment column offset inside each 8-column group
+    const uint32_t aQ = smem_u32(sQ) + wg * 8192;
+    const uint32_t aP = smem_u32(sP) + wg * kTile;
+    float m[2] = {-INFINITY, -INFINITY};               // running row maxima (log2 domain, scaled)
+    float l[2] = {0.f, 0.f};                           // running row sums over this thread's columns
+    float O[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) O[i] = 0.f;
+    mbar_wait(q_full, 0);
+
+    for (int j = 0; j < nblk; ++j) {
+      const int s = j % NKV;
+      mbar_wait(&kv_full[s], (j / NKV) & 1);
+      const uint32_t aK = smem_u32(sKV + s * 2 * kWTile), aV = aK + kWTile;
+      float S[64];                                     // the first K step overwrites it (scale_d = 0)
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const uint32_t ko = (uint32_t)((k >> 2) * kTile + (k & 3) * 32);
+        wgmma_m64n128k16<0, 0>(S, gmma_desc_sw128(aQ + ko, 16, 1024), gmma_desc_sw128(aK + ko, 16, 1024), k > 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // keys beyond Lk (TMA zero fill; only the last block can be partial) drop out as -inf logits
+      const int kvalid = p.Lk - j * 128;
+      if (kvalid < 128) {
+#pragma unroll
+        for (int g = 0; g < 16; ++g)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (8 * g + cq + e >= kvalid) S[4 * g + e] = S[4 * g + 2 + e] = -INFINITY;
+      }
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int g = 0; g < 16; ++g)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) mx[h] = fmaxf(mx[h], fmaxf(S[4 * g + 2 * h], S[4 * g + 2 * h + 1]));
+      float corr[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        const float m_new = fmaxf(m[h], mx[h] * p.scale_log2);
+        corr[h] = ex2(m[h] - m_new);                   // first block: exp2(-inf) = 0
+        m[h] = m_new;
+      }
+      // probabilities -> bf16 -> the K-major swizzled A tile of the PV MMA
+      float rs[2] = {0.f, 0.f};
+#pragma unroll
+      for (int g = 0; g < 16; ++g) {
+        float pe[4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            pe[2 * h + e] = ex2(fmaf(S[4 * g + 2 * h + e], p.scale_log2, -m[h]));
+            rs[h] += pe[2 * h + e];
+          }
+        const uint32_t chunk = aP + (uint32_t)(g >> 3) * 8192;
+        st_frag_pair(chunk, rq, (g & 7) * 8 + cq, pack_bf16x2(pe[0], pe[1]));
+        st_frag_pair(chunk, rq + 8, (g & 7) * 8 + cq, pack_bf16x2(pe[2], pe[3]));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) l[h] = fmaf(l[h], corr[h], rs[h]);
+#pragma unroll
+      for (int g = 0; g < 16; ++g)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) O[4 * g + i] *= corr[i >> 1];
+      fence_proxy_async_smem();
+      named_bar_sync(1 + wg, 128);                     // every row of this warpgroup's P_j is in shared memory
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k)                      // B = V_j, MN-major: 64-channel chunks kTile apart
+        wgmma_m64n128k16<0, 1>(O, gmma_desc_sw128(aP + (k >> 2) * 8192 + (k & 3) * 32, 16, 1024),
+                               gmma_desc_sw128(aV + k * 2048, kTile, 1024));
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[s]);
+    }
+    float inv[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+      inv[h] = 1.f / l[h];
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = q0 + wg * 64 + rq + 8 * h;
+      if (row < p.L) {
+        __nv_bfloat16* op = p.o + (long long)b * p.o_bs + (long long)row * p.o_ld + c0 + cq;
+#pragma unroll
+        for (int g = 0; g < 16; ++g)
+          *reinterpret_cast<uint32_t*>(op + 8 * g) = pack_bf16x2(O[4 * g + 2 * h] * inv[h], O[4 * g + 2 * h + 1] * inv[h]);
+        if (p.lse && (lane & 3) == 0) p.lse[((long long)b * p.heads + head) * p.L + row] = m[h] * kLn2 + logf(l[h]);
+      }
+    }
+  }
+}
+
+// backward at head width 128: the skeleton of fdx_attn_bwd_kernel on 64-row tiles.  Per loop step each
+// warpgroup computes 64 of the 128 columns of S and dP (m64n64, 32 + 32 registers) and writes its half of
+// E1 = P and E2 = dS; then
+//   dQ[:, 64 wg .. +64] += dS . K_j[:, 64 wg .. +64]   (m64n64 per warpgroup)         [ROWS_ARE_KEYS = false]
+//   dV += P^T . dO_i (warpgroup 0),  dK += dS^T . Q_i (warpgroup 1)   (m64n128)        [ROWS_ARE_KEYS = true]
+// Shared memory: R1, R2 2 x 16 KB, a ring of 2 x (C1, C2) 2 x 64 KB, E1, E2 2 x 16 KB.
+template <bool ROWS_ARE_KEYS>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+fdx_attn_bwd128_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_constant__ CUtensorMap mapR2,
+                       const __grid_constant__ CUtensorMap mapC1, const __grid_constant__ CUtensorMap mapC2,
+                       const AttnDev p) {
+  constexpr int RING = 2;
+  constexpr int AN = ROWS_ARE_KEYS ? 128 : 64;         // accumulator columns per warpgroup
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* sR1 = smem;                                 // [2 chunks][64 rows][64 ch]
+  uint8_t* sR2 = smem + kTile;
+  uint8_t* sC = smem + 2 * kTile;                      // RING x (C1, C2), each [2 chunks][128 rows][64 ch]
+  uint8_t* sE1 = sC + RING * 2 * kWTile;               // [2 chunks][64 rows][64 columns]
+  uint8_t* sE2 = sE1 + kTile;
+  float* sStat = reinterpret_cast<float*>(sE2 + kTile);          // RING x (lse[128], dvec[128]) of the columns
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + RING * 256);
+  uint64_t* r_full = bars;
+  uint64_t* c_full = bars + 1;            // [RING]
+  uint64_t* c_empty = c_full + RING;      // [RING]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int head = blockIdx.y, b = blockIdx.z;
+  const int r0 = blockIdx.x * 64;
+  const int nrows = ROWS_ARE_KEYS ? p.Lk : p.L;
+  const int ncols = ROWS_ARE_KEYS ? p.L : p.Lk;
+  const int nstep = (ncols + 127) / 128;
+  const int c0 = head * 128;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&mapR1); tma_prefetch_desc(&mapR2); tma_prefetch_desc(&mapC1); tma_prefetch_desc(&mapC2);
+    mbar_init(r_full, 1);
+    for (int i = 0; i < RING; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 2); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  // setmaxnreg sits inside each role's branch: issued before code both roles run, ptxas ignores it (C7507)
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && lane == 0) {
+      mbar_arrive_expect_tx(r_full, 2 * kTile);
+      tma_load_4d(sR1, &mapR1, r_full, c0, r0, b, 0);
+      tma_load_4d(sR1 + 8192, &mapR1, r_full, c0 + 64, r0, b, 0);
+      tma_load_4d(sR2, &mapR2, r_full, c0, r0, b, 0);
+      tma_load_4d(sR2 + 8192, &mapR2, r_full, c0 + 64, r0, b, 0);
+      for (int j = 0; j < nstep; ++j) {
+        const int s = j % RING;
+        uint8_t* c = sC + s * 2 * kWTile;
+        mbar_wait(&c_empty[s], ((j / RING) & 1) ^ 1);
+        mbar_arrive_expect_tx(&c_full[s], 2 * kWTile);
+        tma_load_4d(c, &mapC1, &c_full[s], c0, j * 128, b, 0);
+        tma_load_4d(c + kTile, &mapC1, &c_full[s], c0 + 64, j * 128, b, 0);
+        tma_load_4d(c + kWTile, &mapC2, &c_full[s], c0, j * 128, b, 0);
+        tma_load_4d(c + kWTile + kTile, &mapC2, &c_full[s], c0 + 64, j * 128, b, 0);
+      }
+    }
+  } else {
+    consumer_regs();
+    const int wg = warp >> 2;                          // columns [64 wg, 64 wg + 64) of S / dP
+    const int rq = (warp & 3) * 16 + (lane >> 2);      // fragment rows rq, rq + 8
+    const int cq = 2 * (lane & 3);
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const long long stat_base = ((long long)b * p.heads + head) * p.L;
+    const bool row_in[2] = {r0 + rq < nrows, r0 + rq + 8 < nrows};
+    // dQ kernel: the statistics of this thread's two query rows; dK/dV kernel: they belong to the COLUMNS
+    float lse_r[2] = {0.f, 0.f}, d_r[2] = {0.f, 0.f};
+    if constexpr (!ROWS_ARE_KEYS) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (row_in[h]) {
+          lse_r[h] = p.lse[stat_base + r0 + rq + 8 * h] * kLog2e;
+          d_r[h] = p.dvec[stat_base + r0 + rq + 8 * h] * p.scale;
+        }
+    }
+    const uint32_t aR1 = smem_u32(sR1), aR2 = smem_u32(sR2);
+    const uint32_t aE1 = smem_u32(sE1), aE2 = smem_u32(sE2);
+    float A[AN / 2];                                   // dQ half | dV (warpgroup 0) or dK (warpgroup 1)
+#pragma unroll
+    for (int i = 0; i < AN / 2; ++i) A[i] = 0.f;
+    mbar_wait(r_full, 0);
+    for (int j = 0; j < nstep; ++j) {
+      const int s = j % RING;
+      const int cbase = j * 128;
+      if constexpr (ROWS_ARE_KEYS) {
+        // stage the query-side statistics of this step (parity buffer j & 1), 128 threads = 128 columns
+        if (wg == 0) {
+          float* st = sStat + (j & 1) * 256;
+          const int t = threadIdx.x;
+          const bool ok = cbase + t < p.L;
+          st[t] = ok ? p.lse[stat_base + cbase + t] * kLog2e : 0.f;
+          st[128 + t] = ok ? p.dvec[stat_base + cbase + t] * p.scale : 0.f;
+        }
+      }
+      mbar_wait(&c_full[s], (j / RING) & 1);
+      const uint32_t aC1 = smem_u32(sC + s * 2 * kWTile), aC2 = aC1 + kWTile;
+      // S (or S^T) = R1 . C1^T ;  dP (or dP^T) = R2 . C2^T  - this warpgroup's 64 columns
+      float Sa[32], Pa[32];                            // the first K step overwrites them (scale_d = 0)
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const uint32_t ro = (uint32_t)((k >> 2) * 8192 + (k & 3) * 32);
+        const uint32_t co = (uint32_t)((k >> 2) * kTile + wg * 8192 + (k & 3) * 32);
+        wgmma_m64n64k16<0, 0>(Sa, gmma_desc_sw128(aR1 + ro, 16, 1024), gmma_desc_sw128(aC1 + co, 16, 1024), k > 0);
+        wgmma_m64n64k16<0, 0>(Pa, gmma_desc_sw128(aR2 + ro, 16, 1024), gmma_desc_sw128(aC2 + co, 16, 1024), k > 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // the statistics are staged and the previous step's accumulation has consumed E1 / E2
+      named_bar_sync(1, 256);
+      const float* st = sStat + (j & 1) * 256;
+      // rows / columns outside the tensors (TMA zero fill; only the last row tile or step) drop out as -inf
+      // logits: P = 0 and dS = 0 there
+      const int col_lim = ncols - cbase - wg * 64;     // columns of this warpgroup inside the tensor
+      if (r0 + 64 > nrows || col_lim < 64) {
+#pragma unroll
+        for (int g = 0; g < 8; ++g)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (!(row_in[h] && 8 * g + cq + e < col_lim)) Sa[4 * g + 2 * h + e] = -INFINITY;
+      }
+      // P = exp2(s * scale*log2e - lse*log2e);  dS = P * (dP * scale - D * scale)
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        const int cl = 8 * g + cq;                     // column inside this warpgroup's 64
+        float lq[2][2], dq[2][2];                      // [h][e]
+        if constexpr (ROWS_ARE_KEYS) {
+          const float2 a2 = *reinterpret_cast<const float2*>(st + wg * 64 + cl);
+          const float2 b2 = *reinterpret_cast<const float2*>(st + 128 + wg * 64 + cl);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) { lq[h][0] = a2.x; lq[h][1] = a2.y; dq[h][0] = b2.x; dq[h][1] = b2.y; }
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) { lq[h][0] = lq[h][1] = lse_r[h]; dq[h][0] = dq[h][1] = d_r[h]; }
+        }
+        float pr[4], ds[4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int i = 4 * g + 2 * h + e;
+            pr[2 * h + e] = ex2(fmaf(Sa[i], p.scale_log2, -lq[h][e]));
+            ds[2 * h + e] = pr[2 * h + e] * fmaf(Pa[i], p.scale, -dq[h][e]);
+          }
+        if constexpr (ROWS_ARE_KEYS) {
+          st_frag_pair(aE1 + wg * 8192, rq, cl, pack_bf16x2(pr[0], pr[1]));
+          st_frag_pair(aE1 + wg * 8192, rq + 8, cl, pack_bf16x2(pr[2], pr[3]));
+        }
+        st_frag_pair(aE2 + wg * 8192, rq, cl, pack_bf16x2(ds[0], ds[1]));
+        st_frag_pair(aE2 + wg * 8192, rq + 8, cl, pack_bf16x2(ds[2], ds[3]));
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 256);                          // both halves of E1 / E2 are published
+      wgmma_fence();
+      if constexpr (ROWS_ARE_KEYS) {
+        // dV += P^T . dO_i (warpgroup 0) | dK += dS^T . Q_i (warpgroup 1); B MN-major, chunks kTile apart
+        const uint32_t aE = wg == 0 ? aE1 : aE2;
+        const uint32_t aB = wg == 0 ? aC2 : aC1;
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          wgmma_m64n128k16<0, 1>(A, gmma_desc_sw128(aE + (k >> 2) * 8192 + (k & 3) * 32, 16, 1024),
+                                 gmma_desc_sw128(aB + k * 2048, kTile, 1024));
+      } else {
+        // dQ[:, 64 wg ..] += dS . K_j[:, 64 wg ..]: B = channel chunk wg of K_j
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          wgmma_m64n64k16<0, 1>(A, gmma_desc_sw128(aE2 + (k >> 2) * 8192 + (k & 3) * 32, 16, 1024),
+                                gmma_desc_sw128(aC1 + wg * kTile + k * 2048, kTile, 1024));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (wg_leader) mbar_arrive(&c_empty[s]);
+    }
+    // epilogue: fragment rows -> bf16
+    __nv_bfloat16* base;
+    long long ld;
+    if constexpr (ROWS_ARE_KEYS) {
+      base = wg == 0 ? p.dv + (long long)b * p.dv_bs : p.dk + (long long)b * p.dk_bs;
+      ld = wg == 0 ? p.dv_ld : p.dk_ld;
+      base += c0 + cq;
+    } else {
+      base = p.dq + (long long)b * p.dq_bs + c0 + wg * 64 + cq;
+      ld = p.dq_ld;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (row_in[h]) {
+        __nv_bfloat16* rp = base + (long long)(r0 + rq + 8 * h) * ld;
+#pragma unroll
+        for (int g = 0; g < AN / 8; ++g)
+          *reinterpret_cast<uint32_t*>(rp + 8 * g) = pack_bf16x2(A[4 * g + 2 * h], A[4 * g + 2 * h + 1]);
+      }
+    }
+  }
+}
+
+int make_map(CUtensorMap* m, const void* ptr, int hd, int rows, int B, long long ld, long long bs,
+             int box_rows = 128) {
   uint64_t dims[4] = {(uint64_t)hd, (uint64_t)rows, (uint64_t)B, 1};
   uint64_t str[3] = {(uint64_t)ld * 2, (uint64_t)bs * 2, (uint64_t)bs * 2 * (uint64_t)B};
-  uint32_t box[4] = {64, 128, 1, 1};
+  uint32_t box[4] = {64, (uint32_t)box_rows, 1, 1};
   uint32_t est[4] = {1, 1, 1, 1};
   return fdx_make_tmap_bf16(m, ptr, 4, dims, str, box, est, 1);
 }
@@ -477,8 +853,8 @@ int make_map(CUtensorMap* m, const void* ptr, int hd, int rows, int B, long long
 int check_desc(const fdx_attn_desc* a, const char* who) {
   FDX_REQUIRE(a && a->q && a->k && a->v, "%s: null tensor", who);
   FDX_REQUIRE(a->B > 0 && a->heads > 0 && a->L > 0 && a->Lk > 0, "%s: bad sizes", who);
-  FDX_REQUIRE(a->dh == 32 || a->dh == 64, "%s: head width %d (stored) must be 32 or 64 - zero-pad narrower heads", who,
-              a->dh);
+  FDX_REQUIRE(a->dh == 32 || a->dh == 64 || a->dh == 128,
+              "%s: head width %d (stored) must be 32 or 64, or 128 - zero-pad narrower heads", who, a->dh);
   FDX_REQUIRE((a->heads * a->dh) % 64 == 0, "%s: heads * dh must be a multiple of 64", who);
   FDX_REQUIRE(a->q_ld % 8 == 0 && a->k_ld % 8 == 0 && a->v_ld % 8 == 0, "%s: row strides must be multiples of 8", who);
   return FDX_OK;
@@ -503,6 +879,29 @@ int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
   d.o = (__nv_bfloat16*)a->o; d.o_ld = a->o_ld; d.o_bs = a->o_bs;
   d.lse = a->lse;
   const bool short_keys = a->Lk <= 128 && !getenv("FDX_ATTN_NO_SHORT");
+  if (a->dh == 128) {
+    const int smem128 = (2 + 2 * (short_keys ? 1 : 2)) * kWTile + 1024 + 64;
+    dim3 grid128((a->L + 127) / 128, a->heads, a->B);
+    static bool attr128[2] = {false, false};
+    if (short_keys) {
+      if (!attr128[0]) {
+        FDX_CUDA(cudaFuncSetAttribute(fdx_attn_fwd128_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      smem128));
+        attr128[0] = true;
+      }
+      fdx_attn_fwd128_kernel<true><<<grid128, kFwd128Threads, smem128, (cudaStream_t)stream>>>(mQ, mK, mV, d);
+    } else {
+      if (!attr128[1]) {
+        FDX_CUDA(cudaFuncSetAttribute(fdx_attn_fwd128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      smem128));
+        attr128[1] = true;
+      }
+      fdx_attn_fwd128_kernel<false><<<grid128, kFwd128Threads, smem128, (cudaStream_t)stream>>>(mQ, mK, mV, d);
+    }
+    fdx_note_kernel(FDX_KERNEL_ATTN_FWD);
+    FDX_LAUNCH_CHECK();
+    return FDX_OK;
+  }
   const int smem = (1 + 2 * (short_keys ? 1 : kKV) + 2) * kTile + kAccXchgBytes + 1024 + 256;
   dim3 grid((a->L + 127) / 128, a->heads, a->B);
   static bool attr[4] = {false, false, false, false};
@@ -552,6 +951,33 @@ int fdx_attention_bwd(const fdx_attn_desc* a, void* stream) {
     const long long total = (long long)a->B * a->L * a->heads;
     attn_dvec_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d);
     FDX_LAUNCH_CHECK();
+  }
+  if (a->dh == 128) {
+    // the row side of a 64-row tile comes in 64-row boxes; the looped column side keeps the 128-row maps
+    CUtensorMap rQ, rK, rV, rDO;
+    if ((s = make_map(&rQ, a->q, hd, a->L, a->B, a->q_ld, a->q_bs, 64)) != FDX_OK) return s;
+    if ((s = make_map(&rK, a->k, hd, a->Lk, a->B, a->k_ld, a->k_bs, 64)) != FDX_OK) return s;
+    if ((s = make_map(&rV, a->v, hd, a->Lk, a->B, a->v_ld, a->v_bs, 64)) != FDX_OK) return s;
+    if ((s = make_map(&rDO, a->d_o, hd, a->L, a->B, a->do_ld, a->do_bs, 64)) != FDX_OK) return s;
+    const int smem128 = 4 * kTile + 2 * 2 * kWTile + 2 * 256 * 4 + 1024 + 64;
+    static bool attr128 = false;
+    if (!attr128) {
+      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_bwd128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    smem128));
+      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_bwd128_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    smem128));
+      attr128 = true;
+    }
+    // dQ: rows = queries (Q, dO), loop (K_j, V_j);  dK/dV: rows = keys (K, V), loop (Q_i, dO_i)
+    fdx_attn_bwd128_kernel<false><<<dim3((a->L + 63) / 64, a->heads, a->B), kBwdThreads, smem128, st>>>(
+        rQ, rDO, mK, mV, d);
+    fdx_note_kernel(FDX_KERNEL_ATTN_BWD);
+    FDX_LAUNCH_CHECK();
+    fdx_attn_bwd128_kernel<true><<<dim3((a->Lk + 63) / 64, a->heads, a->B), kBwdThreads, smem128, st>>>(
+        rK, rV, mQ, mDO, d);
+    fdx_note_kernel(FDX_KERNEL_ATTN_BWD);
+    FDX_LAUNCH_CHECK();
+    return FDX_OK;
   }
   const int smem = (2 + 2 * 2 + 4) * kTile + 2 * 256 * 4 + 2 * kAccXchgBytes + 1024 + 256;
   static bool attr[4] = {false, false, false, false};

@@ -130,7 +130,8 @@ __device__ __forceinline__ void cluster_sync_all() {
 // ----- wgmma ----------------------------------------------------------------------
 // One warpgroup (four consecutive warps, the first a multiple of four) computes D(64 x N, f32 registers)
 // += A(64 x 16) * B(16 x N), both operands read from shared memory through matrix descriptors.  TA / TB = 1
-// selects an MN-major (transposed) operand, 0 a K-major one.
+// selects an MN-major (transposed) operand, 0 a K-major one.  scale_d = 0 ignores D's old contents (D = A * B),
+// so the first K step of a product needs no zeroed registers.
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -138,7 +139,7 @@ __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uint64_t db, int scale_d = 1) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %20, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
@@ -147,10 +148,10 @@ __device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uin
       "}, %16, %17, p, 1, 1, %18, %19;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(scale_d));
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db, int scale_d = 1) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %36, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
@@ -162,10 +163,10 @@ __device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uin
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(scale_d));
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db, int scale_d = 1) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %68, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
@@ -183,7 +184,7 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, ui
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(scale_d));
 }
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n192k16(float (&d)[96], uint64_t da, uint64_t db) {

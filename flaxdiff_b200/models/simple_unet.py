@@ -44,8 +44,10 @@ ATTN_EPS = 1e-4     # TransformerBlock.norm_epsilon, models/attention.py:319
 
 
 def _attn_width(d: int) -> int:
-    """Stored head width for the fused attention kernels: 32 or 64 (narrower heads are zero-padded).
-    FDX_ATTN_PAD64=1 stores every head 64 wide (one head per 128-byte swizzle row)."""
+    """Stored head width for the fused attention kernels: 32, 64 or 128 (narrower heads are zero-padded).
+    FDX_ATTN_PAD64=1 stores every head of up to 64 channels 64 wide (one head per 128-byte swizzle row)."""
+    if d > 64:
+        return 128
     if os.environ.get("FDX_ATTN_PAD64"):
         return 64
     return 32 if d <= 32 else 64
@@ -563,7 +565,8 @@ class Unet:
         out = xn + to_out(softmax(q k^T / sqrt(d)) v), keys / values from `textcontext` (cross-attention,
         77 x 768) or from xn itself.  q / k / v / out projections are tensor-core GEMMs; the attention core is ONE
         fused kernel (fdx_attention_fwd: logits and probabilities stay in registers / shared memory).  Heads
-        narrower than 32 are zero-padded to 32 (the kernel stores heads 32 or 64 wide).
+        narrower than 32 are zero-padded to 32, and heads of 65 - 127 channels to 128 (the kernel stores heads
+        32, 64 or 128 wide).
         FDX_ATTN_UNFUSED=1 selects the round-1 path (separate QK^T / softmax / PV launches)."""
         if os.environ.get("FDX_ATTN_UNFUSED"):
             return self._attn_fwd_unfused(name, xin, dst, heads, W, W16, ctx16)
@@ -572,8 +575,8 @@ class Unet:
         L = hh * ww
         d = C // heads
         dp = _attn_width(d)
-        if d > 64:
-            raise FdxError(f"attention: head width {d} > 64 is not supported")
+        if d > 128:
+            raise FdxError(f"attention: head width {d} > 128 is not supported")
         HD = heads * dp
         base = f"{name}/Attention/Attention2"
         dev = x.device
@@ -652,8 +655,8 @@ class Unet:
         Lk, Cc = ctx.shape[1], ctx.shape[2]
         d = C // heads
         dp = _attn_width(d)
-        if d > 64:
-            raise FdxError(f"attention: head width {d} > 64 is not supported")
+        if d > 128:
+            raise FdxError(f"attention: head width {d} > 128 is not supported")
         HD = heads * dp
         wq = self._pad_heads(W16[f"{base}/to_q/kernel"], 2, d, dp).reshape(C, HD)
         wk = self._pad_heads(W16[f"{base}/to_k/kernel"], 2, d, dp).reshape(Cc, HD)

@@ -314,7 +314,7 @@ int fdx_geglu_bwd(const void* u_bf16, const void* dg_bf16, long long rows, int i
  * never reach HBM: flash-style wgmma kernels with S in registers and P in shared memory; the backward recomputes
  * them from `lse` (two kernels: dQ per query tile, dK + dV per key block; deterministic, no atomics).
  * Tensors: bf16 [B][rows][heads*dh], `*_ld` = elements between rows, `*_bs` = elements between images;
- * dh (as STORED) is 32 or 64 - narrower heads are zero-padded by the caller, `scale` = 1/sqrt(true width).
+ * dh (as STORED) is 32, 64 or 128 - narrower heads are zero-padded by the caller, `scale` = 1/sqrt(true width).
  * lse: f32 [B][heads][L] (written by fwd, read by bwd); dvec_ws: f32 [B][heads][L] scratch (bwd). */
 typedef struct fdx_attn_desc {
   int B, heads, L, Lk, dh;
