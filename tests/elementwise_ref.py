@@ -1,0 +1,336 @@
+"""Float64 references of the memory-bound kernels (GroupNorm, RMSNorm, GEGLU, column sums, nearest 2x upsample)
+and an element-wise comparator whose tolerance is derived, element by element, from the kernels' arithmetic.
+
+Every reference takes the same bf16 values the kernel reads (as float64 tensors, on any device) and returns the
+exact result together with `delta`: a first-order bound on how far the kernel's f32 arithmetic can be from it
+before the output is stored.  The backwards are written in closed form (no autograd), so they run in float64 on
+the GPU at N = 256.
+
+Tolerance model (used by every element-wise test):
+  * bf16 output, got = bf16(v) with |v - ref| <= delta:
+        |got - ref| <= ulp_bf16(ref) + (1 + 2^-8) * delta                                           (k = 1)
+    Round to nearest gives |bf16(v) - v| <= ulp(v)/2 <= 2^-8 |v| <= 2^-8 (|ref| + delta), and 2^-8 |ref| < ulp(ref)
+    (bf16 has 8 significant bits).  One ulp is the output rounding; nothing else is allowed for free.
+  * f32 output: |got - ref| <= 2^-24 (|ref| + delta) + delta.
+  * delta collects the known error sources, each bounded where it arises:
+      - f32 sums:  |fl(sum t) - sum t| <= gamma(D) * sum |t|, D the longest chain of dependent additions
+        (Higham, Accuracy and Stability of Numerical Algorithms, 2nd ed., eq. 4.4), gamma(D) = D u / (1 - D u),
+        u = 2^-24.  D is counted from the kernel's loop structure where it is stated below, and otherwise taken
+        as the number of terms, which bounds every summation order.
+      - tanh.approx.f32 (f2_tanh in fdx_common.cuh, gelu_tanh_f in fdx_geglu.cu): relative error at most
+        2^-10.987 (PTX ISA, tanh); TANH below rounds that up to 2^-10.9.  SiLU is h (1 + tanh h) with h = z/2, so
+        its error is |h tanh h| TANH, about |h| 2^-11 for z << 0 where the output itself is near 0.
+      - rsqrtf: at most 2 ulp (CUDA C Programming Guide, Mathematical Functions), i.e. 4u relative.
+      - individual f32 roundings: u relative each; the count per formula is stated where it is used.
+      - the statistics a normalisation divides by: their relative error propagates through mean / rstd.
+    These are per-element bounds: the terms that involve a whole group (GroupNorm) or pixel (RMSNorm) are
+    means over that unit, i.e. epsilon * s with s the unit's scale.  Constants come from this derivation; if a
+    kernel exceeds its bound, that is a finding to explain, not a reason to widen the bound.
+"""
+from __future__ import annotations
+
+import math
+
+import torch
+import torch.nn.functional as Fnn
+
+U32 = 2.0 ** -24             # unit roundoff of f32
+U_BF16 = 2.0 ** -8           # unit roundoff of bf16 (8 significant bits)
+TANH = 2.0 ** -10.9          # relative error bound of tanh.approx.f32 (documented 2^-10.987)
+RSQRT = 4 * U32              # rsqrtf: 2 ulp of the result
+# bf16 x bf16 products are exact in f32; the tensor cores may add with truncation instead of rounding, so every
+# addition of the convolution's K-long accumulation counts 2u.
+TC_ADD = 2 * U32
+
+
+def gamma(depth) -> float:
+    d = float(depth) * U32
+    return d / (1.0 - d)
+
+
+def ulp_bf16(ref: torch.Tensor) -> torch.Tensor:
+    """Spacing of bf16 numbers at |ref| (2^(e-7) for |ref| in [2^e, 2^(e+1)); constant below the smallest normal)."""
+    a = ref.abs().to(torch.float64).clamp_min(2.0 ** -126)
+    _, e = torch.frexp(a)                     # a = m 2^e, m in [0.5, 1)
+    return torch.ldexp(torch.ones_like(a), (e - 8).to(torch.int32))
+
+
+def bf16_bound(ref: torch.Tensor, delta) -> torch.Tensor:
+    return ulp_bf16(ref) + (1 + U_BF16) * delta
+
+
+def f32_bound(ref: torch.Tensor, delta) -> torch.Tensor:
+    return U32 * (ref.abs() + delta) + delta
+
+
+def assert_elementwise(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor, what: str = "") -> float:
+    """Fail if any element of `got` is not finite or lies outside |got - ref| <= bound.  Returns the worst
+    |got - ref| / bound, so that callers can report how close a kernel comes to its bound."""
+    g = got.detach().to(torch.float64)
+    r = ref.detach().to(device=g.device, dtype=torch.float64)
+    b = torch.as_tensor(bound, dtype=torch.float64, device=g.device).expand_as(r)
+    assert g.shape == r.shape, (what, tuple(g.shape), tuple(r.shape))
+    err = (g - r).abs()
+    frac = err / b
+    bad = ~(err <= b) | ~torch.isfinite(g)            # NaN compares false: an unwritten NaN-prefilled element fails
+    nbad = int(bad.sum())
+    worst = torch.where(torch.isfinite(frac), frac, torch.full_like(frac, math.inf))
+    if nbad:
+        i = int(torch.argmax(torch.where(bad, worst, torch.zeros_like(worst))))
+    else:
+        i = int(torch.argmax(worst))
+    if g.numel() == 0:
+        return 0.0
+    idx = tuple(int(v) for v in torch.unravel_index(torch.tensor(i), tuple(g.shape))) if g.dim() else ()
+    gi, ri, bi = g.reshape(-1)[i].item(), r.reshape(-1)[i].item(), b.reshape(-1)[i].item()
+    ei = abs(gi - ri) if math.isfinite(gi) else math.inf
+    ulps = ei / ulp_bf16(torch.tensor(ri, dtype=torch.float64)).item()
+    assert nbad == 0, (f"{what}: {nbad} of {g.numel()} elements outside the bound; worst at {idx}: got {gi!r}, "
+                       f"ref {ri!r}, |err| = {ei:.4g} = {ulps:.3g} bf16 ulp = {ei / bi:.3g} x its bound {bi:.4g}")
+    return float(worst.max()) if worst.numel() else 0.0
+
+
+# ----------------------------------------------------------------------------------------------- GroupNorm
+def _g(t: torch.Tensor, G: int) -> torch.Tensor:
+    """(N, H, W, C) -> (N, HW, G, C/G)."""
+    return t.reshape(t.shape[0], -1, G, t.shape[-1] // G)
+
+
+def _gmean(t: torch.Tensor) -> torch.Tensor:
+    """Mean over the (pixel, channel-in-group) unit of a grouped tensor, kept for broadcasting."""
+    return t.mean((1, 3), keepdim=True)
+
+
+def gn_stats_ref(x: torch.Tensor, G: int):
+    """fdx_groupnorm_stats: [N][G] (sum, sum of squares) -> (value, delta).  gn_stats_kernel gives each thread
+    ceil(HW C/(8 G) / 256) 16-byte vectors of 8 serial additions, then a 5-level warp tree and the 8 warps in
+    order: D = 8 ceil(HW C / (2048 G)) + 13.  bf16 squares are exact in f32."""
+    xg = _g(x, G)
+    n_items = xg.shape[1] * xg.shape[3] // 8
+    D = 8 * math.ceil(n_items / 256) + 13
+    val = torch.stack([xg.sum((1, 3)), (xg * xg).sum((1, 3))], -1)
+    delta = gamma(D) * torch.stack([xg.abs().sum((1, 3)), (xg * xg).sum((1, 3))], -1)
+    return val, delta
+
+
+class GnFwd:
+    """Closed-form GroupNorm (flax: f32 statistics, var = max(0, E[x^2] - E[x]^2), y = (x - mean) rstd gamma + beta)
+    with optional SiLU, and the f32 error of the statistics the kernels derive from fdx_groupnorm_stats."""
+
+    def __init__(self, x, gamma_, beta_, G: int, eps: float, silu: bool):
+        self.G, self.silu, self.shape = G, silu, x.shape
+        N, H, W, C = x.shape
+        self.HW, self.cpg = H * W, C // G
+        xg = _g(x, G)
+        self.xg = xg
+        self.gam = gamma_.reshape(1, 1, G, -1).to(torch.float64)
+        self.bet = beta_.reshape(1, 1, G, -1).to(torch.float64)
+        mu = _gmean(xg)
+        ex2 = _gmean(xg * xg)
+        var = (ex2 - mu * mu).clamp_min(0)
+        self.mu, self.r = mu, 1.0 / torch.sqrt(var + eps)
+        self.xh = (xg - mu) * self.r
+        self.z = self.gam * self.xh + self.bet
+        # statistics: mean = s/cnt (1 rounding), var = q/cnt - mean^2 (3 roundings), rstd (2 ulp):
+        #   dmu <= (D+1) u mean|x|,   drstd/rstd <= (D+3) u (E[x^2] + mean^2) / (var + eps) + 5u
+        # D covers both producers of the sums: gn_stats_kernel (gn_stats_ref) and the per-channel column sums
+        # of fdx_groupnorm_apply_cols (each rounded once to f32, then 4 slots x ceil(cpg/32) per lane and a
+        # 5-level warp tree)
+        D = max(8 * math.ceil(self.HW * self.cpg / 8 / 256) + 13, 4 * math.ceil(self.cpg / 32) + 6)
+        self.dmu = gamma(D + 1) * _gmean(xg.abs())
+        self.rho_r = gamma(D + 3) * (ex2 + mu * mu) / (var + eps) + RSQRT + U32
+        self.dxh = self.r * ((xg - mu).abs() * self.rho_r + self.dmu)      # error of the kernel's normalised x
+        # z = fma(x, a, b) with a = rstd gamma and b = beta - mean a: 3 roundings on |a|(|x| + |mean|) + |beta|
+        self.dz = self.gam.abs() * self.dxh + 3 * U32 * (self.gam.abs() * self.r * (xg.abs() + mu.abs()) +
+                                                         self.bet.abs())
+        h = 0.5 * self.z
+        self.h, self.t = h, torch.tanh(h)
+
+    def forward(self):
+        """-> (y, delta) as (N, H, W, C).  y = h (1 + tanh h) is one fma on the approximate tanh."""
+        if not self.silu:
+            return self.z.reshape(self.shape), self.dz.reshape(self.shape)
+        y = self.h * (1 + self.t)
+        sig = 0.5 * (1 + self.t)
+        dsilu = sig * (1 + self.h * (1 - self.t))
+        delta = dsilu.abs() * self.dz + (self.h * self.t).abs() * TANH + U32 * y.abs()
+        return y.reshape(self.shape), delta.reshape(self.shape)
+
+
+def gn_forward_ref(x, gamma_, beta_, G, eps, silu):
+    return GnFwd(x, gamma_, beta_, G, eps, silu).forward()
+
+
+def gn_backward_ref(x, dy, gamma_, beta_, G, eps, silu, dy_delta=None):
+    """Closed-form GroupNorm(+SiLU) backward -> dict of (value, delta) for dx, dgamma, dbeta and the per-image /
+    total column sums of dx.  `dy_delta` is a per-element bound on the error of the dy the kernel sees (the fused
+    path's convolution data gradient and its bf16 rounding).
+
+        dz = dy silu'(z),  g = gamma dz,  dx = rstd (g - mean_g(g) - xhat mean_g(g xhat))
+        dbeta = sum_{n,p} dz,  dgamma = sum_{n,p} dz xhat
+    """
+    f = GnFwd(x, gamma_, beta_, G, eps, silu)
+    N = x.shape[0]
+    dyg = _g(dy, G)
+    gam_a, r = f.gam.abs(), f.r
+    if silu:
+        sig = 0.5 * (1 + f.t)
+        dsilu = sig * (1 + f.h * (1 - f.t))
+        dz = dyg * dsilu
+        # silu'(z) = (1+t)/2 (1 + h(1-t)): d silu'/dt = 1/2 - h t, |silu''| <= 1/2, then 6 roundings on the
+        # pair arithmetic (each <= u (1 + 2|h|) |dy|)
+        e_dz = dyg.abs() * ((0.5 - f.h * f.t).abs() * f.t.abs() * TANH + 0.5 * f.dz + 6 * U32 * (1 + 2 * f.h.abs()))
+    else:
+        dsilu = torch.ones_like(dyg)
+        dz = dyg
+        e_dz = torch.zeros_like(dyg)
+    if dy_delta is not None:
+        e_dz = e_dz + dsilu.abs() * _g(dy_delta, G)
+    g = f.gam * dz
+    m1, m2 = _gmean(g), _gmean(g * f.xh)
+    dx = r * (g - m1 - f.xh * m2)
+    # the kernel forms x*c2 and c3 = mean*c2 - rstd*m1 separately: its absolute-value scale of xhat is
+    # rstd (|x| + |mean|), plus the statistics' error
+    xa = r * (f.xg.abs() + f.mu.abs()) + f.dxh
+    ga = gam_a * dz.abs()
+    # f32 sums of pass 1 (S0 = sum dz, S1 = sum dz x per image and channel, any arrangement: at most HW terms in
+    # a chain plus the row / CTA / cluster / slot reductions), the group sums over cpg channels and the ~16
+    # scalar roundings of c2, c3 and the two fmas
+    rows = max(1, 256 // (x.shape[-1] // 8))
+    gb = gamma(f.HW + 2 * rows + 2 * f.cpg + 80) + f.rho_r
+    e_g = gam_a * e_dz
+    d_dx = (r * (e_g + _gmean(e_g) + xa * _gmean(e_g * xa))                 # error of dz
+            + r * (f.dxh * _gmean((g * f.xh).abs()) + f.xh.abs() * _gmean(ga * f.dxh))   # statistics
+            + gb * r * (ga + _gmean(ga) + xa * _gmean(ga * xa)))            # f32 roundings and sums
+    dx_abs = r * (ga + _gmean(ga) + xa * _gmean(ga * xa))
+    out = {}
+    shp = x.shape
+
+    def ug(t):
+        return t.reshape(shp)
+
+    out["dx"] = (ug(dx), ug(d_dx))
+    # dgamma / dbeta: per-image sums as above, then the sum over N images (atomics or the finalize kernel)
+    gr = gamma(f.HW + 2 * rows + N + 128)
+    out["dbeta"] = (dz.sum((0, 1)).reshape(-1), (e_dz.sum((0, 1)) + gr * dz.abs().sum((0, 1))).reshape(-1))
+    out["dgamma"] = ((dz * f.xh).sum((0, 1)).reshape(-1),
+                     (e_dz * xa + dz.abs() * f.dxh).sum((0, 1)).reshape(-1) +
+                     ((gr + f.rho_r) * dz.abs() * xa).sum((0, 1)).reshape(-1))
+    # column sums of dx before any addend and before the bf16 rounding
+    ci = dx.sum(1).reshape(N, -1)
+    d_ci = (d_dx.sum(1) + gamma(f.HW + 2 * rows + 64) * dx_abs.sum(1)).reshape(N, -1)
+    out["csum_img"] = (ci, d_ci)
+    out["csum_tot"] = (ci.sum(0), d_ci.sum(0) + gamma(N + 64) * (dx_abs.sum(1).reshape(N, -1)).sum(0))
+    return out
+
+
+def conv3x3_dgrad_ref(dy, w_hwio):
+    """d/dx of a 3x3 SAME cross-correlation (HWIO weights), NHWC -> (value, delta of the tensor-core engine):
+    K = 9 Cout exact products accumulated in f32 (TC_ADD each), plus <= 16 split-K / epilogue additions."""
+    W = w_hwio.to(torch.float64).permute(3, 2, 0, 1)       # (Cout, Cin, 3, 3)
+    d = dy.to(torch.float64).permute(0, 3, 1, 2)
+    val = Fnn.conv_transpose2d(d, W, padding=1).permute(0, 2, 3, 1)
+    mag = Fnn.conv_transpose2d(d.abs(), W.abs(), padding=1).permute(0, 2, 3, 1)
+    K = 9 * w_hwio.shape[-1]
+    return val, (K + 16) * TC_ADD * mag
+
+
+def conv_gn_backward_ref(x, dy, w_hwio, gamma_, beta_, G, eps):
+    """d/dx of conv3x3(silu(groupnorm(x))) given dy = d/d(conv output).  The data gradient reaches the GroupNorm
+    backward as bf16: either da itself (two-pass path) or dz = da silu'(z) (fused epilogue) is rounded, so the
+    input error is the engine's plus 2^-8 (|da| + its error), scaled by |silu'| <= 1.1 -- the same bound either way."""
+    da, e_da = conv3x3_dgrad_ref(dy, w_hwio)
+    return gn_backward_ref(x, da, gamma_, beta_, G, eps, True, dy_delta=e_da + U_BF16 * 1.1 * (da.abs() + e_da))
+
+
+# ----------------------------------------------------------------------------------------------- RMSNorm
+def rms_forward_ref(x, scale, eps):
+    """y = x rstd scale, rstd = 1/sqrt(mean_c x^2 + eps) per pixel -> (value, delta).
+    rms_fwd_kernel: per lane ceil(C/256) vectors of 8 serial squares, then a 5-level warp tree:
+    D = 8 ceil(C/256) + 5; q/C and + eps (2 roundings), rsqrtf, then two products."""
+    C = x.shape[-1]
+    q = (x * x).mean(-1, keepdim=True)
+    r = 1.0 / torch.sqrt(q + eps)
+    y = x * r * scale
+    rho = gamma(8 * math.ceil(C / 256) + 5 + 2) / 2 + RSQRT + 2 * U32
+    return y, rho * y.abs()
+
+
+def rms_backward_ref(x, dy, scale, eps, npix_per_sweep: int):
+    """dx = rstd (g - xhat mean_c(g xhat)), g = dy scale, xhat = x rstd;  dscale = sum_p dy xhat.
+    -> dict of (value, delta).  rms_bwd_kernel sums mean_c(g xhat) like the forward sums x^2 (D as above, plus
+    the division by C); dscale is a per-warp serial sum over ceil(npix / npix_per_sweep) pixels, 8 warps through
+    shared-memory atomics and one global atomic per block (npix_per_sweep / 8 of them)."""
+    C = x.shape[-1]
+    q = (x * x).mean(-1, keepdim=True)
+    r = 1.0 / torch.sqrt(q + eps)
+    xh = x * r
+    g = dy * scale
+    m = (g * xh).mean(-1, keepdim=True)
+    dx = r * (g - xh * m)
+    rho = gamma(8 * math.ceil(C / 256) + 5 + 2) / 2 + RSQRT + U32
+    gc = gamma(8 * math.ceil(C / 256) + 5 + 1)
+    d_dx = (rho + gc + 4 * U32) * r * (g.abs() + xh.abs() * (g * xh).abs().mean(-1, keepdim=True))
+    npix = x.numel() // C
+    ds = (dy * xh).reshape(-1, C).sum(0)
+    D = math.ceil(npix / npix_per_sweep) + 8 + npix_per_sweep // 8 + 1
+    d_ds = (gamma(D) + rho + U32) * (dy * xh).abs().reshape(-1, C).sum(0)
+    return {"dx": (dx, d_dx), "dscale": (ds, d_ds)}
+
+
+# ----------------------------------------------------------------------------------------------- GEGLU
+GELU_C, GELU_A = math.sqrt(2 / math.pi), 0.044715
+
+
+def _gelu_parts(b):
+    inner = GELU_C * (b + GELU_A * b ** 3)
+    t = torch.tanh(inner)
+    # the f32 argument: b^3 (2 roundings), a b^3, the add, the product by c: 5 roundings on |inner|-scale terms
+    d_inner = 5 * U32 * GELU_C * (b.abs() + GELU_A * b.abs() ** 3)
+    dt = TANH * t.abs() + (1 - t * t) * d_inner                    # error of the kernel's t
+    return inner, t, dt
+
+
+def geglu_forward_ref(u):
+    """u = [lin | gel] (rows, 2 inner) -> g = lin * 0.5 gel (1 + tanh(c (gel + 0.044715 gel^3))) (jax.nn.gelu,
+    approximate=True), with delta: |lin| 0.5 |gel| dt from tanh, plus 3 roundings of the products."""
+    inner = u.shape[1] // 2
+    a, b = u[:, :inner], u[:, inner:]
+    _, t, dt = _gelu_parts(b)
+    gl = 0.5 * b * (1 + t)
+    val = a * gl
+    delta = a.abs() * 0.5 * b.abs() * dt + 3 * U32 * (a * 0.5 * b).abs() * (1 + t.abs())
+    return val, delta
+
+
+def geglu_backward_ref(u, dg):
+    """du = [dg gelu(gel) | dg lin gelu'(gel)], gelu'(b) = (1+t)/2 + b (1-t^2) c (1 + 3 a b^2) / 2, with delta."""
+    inner = u.shape[1] // 2
+    a, b = u[:, :inner], u[:, inner:]
+    _, t, dt = _gelu_parts(b)
+    k = GELU_C * (1 + 3 * GELU_A * b * b)
+    gl = 0.5 * b * (1 + t)
+    gp = 0.5 * (1 + t) + 0.5 * b * (1 - t * t) * k
+    d_lin = dg * gl
+    d_gel = dg * a * gp
+    e_lin = dg.abs() * 0.5 * b.abs() * dt + 3 * U32 * (dg * 0.5 * b).abs() * (1 + t.abs())
+    # d gelu'/dt = 1/2 - b t k; the ~10 roundings of the derivative formula on its absolute-value form
+    gp_abs = 0.5 * (1 + t.abs()) + 0.5 * b.abs() * (1 + t * t) * k
+    e_gel = (dg * a).abs() * ((0.5 - b * t * k).abs() * dt + 12 * U32 * gp_abs)
+    return torch.cat([d_lin, d_gel], 1), torch.cat([e_lin, e_gel], 1)
+
+
+# ----------------------------------------------------------------------------------------------- streaming
+def colsum_ref(x, per_image: bool):
+    x = x.to(torch.float64)
+    return x.sum((1, 2)) if per_image else x.sum((0, 1, 2))
+
+
+def upsample2x_ref(x):
+    return x.repeat_interleave(2, 1).repeat_interleave(2, 2)
+
+
+def upsample2x_bwd_ref(dy):
+    """Adjoint of nearest 2x: each input pixel receives the sum of its 2x2 output block."""
+    N, H2, W2, C = dy.shape
+    return dy.to(torch.float64).reshape(N, H2 // 2, 2, W2 // 2, 2, C).sum((2, 4))

@@ -122,15 +122,19 @@ def test_rmsnorm_fwd_bwd(C):
     assert rel(dx, xr.grad) < 1e-2 and rel(ds, sr.grad) < 5e-3
 
 
-@pytest.mark.parametrize("u8", [True, False])
-@pytest.mark.parametrize("kind", [0, 1, 2])
-def test_diffuse_forward(u8, kind):
+# B = 256, 64x64x3 (BASELINE): B*E/4 = 786,432 four-element items over 8*SMs*256 = 270,336 threads (132 SMs), so
+# the grid-stride loop runs about three times and the per-sample index b changes inside a thread's sweep
+BASELINE_BH = (256, 64)
+
+
+@pytest.mark.parametrize("kind,u8,B,H", [pytest.param(k, u, 5, 16, id=f"{k}-{u}") for k in (0, 1, 2) for u in (True, False)] +
+                         [pytest.param(k, u, *BASELINE_BH, id=f"{k}-{u}-B256") for k in (0, 1, 2) for u in (True, False)])
+def test_diffuse_forward(u8, kind, B, H):
     rng = np.random.default_rng(0)
-    B, H = 5, 16
     img = rng.integers(0, 256, (B, H, H, 3), dtype=np.uint8)
     x0 = img if u8 else img.astype(np.float32)
     eps = rng.standard_normal((B, H, H, 3), dtype=np.float32)
-    sigma = np.array([0.002, 0.3, 1.0, 7.0, 80.0], dtype=np.float32)
+    sigma = np.resize(np.array([0.002, 0.3, 1.0, 7.0, 80.0], dtype=np.float32), B)
     alpha = np.ones(B, np.float32) if kind == 0 else np.sqrt(np.maximum(1 - np.minimum(sigma, 0.99) ** 2, 0)).astype(np.float32)
     c_in, _, _ = R.karras_coeffs(sigma)
     x_t, tgt, mi = ops.diffuse_forward(torch.from_numpy(x0).to(dev), torch.from_numpy(eps).to(dev),
@@ -146,50 +150,50 @@ def test_diffuse_forward(u8, kind):
 
 
 def test_loss_fwd_bwd():
-    rng = np.random.default_rng(1)
-    B, H = 4, 16
-    F, x_t, tg = (rng.standard_normal((B, H, H, 3), dtype=np.float32) for _ in range(3))
-    sigma = np.array([0.01, 0.5, 2.0, 50.0], dtype=np.float32)
-    _, c_out, c_skip = R.karras_coeffs(sigma)
-    w = R.karras_weight(sigma)
-    Ft = torch.from_numpy(F).to(dev)
-    loss, dF = ops.loss_fwd_bwd(Ft, torch.from_numpy(x_t).to(dev), torch.from_numpy(tg).to(dev),
-                                torch.from_numpy(c_out).to(dev), torch.from_numpy(c_skip).to(dev),
-                                torch.from_numpy(w).to(dev))
-    pred = c_out.reshape(-1, 1, 1, 1) * F + c_skip.reshape(-1, 1, 1, 1) * x_t
-    want = R.weighted_l2_loss(pred, tg, w)
-    assert abs(loss.item() - want) / want < 1e-5
-    Fr = torch.from_numpy(F).requires_grad_(True)
-    pr = torch.from_numpy(c_out).view(-1, 1, 1, 1) * Fr + torch.from_numpy(c_skip).view(-1, 1, 1, 1) * torch.from_numpy(x_t)
-    (0.5 * (pr - torch.from_numpy(tg)) ** 2 * torch.from_numpy(w).view(-1, 1, 1, 1)).mean().backward()
-    assert rel(dF, Fr.grad) < 1e-5
+    for B, H in ((4, 16), BASELINE_BH):
+        rng = np.random.default_rng(1)
+        F, x_t, tg = (rng.standard_normal((B, H, H, 3), dtype=np.float32) for _ in range(3))
+        sigma = np.resize(np.array([0.01, 0.5, 2.0, 50.0], dtype=np.float32), B)
+        _, c_out, c_skip = R.karras_coeffs(sigma)
+        w = R.karras_weight(sigma)
+        Ft = torch.from_numpy(F).to(dev)
+        loss, dF = ops.loss_fwd_bwd(Ft, torch.from_numpy(x_t).to(dev), torch.from_numpy(tg).to(dev),
+                                    torch.from_numpy(c_out).to(dev), torch.from_numpy(c_skip).to(dev),
+                                    torch.from_numpy(w).to(dev))
+        pred = c_out.reshape(-1, 1, 1, 1) * F + c_skip.reshape(-1, 1, 1, 1) * x_t
+        want = R.weighted_l2_loss(pred, tg, w)
+        assert abs(loss.item() - want) / want < 1e-5
+        Fr = torch.from_numpy(F).requires_grad_(True)
+        pr = torch.from_numpy(c_out).view(-1, 1, 1, 1) * Fr + torch.from_numpy(c_skip).view(-1, 1, 1, 1) * torch.from_numpy(x_t)
+        (0.5 * (pr - torch.from_numpy(tg)) ** 2 * torch.from_numpy(w).view(-1, 1, 1, 1)).mean().backward()
+        assert rel(dF, Fr.grad) < 1e-5
 
 
 def test_affine_combine_sampler_rules():
-    rng = np.random.default_rng(2)
-    B, H = 3, 8
-    x, x0, noise = (torch.from_numpy(rng.standard_normal((B, H, H, 3), dtype=np.float32)).to(dev) for _ in range(3))
-    cs = np.array([80.0, 3.0, 0.5], dtype=np.float32)
-    ns = np.array([40.0, 1.0, 0.1], dtype=np.float32)
-    one = np.ones(B, np.float32)
-    from flaxdiff_b200.predictors import _affine
-    t = lambda a: torch.from_numpy(a).to(dev)  # noqa: E731
-    dt = ns - cs
-    k = (one * ns - one * cs) / dt
-    g = dt / cs
-    got = _affine([x, x0], [t(1 + g), t(-k * g)])
-    want = R.euler_step(x.cpu().numpy(), x0.cpu().numpy(), one, cs, one, ns)
-    np.testing.assert_allclose(got.cpu().numpy(), want, rtol=2e-5, atol=2e-5)
-    up = (ns ** 2 * (cs ** 2 - ns ** 2) / cs ** 2) ** 0.5
-    down = (ns ** 2 - up ** 2) ** 0.5
-    g2 = (down - cs) / cs
-    got = _affine([x, x0, noise], [t(1 + g2), t(-k * g2), t(up)])
-    want = R.euler_ancestral_step(x.cpu().numpy(), x0.cpu().numpy(), noise.cpu().numpy(), one, cs, one, ns)
-    np.testing.assert_allclose(got.cpu().numpy(), want, rtol=2e-5, atol=2e-5)
-    o1, o2 = _affine([x, x0], [t(one), t(one * 2)], [t(one * 0), t(one * -1)])
-    np.testing.assert_allclose(o2.cpu().numpy(), -x0.cpu().numpy(), rtol=0, atol=0)
-    out, _, _ = ops.affine_combine([x.contiguous()], torch.ones(1, B, device=dev), clip=(-1.0, 1.0))
-    assert out.max().item() <= 1.0 and out.min().item() >= -1.0
+    for B, H in ((3, 8), BASELINE_BH):
+        rng = np.random.default_rng(2)
+        x, x0, noise = (torch.from_numpy(rng.standard_normal((B, H, H, 3), dtype=np.float32)).to(dev) for _ in range(3))
+        cs = np.resize(np.array([80.0, 3.0, 0.5], dtype=np.float32), B)
+        ns = np.resize(np.array([40.0, 1.0, 0.1], dtype=np.float32), B)
+        one = np.ones(B, np.float32)
+        from flaxdiff_b200.predictors import _affine
+        t = lambda a: torch.from_numpy(a).to(dev)  # noqa: E731
+        dt = ns - cs
+        k = (one * ns - one * cs) / dt
+        g = dt / cs
+        got = _affine([x, x0], [t(1 + g), t(-k * g)])
+        want = R.euler_step(x.cpu().numpy(), x0.cpu().numpy(), one, cs, one, ns)
+        np.testing.assert_allclose(got.cpu().numpy(), want, rtol=2e-5, atol=2e-5)
+        up = (ns ** 2 * (cs ** 2 - ns ** 2) / cs ** 2) ** 0.5
+        down = (ns ** 2 - up ** 2) ** 0.5
+        g2 = (down - cs) / cs
+        got = _affine([x, x0, noise], [t(1 + g2), t(-k * g2), t(up)])
+        want = R.euler_ancestral_step(x.cpu().numpy(), x0.cpu().numpy(), noise.cpu().numpy(), one, cs, one, ns)
+        np.testing.assert_allclose(got.cpu().numpy(), want, rtol=2e-5, atol=2e-5)
+        o1, o2 = _affine([x, x0], [t(one), t(one * 2)], [t(one * 0), t(one * -1)])
+        np.testing.assert_allclose(o2.cpu().numpy(), -x0.cpu().numpy(), rtol=0, atol=0)
+        out, _, _ = ops.affine_combine([x.contiguous()], torch.ones(1, B, device=dev), clip=(-1.0, 1.0))
+        assert out.max().item() <= 1.0 and out.min().item() >= -1.0
 
 
 def test_adamw_ema_matches_oracle():
