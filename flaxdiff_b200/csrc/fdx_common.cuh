@@ -117,16 +117,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ----- clusters ----------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
 // ----- wgmma ----------------------------------------------------------------------
 // One warpgroup (four consecutive warps, the first a multiple of four) computes D(64 x N, f32 registers)
 // += A(64 x 16) * B(16 x N), both operands read from shared memory through matrix descriptors.  TA / TB = 1

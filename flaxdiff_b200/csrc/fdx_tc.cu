@@ -530,11 +530,6 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
   const long long pix_blocks = (long long)d.nxb * d.nyb * d.nnb;
 
   if (L.mode != TC_MNMN) {
-    // Round 1 narrowed the column tile until the launch had two waves of tiles; narrower tiles re-read the A
-    // operand once per column block and add rounds.  FDX_TC_BN_V1=1 restores the old rule.
-    static const bool bn_v1 = getenv("FDX_TC_BN_V1") != nullptr;
-    while (bn_v1 && BN > 64 && pix_blocks * ((L.Ncols + BN - 1) / BN) < 2LL * fdx_num_sms())
-      BN /= 2;
     d.nblks = (L.Ncols + BN - 1) / BN;
     d.kchunks = (L.K + kBK - 1) / kBK;
     d.ntiles = (int)(pix_blocks * d.nblks);

@@ -53,10 +53,6 @@ def _attn_width(d: int) -> int:
     return 32 if d <= 32 else 64
 
 
-# 1x1 residual convolutions (ResidualBlock.residual_conv): conv-geometry launches by default, so the layers with
-# 64 / 128 output channels run on the transposed engine; FDX_RES1X1_GEMM=1 restores the flat GEMM launch.
-_RES1X1_GEMM = bool(os.environ.get("FDX_RES1X1_GEMM"))
-_GN_APPLY_V1 = bool(os.environ.get("FDX_GN_APPLY_V1"))
 
 class _SideStream:
     """Weight-gradient kernels have no consumer before the optimizer step, so the backward pass issues them
@@ -107,7 +103,7 @@ class Node:
     def colstats(self):
         """(workspace, channel offset) for a producer's epilogue, or None when the images are too small
         for the fused sums (the consumer then runs the statistics kernel)."""
-        if os.environ.get("FDX_NO_COLSTATS") or self.t.shape[1] * self.t.shape[2] < ops.COLSTATS_MIN_PIXELS:
+        if self.t.shape[1] * self.t.shape[2] < ops.COLSTATS_MIN_PIXELS:
             return None
         root = self.parent if self.parent is not None else self
         if root.cs is None:
@@ -115,24 +111,14 @@ class Node:
         self.cs_ok = True
         return (root.cs, self.coff)
 
-    def stats(self, groups: int) -> torch.Tensor:
-        """GroupNorm statistics of this tensor: from the producers' epilogue sums when all of them
-        contributed, else one pass of fdx_groupnorm_stats."""
+    def norm_apply(self, groups: int, gamma, beta, eps: float, silu: bool):
+        """(GroupNorm(+SiLU) of this tensor, its statistics): ONE launch when every producer's epilogue left its
+        column sums (fdx_groupnorm_apply_cols), else a pass of fdx_groupnorm_stats + apply."""
         done = all(k.cs_ok for k in self.kids) if self.kids else self.cs_ok
         root = self.parent if self.parent is not None else self
         if done and root.cs is not None:
-            return ops.groupnorm_stats_from_cols(root.cs, groups, self.coff, self.t.shape[-1])
-        return ops.groupnorm_stats(self.t, groups)
-
-    def norm_apply(self, groups: int, gamma, beta, eps: float, silu: bool):
-        """(GroupNorm(+SiLU) of this tensor, its statistics): ONE launch when the producers' epilogues left the
-        column sums (fdx_groupnorm_apply_cols), else statistics (from columns or by their own pass) + apply.
-        FDX_GN_APPLY_V1=1 keeps the separate stats_from_cols launch."""
-        done = all(k.cs_ok for k in self.kids) if self.kids else self.cs_ok
-        root = self.parent if self.parent is not None else self
-        if done and root.cs is not None and groups <= 64 and not _GN_APPLY_V1:
             return ops.groupnorm_apply_cols(self.t, groups, root.cs, self.coff, gamma, beta, eps, silu)
-        st = self.stats(groups)
+        st = ops.groupnorm_stats(self.t, groups)
         return ops.groupnorm_apply(self.t, groups, st, gamma, beta, eps, silu), st
 
     def grad_buf(self) -> torch.Tensor:
@@ -541,11 +527,8 @@ class Unet:
         if cin != cout:
             Bn, hh, ww, _ = x.shape
             r = torch.empty((Bn, hh, ww, cout), dtype=BF16, device=x.device)
-            if _RES1X1_GEMM:      # round-1 launch: one flat GEMM over all pixels (pixels-as-M engine)
-                ops.gemm(GEMM_KMN, x, W16[f"{name}/residual_conv/conv/kernel"], r, Bn * hh * ww, cout, cin,
-                         x.stride(2), cout, cout, bias=W[f"{name}/residual_conv/conv/bias"])
-            else:                 # conv geometry: eligible for the transposed engine (8 epilogue warps)
-                ops.conv1x1_fwd(x, W16[f"{name}/residual_conv/conv/kernel"], W[f"{name}/residual_conv/conv/bias"], out=r)
+            # conv geometry: eligible for the transposed engine (8 epilogue warps)
+            ops.conv1x1_fwd(x, W16[f"{name}/residual_conv/conv/kernel"], W[f"{name}/residual_conv/conv/bias"], out=r)
         else:
             r = x
         ops.conv3x3_fwd(a2, W16[f"{name}/conv2/conv/kernel"], W[f"{name}/conv2/conv/bias"], res=r, out=dst.t,
@@ -1034,19 +1017,8 @@ class Unet:
         dx, acc = want(xin)
         gn1 = (dh, W16[f"{name}/conv1/conv/kernel"], x, G, st1, W[f"{name}/{self._n1}/scale"],
                W[f"{name}/{self._n1}/bias"], RES_EPS, Gd[f"{name}/{self._n1}/scale"], Gd[f"{name}/{self._n1}/bias"], dx)
-        if os.environ.get("FDX_RES_BWD_V1"):        # round-1 order (GroupNorm backward, then the residual pass)
-            ops.conv_dgrad_groupnorm_bwd(*gn1, acc)
-            if cin != cout:
-                ops.gemm(GEMM_KK, dout, W16[kres + "kernel"].view(cin, cout), dx, M, cin, cout, dout.stride(2), cout,
-                         dx.stride(2), res=dx, r_ld=dx.stride(2))
-            else:
-                ops.act_add(dx, dout, dx)
-        elif cin != cout:
-            if _RES1X1_GEMM:
-                ops.gemm(GEMM_KK, dout, W16[kres + "kernel"].view(cin, cout), dx, M, cin, cout, dout.stride(2), cout,
-                         dx.stride(2), res=dx if acc else None, r_ld=dx.stride(2) if acc else 0)
-            else:
-                ops.conv1x1_dgrad(dout, W16[kres + "kernel"], dx, accumulate=acc)
+        if cin != cout:
+            ops.conv1x1_dgrad(dout, W16[kres + "kernel"], dx, accumulate=acc)
             ops.conv_dgrad_groupnorm_bwd(*gn1, True)
         elif acc:
             ops.conv_dgrad_groupnorm_bwd(*gn1, True)

@@ -7,7 +7,6 @@ Python: each wrapper marshals pointers, shapes and the current CUDA stream.
 from __future__ import annotations
 
 import ctypes
-import os
 from typing import Optional
 
 import torch
@@ -183,7 +182,7 @@ def groupnorm_apply_cols(x, groups, cs: "ColStats", c0: int, gamma, beta, eps: f
 def groupnorm_bwd(x, dy, groups, stats, gamma, beta, eps, silu, dgamma, dbeta, dx,
                   accumulate: bool = False, csum_img=None, csum_tot=None, addend=None) -> torch.Tensor:
     """dx (+)= d/dx GroupNorm(+SiLU); `addend`: dx = d/dx + addend (another tensor of the same shape)."""
-    red = torch.empty(2 * x.shape[0] * (x.shape[-1] + groups), dtype=torch.float32, device=x.device)
+    red = torch.empty(2 * x.shape[0] * groups, dtype=torch.float32, device=x.device)
     if addend is not None:
         assert not accumulate
         check(load().fdx_groupnorm_bwd_add(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")),
@@ -232,19 +231,18 @@ def conv3x3_dgrad_gn(dy: torch.Tensor, w_hwio: torch.Tensor, dz: torch.Tensor, x
 
 def groupnorm_bwd_dz(x, dz, groups, stats, gamma, eps, ws_slots, dgamma, dbeta, dx,
                      accumulate: bool = False, csum_img=None, csum_tot=None, addend=None) -> torch.Tensor:
-    red = torch.empty(2 * x.shape[0] * (x.shape[-1] + groups), dtype=torch.float32, device=x.device)
     if addend is not None:
         assert not accumulate, "groupnorm_bwd_dz: addend and accumulate are exclusive"
         check(load().fdx_groupnorm_bwd_dz_add(ctypes.byref(act(x, "x")), ctypes.byref(act(dz, "dz")),
                                               ctypes.c_int(groups), ptr(stats), ptr(gamma), ctypes.c_float(eps),
-                                              ptr(ws_slots), ctypes.c_int(ws_slots.shape[0]), ptr(red), ptr(dgamma),
+                                              ptr(ws_slots), ctypes.c_int(ws_slots.shape[0]), None, ptr(dgamma),
                                               ptr(dbeta), ctypes.byref(act(dx, "dx")),
                                               ctypes.byref(act(addend, "addend")), ptr(csum_img), ptr(csum_tot),
                                               stream_ptr()), "groupnorm_bwd_dz_add")
         return dx
     check(load().fdx_groupnorm_bwd_dz(ctypes.byref(act(x, "x")), ctypes.byref(act(dz, "dz")),
                                       ctypes.c_int(groups), ptr(stats), ptr(gamma), ctypes.c_float(eps),
-                                      ptr(ws_slots), ctypes.c_int(ws_slots.shape[0]), ptr(red), ptr(dgamma),
+                                      ptr(ws_slots), ctypes.c_int(ws_slots.shape[0]), None, ptr(dgamma),
                                       ptr(dbeta), ctypes.byref(act(dx, "dx")),
                                       ctypes.c_int(1 if accumulate else 0), ptr(csum_img), ptr(csum_tot),
                                       stream_ptr()), "groupnorm_bwd_dz")
@@ -265,15 +263,11 @@ def conv_dgrad_groupnorm_bwd(dy, w_hwio, x, groups, stats, gamma, beta, eps, dga
     """d/dx of conv3x3(silu(groupnorm(x))) given dy = d/d(conv output): the data gradient with the first pass
     of the GroupNorm backward in its epilogue (dz = dy * silu'(z), sum dz, sum dz*x) where that convolution runs
     on the transposed engine, then ONE pass over x and dz; elsewhere data gradient + the two-pass GroupNorm
-    backward.  FDX_GN_FUSE=0: never fused; FDX_GN_FUSE=1: fused wherever an image has >= 128 pixels (also on the
-    pixels-as-M engine)."""
+    backward.  `fused=True` fuses wherever an image has >= 128 pixels (also on the pixels-as-M engine),
+    `fused=False` never."""
     da = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
     if fused is None:
-        env = os.environ.get("FDX_GN_FUSE")
-        if env is None or env == "":
-            fused = _gn_fuse_default(x, dy)
-        else:
-            fused = env != "0" and x.shape[1] * x.shape[2] >= GN_FUSE_MIN_PIXELS
+        fused = _gn_fuse_default(x, dy)
     if fused and x.shape[1] * x.shape[2] >= GN_FUSE_MIN_PIXELS:
         ab = groupnorm_coeffs(stats, gamma, beta, x.shape[1] * x.shape[2], eps)
         ws = conv3x3_dgrad_gn(dy, w_hwio, da, x, ab)

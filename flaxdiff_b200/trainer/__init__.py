@@ -469,7 +469,10 @@ class GeneralDiffusionTrainer:
         self._comm = get_comm() if (self.distributed_training and self.device.type == "cuda") else None
         nb = grad_buckets if grad_buckets is not None else int(os.environ.get("FDX_GRAD_BUCKETS", "4"))
         self._exchange = GradExchange(self._comm, self._gbuf, nb) if self._comm is not None else None
-        self._overlap = self._exchange is not None and os.environ.get("FDX_NO_DP_OVERLAP", "0") in ("", "0")
+        # Bucketed all-reduce launched from the backward inside the training graph is opt-in (FDX_NO_DP_OVERLAP=0):
+        # the NCCL CTAs take SMs from the persistent one-CTA-per-SM tensor-core kernels, which then need a second
+        # wave.  By default the gradients are exchanged in one call after the backward.
+        self._overlap = self._exchange is not None and os.environ.get("FDX_NO_DP_OVERLAP", "1") in ("", "0")
 
     # ------------------------------------------------------------------ state
     def generate_states(self, optimizer, rngs, existing_state=None, existing_best_state=None, model=None,

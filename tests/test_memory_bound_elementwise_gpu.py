@@ -6,9 +6,8 @@ channel slots of a wider buffer have sentinel neighbours that must come back bit
 reference runs on the device.  Copies, single bf16 adds and casts are checked bit-exactly; everything else
 against the per-element bound of elementwise_ref (derived there, never tuned to a run).
 
-The GroupNorm backward arrangement is selected once per process (FDX_GN_FINALIZE, FDX_GN_2PASS, FDX_GN_PIPE) and
-gn_grid reads FDX_GN_WAVES once: test_gn_arrangements_in_child_processes runs the GroupNorm cases again in a
-child pytest process for each setting."""
+gn_grid reads FDX_GN_WAVES once per process: test_gn_arrangements_in_child_processes runs the GroupNorm cases again
+in child pytest processes with other grid sizes (FDX_GN_WAVES = 0, 1, 8 and an uncapped grid)."""
 import ctypes
 import math
 import os
@@ -98,7 +97,6 @@ GN_SHAPES = [  # (N, H, W, C, G): ragged and tiny images, every channel count of
     (3, 7, 9, 64, 8), (2, 1, 1, 64, 8), (3, 32, 32, 64, 8), (4, 3, 5, 192, 8), (2, 32, 48, 192, 8),
     (2, 16, 16, 320, 8), (3, 1, 1, 512, 8), (2, 9, 7, 512, 16), (3, 8, 8, 256, 32), (2, 8, 8, 768, 8),
     (2, 16, 16, 1024, 8), (2, 7, 9, 1536, 8), (2, 3, 5, 2048, 8), (2, 32, 32, 2048, 8),
-    # more images than a pipeline stage holds (FDX_GN_PIPE=2: 4 MB per image, 6 per ~24 MB stage, 3 stages);
     # with 132 SMs gn_grid caps apply at 82 CTAs per image (2 iterations) and the backward at 49 (4 iterations)
     (16, 128, 128, 64, 8),
 ]
@@ -268,14 +266,17 @@ def test_groupnorm_conv_dgrad_fused_elementwise(N, H, W, C, Co):
                 R.assert_elementwise(got, v, R.f32_bound(v, d), "fused " + name)
 
 
-@pytest.mark.parametrize("env_kv", [{"FDX_GN_FINALIZE": "1"}, {"FDX_GN_2PASS": "0"},
-                                    {"FDX_GN_2PASS": "0", "FDX_GN_PIPE": "2"}, {"FDX_GN_WAVES": "0"}],
-                         ids=["separate-finalize", "cluster", "pipelined", "one-cta-per-image"])
+@pytest.mark.parametrize("env_kv", [{"FDX_GN_WAVES": "0"}, {"FDX_GN_WAVES": "1"}, {"FDX_GN_WAVES": "8"},
+                                    {"FDX_GN_WAVES": "1000"}],
+                         ids=["one-cta-per-image", "one-wave", "eight-waves", "uncapped"])
 def test_gn_arrangements_in_child_processes(env_kv):
-    """Each setting is read once per process: run every GroupNorm case above in a child with it set.
+    """The grid size is read once per process: run every GroupNorm case above in a child with it set.
     FDX_GN_WAVES=0 caps gn_grid at one CTA per image, so the pixel loops of the apply and both backward passes
     iterate ceil(HW / (rows * unroll)) times: 128 (apply) and 171 (backward) at 128x128x64, 39 and 52 at
-    32x48x192; _gn_check_all asserts >= 2 for every capped shape."""
+    32x48x192; _gn_check_all asserts >= 2 for every capped shape.  One and eight waves split the pixels of an image
+    over other CTA counts than the default two.  With the uncapped grid every CTA runs at most one loop iteration, so
+    the most CTAs add partial sums into the same red / dgamma / dbeta / column-sum entries (171 per image for the
+    backward at 128x128x64)."""
     if IN_CHILD:
         pytest.skip("already a child")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
