@@ -856,7 +856,26 @@ int check_desc(const fdx_attn_desc* a, const char* who) {
   FDX_REQUIRE(a->dh == 32 || a->dh == 64 || a->dh == 128,
               "%s: head width %d (stored) must be 32 or 64, or 128 - zero-pad narrower heads", who, a->dh);
   FDX_REQUIRE((a->heads * a->dh) % 64 == 0, "%s: heads * dh must be a multiple of 64", who);
-  FDX_REQUIRE(a->q_ld % 8 == 0 && a->k_ld % 8 == 0 && a->v_ld % 8 == 0, "%s: row strides must be multiples of 8", who);
+  FDX_REQUIRE(a->q_ld % 8 == 0, "%s: q_ld must be a multiple of 8 elements", who);
+  FDX_REQUIRE(a->k_ld % 8 == 0, "%s: k_ld must be a multiple of 8 elements", who);
+  FDX_REQUIRE(a->v_ld % 8 == 0, "%s: v_ld must be a multiple of 8 elements", who);
+  FDX_REQUIRE(a->q_bs % 8 == 0, "%s: q_bs must be a multiple of 8 elements", who);
+  FDX_REQUIRE(a->k_bs % 8 == 0, "%s: k_bs must be a multiple of 8 elements", who);
+  FDX_REQUIRE(a->v_bs % 8 == 0, "%s: v_bs must be a multiple of 8 elements", who);
+  FDX_REQUIRE((reinterpret_cast<uintptr_t>(a->q) & 15) == 0, "%s: q must be 16-byte aligned", who);
+  FDX_REQUIRE((reinterpret_cast<uintptr_t>(a->k) & 15) == 0, "%s: k must be 16-byte aligned", who);
+  FDX_REQUIRE((reinterpret_cast<uintptr_t>(a->v) & 15) == 0, "%s: v must be 16-byte aligned", who);
+  return FDX_OK;
+}
+
+// o, d_o, dq, dk, dv are written / read with 16-byte vector accesses (and TMA needs 16-byte aligned rows): the
+// base pointer must be 16-byte aligned and both strides multiples of 8 bf16 elements, or some row starts off a
+// 16-byte boundary and the access faults
+int check_io(const void* ptr, long long ld, long long bs, const char* name, const char* ld_name, const char* bs_name,
+             const char* who) {
+  FDX_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "%s: %s must be 16-byte aligned", who, name);
+  FDX_REQUIRE(ld % 8 == 0, "%s: %s must be a multiple of 8 elements", who, ld_name);
+  FDX_REQUIRE(bs % 8 == 0, "%s: %s must be a multiple of 8 elements", who, bs_name);
   return FDX_OK;
 }
 
@@ -868,6 +887,7 @@ int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
   int s = check_desc(a, "attention_fwd");
   if (s != FDX_OK) return s;
   FDX_REQUIRE(a->o, "attention_fwd: null output");
+  if ((s = check_io(a->o, a->o_ld, a->o_bs, "o", "o_ld", "o_bs", "attention_fwd")) != FDX_OK) return s;
   const int hd = a->heads * a->dh;
   CUtensorMap mQ, mK, mV;
   if ((s = make_map(&mQ, a->q, hd, a->L, a->B, a->q_ld, a->q_bs)) != FDX_OK) return s;
@@ -931,6 +951,12 @@ int fdx_attention_bwd(const fdx_attn_desc* a, void* stream) {
   int s = check_desc(a, "attention_bwd");
   if (s != FDX_OK) return s;
   FDX_REQUIRE(a->o && a->d_o && a->lse && a->dvec_ws && a->dq && a->dk && a->dv, "attention_bwd: null pointer");
+  const char* who = "attention_bwd";
+  if ((s = check_io(a->o, a->o_ld, a->o_bs, "o", "o_ld", "o_bs", who)) != FDX_OK) return s;
+  if ((s = check_io(a->d_o, a->do_ld, a->do_bs, "d_o", "do_ld", "do_bs", who)) != FDX_OK) return s;
+  if ((s = check_io(a->dq, a->dq_ld, a->dq_bs, "dq", "dq_ld", "dq_bs", who)) != FDX_OK) return s;
+  if ((s = check_io(a->dk, a->dk_ld, a->dk_bs, "dk", "dk_ld", "dk_bs", who)) != FDX_OK) return s;
+  if ((s = check_io(a->dv, a->dv_ld, a->dv_bs, "dv", "dv_ld", "dv_bs", who)) != FDX_OK) return s;
   const int hd = a->heads * a->dh;
   CUtensorMap mQ, mK, mV, mDO;
   if ((s = make_map(&mQ, a->q, hd, a->L, a->B, a->q_ld, a->q_bs)) != FDX_OK) return s;

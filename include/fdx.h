@@ -313,7 +313,9 @@ int fdx_geglu_bwd(const void* u_bf16, const void* dg_bf16, long long rows, int i
  * backward under jax.value_and_grad (trainer/general_diffusion_trainer.py:321).  The logits and probabilities
  * never reach HBM: flash-style wgmma kernels with S in registers and P in shared memory; the backward recomputes
  * them from `lse` (two kernels: dQ per query tile, dK + dV per key block; deterministic, no atomics).
- * Tensors: bf16 [B][rows][heads*dh], `*_ld` = elements between rows, `*_bs` = elements between images;
+ * Tensors: bf16 [B][rows][heads*dh], `*_ld` = elements between rows, `*_bs` = elements between images.  Every
+ * `*_ld` and `*_bs` must be a multiple of 8 and q, k, v, o, d_o, dq, dk, dv 16-byte aligned (TMA boxes and
+ * 16-byte vector accesses); otherwise FDX_ERR_INVALID_ARG, naming the field, before anything is launched.
  * dh (as STORED) is 32, 64 or 128 - narrower heads are zero-padded by the caller, `scale` = 1/sqrt(true width).
  * lse: f32 [B][heads][L] (written by fwd, read by bwd); dvec_ws: f32 [B][heads][L] scratch (bwd). */
 typedef struct fdx_attn_desc {

@@ -1,5 +1,5 @@
 """Float64 references of the memory-bound kernels (GroupNorm, RMSNorm, GEGLU, column sums, nearest 2x upsample)
-and an element-wise comparator whose tolerance is derived, element by element, from the kernels' arithmetic.
+and of the fused attention, and an element-wise comparator whose tolerance is derived, element by element, from the kernels' arithmetic.
 
 Every reference takes the same bf16 values the kernel reads (as float64 tensors, on any device) and returns the
 exact result together with `delta`: a first-order bound on how far the kernel's f32 arithmetic can be from it
@@ -334,3 +334,125 @@ def upsample2x_bwd_ref(dy):
     """Adjoint of nearest 2x: each input pixel receives the sum of its 2x2 output block."""
     N, H2, W2, C = dy.shape
     return dy.to(torch.float64).reshape(N, H2 // 2, 2, W2 // 2, 2, C).sum((2, 4))
+
+
+# ----------------------------------------------------------------------------------------------- attention
+# ex2.approx.ftz.f32: at most 2 ulp of the result over the full range (PTX ISA, ex2; the figure behind __expf's
+# 2 + 1.173 |x| ulp in the CUDA C Programming Guide), i.e. 4u relative.  Subnormal results flush to 0: an absolute
+# error below FTZ on a weight that is at most 1 against a row sum that is at least 1.
+EX2 = 4 * U32
+FTZ = 2.0 ** -126
+LOGF = 2 * U32               # logf: 1 ulp (CUDA C Programming Guide, Mathematical Functions), 2u relative
+
+
+def _attn_rows(q, k, v, dO, sc):
+    """One (image, head) and a chunk of its query rows: q, dO (R, dh), k, v (Lk, dh), float64.  -> dict of the
+    exact forward / backward pieces and their bounds; dk / dv are this chunk's share of the sums over queries."""
+    R, dh = q.shape
+    Lk = k.shape[0]
+    nblk = math.ceil(Lk / 128)
+    Lkp = 128 * nblk                     # keys of the zero-filled key blocks: the depth of every sum over keys
+    ka, va = k.abs(), v.abs()
+    S = q @ k.T
+    t = sc * S
+    tmax = t.amax(1, keepdim=True)
+    e = torch.exp(t - tmax)
+    lsum = e.sum(1, keepdim=True)
+    lse = tmax + torch.log(lsum)
+    P = e / lsum
+    O = P @ v
+    # S = Q K^T: exact bf16 products, an f32 wgmma chain of dh additions
+    es = sc * dh * TC_ADD * (q.abs() @ ka.T)
+    # Relative error of each key's weight 2^x, x = fmaf(s, scale_log2, -m), shared by the numerator (acc) and the
+    # denominator (l):
+    #   S error (es); scale_log2 = fl(scale fl(log2 e)) is 2u off, on |t|; the fma rounds once on
+    #   |x| <= log2e (tmax - t), m being the running maximum (m <= the final one, t log2e <= m); ex2: EX2.
+    #   corr = ex2(m_old - m_new) scales acc and l by the same factor: its error is a relative error of the weights
+    #   of the earlier blocks' keys, shared by numerator and denominator, and is counted here once -- EX2 per
+    #   block and the rounding of m_old - m_new, whose sum over the later blocks is <= log2e (tmax - t).
+    eta = es + 2 * U32 * t.abs() + 2 * U32 * (tmax - t) + nblk * EX2
+    Pe = P * eta
+    # O = sum bf16(p) v / sum p (l from the unrounded p):
+    #   a weight error moves O by sum_k P_k eta_k (v_k - O) <= (P eta) |v| + |O| sum_k P eta;
+    #   P rounded to bf16 for the PV MMA only: U_BF16 sum P |v| (the dominant term);
+    #   PV accumulated by wgmma over every key of every block (Lkp terms, TC_ADD each) and the acc * corr + O_j
+    #   chain across blocks (gamma(nblk));  l: an f32 sum of <= Lkp terms, the block combine and two quad
+    #   shuffles (dh = 128), relative gamma(Lkp + nblk + 2) since every term is positive;
+    #   1 / l and acc * inv: 2u.  Flushed weights: FTZ per key.
+    eps_l = gamma(Lkp + nblk + 2)
+    spa = P @ va
+    d_o = (Pe @ va + O.abs() * Pe.sum(1, keepdim=True)
+           + (U_BF16 + TC_ADD * Lkp + gamma(nblk) + eps_l + 2 * U32) * spa + FTZ * Lk * va.amax(0))
+    # lse = m ln2 + logf(l): m's own rounding cancels against the -m inside every exponent; the weight errors
+    # (without the bf16 rounding) and l's sum error move log l; logf 1 ulp of log l; fl(ln 2) and the product m ln2
+    # 2u on |tmax| (the f32 rounding of the sum is f32_bound's)
+    d_lse = Pe.sum(1) + eps_l + LOGF * torch.log(lsum).squeeze(1) + 2 * U32 * tmax.abs().squeeze(1)
+    out = {"o": (O, d_o), "lse": (lse.squeeze(1), d_lse)}
+    if dO is None:
+        return out
+    # D = rowsum(dO o O) from the kernel's bf16 O (its bound ob), a serial f32 fma chain of dh terms
+    ob = bf16_bound(O, d_o)
+    dOa = dO.abs()
+    D = (dO * O).sum(1, keepdim=True)
+    e_D = (dOa * ob).sum(1, keepdim=True) + gamma(dh) * (dOa * (O.abs() + ob)).sum(1, keepdim=True)
+    # dP = dO V^T: an f32 wgmma chain of dh additions
+    dP = dO @ v.T
+    e_dP = dh * TC_ADD * (dOa @ va.T)
+    # P recomputed from the kernel's lse: p = ex2(fmaf(s, scale_log2, -fl(lse fl(log2 e)))); relative error from S,
+    # scale_log2 (2u |t|), the kernel's lse (its f32 bound), fl(log2 e) and the product (2u |lse|), the fma's one
+    # rounding on |x| = log2e |t - lse| and ex2; plus FTZ absolute
+    lse_b = f32_bound(lse, d_lse.unsqueeze(1))
+    eps_p = es + 2 * U32 * t.abs() + lse_b + 2 * U32 * lse.abs() + U32 * (t - lse).abs() + EX2
+    ep = P * eps_p + FTZ
+    # dS = p fmaf(dP, scale, -fl(D scale)): exact dS = P g, g = scale (dP - D); the fma and the product round once
+    # each; dS rounded to bf16 for the output GEMMs
+    g = sc * (dP - D)
+    e_g = sc * (e_dP + e_D + U32 * D.abs()) + U32 * g.abs()
+    dS = P * g
+    e_dS = ep * g.abs() + P * e_g + U32 * dS.abs()
+    dSa = dS.abs() + e_dS
+    e_dSb = e_dS + U_BF16 * dSa
+    # the output GEMMs: dQ = dS K accumulates over every key block (Lkp terms); dK = dS^T Q and dV = bf16(P)^T dO
+    # over every query tile -- their depth is added by the caller, which knows L; here the sums of |terms|
+    Pa = P + ep
+    e_Pb = ep + U_BF16 * Pa
+    out["dq"] = (dS @ k, e_dSb @ ka + TC_ADD * Lkp * (dSa @ ka))
+    out["dk"] = (dS.T @ q, e_dSb.T @ q.abs(), dSa.T @ q.abs())
+    out["dv"] = (P.T @ dO, e_Pb.T @ dOa, Pa.T @ dOa)
+    return out
+
+
+def attention_ref(q, k, v, heads: int, dh: int, scale: float, d_o=None, max_elems: int = 1 << 22):
+    """Closed-form float64 softmax attention of fdx_attention_fwd / _bwd (o = softmax(q k^T scale) v per (image,
+    head); dS = P o (dP - D) scale, dQ = dS K, dK = dS^T Q, dV = P^T dO).  q, d_o: (B, L, heads dh), k, v: (B, Lk,
+    heads dh), the bf16 values as float64 on any device; `scale` as the f32 the kernel receives.  Runs per (image,
+    head) in chunks of at most `max_elems` (query, key) pairs.  -> dict of (value, delta): o (B, L, HD), lse (B,
+    heads, L) and, with d_o, dq (B, L, HD), dk, dv (B, Lk, HD).  Compare o, dq, dk, dv with bf16_bound, lse with
+    f32_bound."""
+    B, L, HD = q.shape
+    Lk = k.shape[1]
+    sc = float(torch.tensor(scale, dtype=torch.float32))
+    Lp = 128 * math.ceil(L / 128)       # queries of the zero-filled query tiles: the depth of the sums over queries
+    z = lambda *s: torch.zeros(*s, dtype=torch.float64, device=q.device)  # noqa: E731
+    res = {"o": (z(B, L, HD), z(B, L, HD)), "lse": (z(B, heads, L), z(B, heads, L))}
+    if d_o is not None:
+        res.update({n: (z(B, r, HD), z(B, r, HD)) for n, r in (("dq", L), ("dk", Lk), ("dv", Lk))})
+    R = max(1, max_elems // Lk)
+    for b in range(B):
+        for h in range(heads):
+            cs = slice(h * dh, (h + 1) * dh)
+            kh, vh = k[b, :, cs], v[b, :, cs]
+            acc = {n: [z(Lk, dh), z(Lk, dh), z(Lk, dh)] for n in ("dk", "dv")} if d_o is not None else {}
+            for r0 in range(0, L, R):
+                rs = slice(r0, min(L, r0 + R))
+                out = _attn_rows(q[b, rs, cs], kh, vh, None if d_o is None else d_o[b, rs, cs], sc)
+                for n in ("o", "dq") if d_o is not None else ("o",):
+                    res[n][0][b, rs, cs], res[n][1][b, rs, cs] = out[n]
+                res["lse"][0][b, h, rs], res["lse"][1][b, h, rs] = out["lse"]
+                for n in acc:
+                    for i in range(3):
+                        acc[n][i] += out[n][i]
+            for n in acc:
+                val, err, mag = acc[n]
+                res[n][0][b, :, cs], res[n][1][b, :, cs] = val, err + TC_ADD * Lp * mag
+    return res

@@ -50,6 +50,61 @@ def test_ops_refuse_cpu_tensors(lib):
         ops.groupnorm_stats(x, 8)
 
 
+_ATTN_CHILD = r"""
+import ctypes, json, sys
+from flaxdiff_b200 import _lib
+lib = _lib.load()
+base = 1 << 40                                   # fake, 16-byte aligned addresses: nothing is ever dereferenced
+B, heads, dh, L, Lk = 2, 8, 64, 100, 77
+HD = heads * dh
+
+
+def desc():
+    a = _lib.fdx_attn_desc()
+    a.B, a.heads, a.L, a.Lk, a.dh, a.scale = B, heads, L, Lk, dh, 0.125
+    for i, (t, rows) in enumerate((("q", L), ("k", Lk), ("v", Lk), ("o", L), ("do", L), ("dq", L), ("dk", Lk),
+                                   ("dv", Lk))):
+        setattr(a, "d_o" if t == "do" else t, base + i * (1 << 30))
+        setattr(a, t + "_ld", HD)
+        setattr(a, t + "_bs", rows * HD)
+    a.lse, a.dvec_ws = base + (9 << 30), base + (10 << 30)
+    return a
+
+
+out = []
+for entry, field, value in json.loads(sys.argv[1]):
+    a = desc()
+    setattr(a, field, (base + value) if value < 16 else value)
+    fn = lib.fdx_attention_fwd if entry == "fwd" else lib.fdx_attention_bwd
+    st = fn(ctypes.byref(a), None)
+    out.append([st, lib.fdx_last_error().decode()])
+print(json.dumps(out))
+"""
+
+
+def test_attention_rejects_misaligned_strides_and_pointers(lib):
+    """fdx_attention_fwd / _bwd refuse, naming the field, every row / batch stride that is not a multiple of
+    8 elements and every tensor pointer off a 16-byte boundary: the kernels access o, d_o, dq, dk, dv with
+    16-byte (and 4-byte) vector loads and stores, and TMA reads q, k, v, d_o in 16-byte units.  The calls run in
+    a child process that sees no GPU, on fake addresses: a check that let one through could launch nothing."""
+    import json
+    import subprocess
+    import sys
+    cases = []
+    for entry, tensors in (("fwd", ("q", "k", "v", "o")), ("bwd", ("q", "k", "v", "o", "do", "dq", "dk", "dv"))):
+        for t in tensors:
+            cases += [(entry, t + "_ld", 8 * 64 + 4), (entry, t + "_bs", 100 * 8 * 64 + 2)]
+            cases.append((entry, "d_o" if t == "do" else t, 8))          # base + 8 bytes: 8- but not 16-aligned
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    r = subprocess.run([sys.executable, "-c", _ATTN_CHILD, json.dumps(cases)], capture_output=True, text=True,
+                       env=env, cwd=ROOT, timeout=300)
+    assert r.returncode == 0, r.stderr[-3000:]
+    res = json.loads(r.stdout.strip().splitlines()[-1])
+    for (entry, field, _), (status, msg) in zip(cases, res):
+        who = "attention_fwd" if entry == "fwd" else "attention_bwd"
+        assert status == -1 and msg.startswith(f"{who}: {field} must be"), (entry, field, status, msg)
+
+
 def test_product_does_not_import_oracle():
     """The oracle is test infrastructure: nothing under flaxdiff_b200/ may reference it."""
     for dp, _, fs in os.walk(os.path.join(ROOT, "flaxdiff_b200")):

@@ -171,3 +171,212 @@ def test_comparator_rejects_what_relative_l2_accepts():
     nan[0, 0, 0, 0] = math.nan                                  # an element left at its NaN prefill
     with pytest.raises(AssertionError, match="1 of"):
         R.assert_elementwise(nan, y, bound)
+
+
+# ----------------------------------------------------------------------------------------------- attention
+LOG2E32 = float(torch.tensor(math.log2(math.e), dtype=torch.float32))
+LN2_32 = float(torch.tensor(math.log(2), dtype=torch.float32))
+
+
+def _f32(t):
+    return t.to(torch.float64).float()
+
+
+def _ex2(x):
+    """ex2.ftz in f32: subnormal results flush to 0."""
+    y = torch.exp2(x)
+    return torch.where(y < 2.0 ** -126, torch.zeros_like(y), y)
+
+
+def _attn_inputs(B, heads, L, Lk, dh, d_true, regime, seed=0):
+    """bf16 q, k, v, dO (as float64) whose logits sc q.k follow `regime`."""
+    g = torch.Generator().manual_seed(seed)
+
+    def rn(rows, s=1.0):
+        return torch.randn(B, rows, heads, dh, generator=g, dtype=torch.float64) * s
+    q, k, v, dO = rn(L), rn(Lk), rn(Lk), rn(L)
+    e = torch.zeros(dh, dtype=torch.float64)
+    e[0] = 1.0
+    root = math.sqrt(d_true)                         # sc * root = 1: a logit unit per unit along e
+    kpos = torch.arange(Lk, dtype=torch.float64).view(1, Lk, 1, 1) / 128
+    if regime == "random":
+        q = q * 1.5
+    elif regime == "rising":                         # every key block holds a larger maximum: each one rescales
+        q, k = 0.5 * q + root * e, 0.5 * k + 3 * kpos * e
+    elif regime == "first_max":                      # the first key block holds the maximum
+        q, k = 0.5 * q + root * e, 0.5 * k + 3 * (Lk / 128 - kpos) * e
+    elif regime == "one_hot":                        # logit spread ~40: most exponentials flush to 0
+        q = 40 * q
+    elif regime == "negative":                       # every valid logit about -30: a leaked logit 0 would dominate
+        q, k = 0.1 * q - 6 * root * e, 0.1 * k + 5 * e
+    elif regime == "constant":
+        q = torch.zeros_like(q)
+    else:
+        raise ValueError(regime)
+    out = []
+    for t in (q, k, v, dO):
+        t = t.clone()
+        t[..., d_true:] = 0
+        out.append(_bf(t.reshape(t.shape[0], t.shape[1], heads * dh)))
+    return out
+
+
+def _attn_emulate(q, k, v, dO, heads, dh, scale, leak=False, drop_tile=None, lse_off=None):
+    """f32 emulation of fdx_attn.cu's arithmetic per (image, head): 128-key blocks with zero-filled, masked tail
+    keys, the online maximum and corr, P rounded to bf16 for PV with l from the unrounded p, D from the bf16 O,
+    and in the backward P recomputed from the emulated lse, bf16 P and dS.  Planted defects: `leak` counts one
+    zero-filled tail key in l; `drop_tile` = t drops query tile t's contribution to dK / dV of the last key in
+    head 0;
+    `lse_off` = (row, offset) recomputes that row's P from lse + offset."""
+    B, L, HD = q.shape
+    Lk = k.shape[1]
+    sc = float(torch.tensor(scale, dtype=torch.float32))
+    sl2 = float(torch.tensor(sc * LOG2E32, dtype=torch.float32))
+    nblk = math.ceil(Lk / 128)
+    o, lse = torch.zeros(B, L, HD), torch.zeros(B, heads, L)
+    dq, dk, dv = torch.zeros(B, L, HD), torch.zeros(B, Lk, HD), torch.zeros(B, Lk, HD)
+    for b in range(B):
+        for h in range(heads):
+            cs = slice(h * dh, (h + 1) * dh)
+            qh, kh, vh, dOh = (t[b, :, cs].float() for t in (q, k, v, dO))
+            kp = torch.zeros(128 * nblk, dh)
+            vp = torch.zeros(128 * nblk, dh)
+            kp[:Lk], vp[:Lk] = kh, vh
+            m = torch.full((L, 1), -math.inf)
+            l, acc = torch.zeros(L, 1), torch.zeros(L, dh)
+            for j in range(nblk):
+                kb, vb = kp[128 * j:128 * j + 128], vp[128 * j:128 * j + 128]
+                S = qh @ kb.T
+                valid = torch.arange(128) < Lk - 128 * j
+                mx = torch.where(valid, S, torch.full_like(S, -math.inf)).amax(1, keepdim=True)
+                m_new = torch.maximum(m, _f32(mx.double() * sl2))
+                corr = _ex2(_f32(m.double() - m_new.double()))
+                pe = _ex2(_f32(S.double() * sl2 - m_new.double()))
+                pe = torch.where(valid, pe, torch.zeros_like(pe))
+                rs = pe.sum(1, keepdim=True)
+                if leak and j == nblk - 1 and not valid.all():
+                    rs = rs + _ex2(-m_new)                       # a zero-filled key: logit 0 counted in l
+                Oj = pe.bfloat16().float() @ vb
+                l = _f32(l.double() * corr.double() + rs.double())
+                acc = _f32(acc.double() * corr.double() + Oj.double())
+                m = m_new
+            ob = (acc * (1 / l)).bfloat16().float()
+            o[b, :, cs] = ob
+            lse_h = _f32(_f32(m.double() * LN2_32).double() + torch.log(l.double()))
+            lse[b, h] = lse_h.squeeze(1)
+            # backward, fed the emulated o and lse
+            D = (dOh * ob).sum(1, keepdim=True)
+            lse_used = lse_h.clone()
+            if lse_off is not None:
+                lse_used[lse_off[0]] += lse_off[1]
+            lse_r = _f32(lse_used.double() * LOG2E32)
+            d_r = _f32(D.double() * sc)
+            S = qh @ kh.T
+            dP = dOh @ vh.T
+            p = _ex2(_f32(S.double() * sl2 - lse_r.double()))
+            ds = _f32(p.double() * _f32(dP.double() * sc - d_r.double()).double())
+            pb, dsb = p.bfloat16().float(), ds.bfloat16().float()
+            dq[b, :, cs] = dsb @ kh
+            if drop_tile is not None and h == 0:
+                keep = torch.ones(L, 1)
+                keep[128 * drop_tile:128 * drop_tile + 128] = 0
+                pk, dk_last = pb[:, -1:] * keep, dsb[:, -1:] * keep
+                pb, dsb = torch.cat([pb[:, :-1], pk], 1), torch.cat([dsb[:, :-1], dk_last], 1)
+            dk[b, :, cs] = dsb.T @ qh
+            dv[b, :, cs] = pb.T @ dOh
+    bf = lambda t: t.bfloat16().double()  # noqa: E731
+    return {"o": bf(o), "lse": lse.double(), "dq": bf(dq), "dk": bf(dk), "dv": bf(dv)}
+
+
+def _attn_autograd(q, k, v, dO, heads, dh, scale):
+    B, L, HD = q.shape
+    Lk = k.shape[1]
+    sc = float(torch.tensor(scale, dtype=torch.float32))
+    qr, kr, vr = (t.view(t.shape[0], t.shape[1], heads, dh).clone().requires_grad_(True) for t in (q, k, v))
+    logits = torch.einsum("blhd,bkhd->bhlk", qr, kr) * sc
+    o = torch.einsum("bhlk,bkhd->blhd", torch.softmax(logits, -1), vr).reshape(B, L, HD)
+    o.backward(dO)
+    return (o.detach(), torch.logsumexp(logits, -1).detach(), qr.grad.reshape(B, L, HD),
+            kr.grad.reshape(B, Lk, HD), vr.grad.reshape(B, Lk, HD))
+
+
+def _attn_check(got, ref, names=("o", "lse", "dq", "dk", "dv")):
+    worst = {}
+    for n in names:
+        val, d = ref[n]
+        bound = R.f32_bound(val, d) if n == "lse" else R.bf16_bound(val, d)
+        worst[n] = R.assert_elementwise(got[n], val, bound, n)
+    return worst
+
+
+@pytest.mark.parametrize("B,heads,L,Lk,dh,d_true", [(2, 2, 70, 77, 32, 16), (1, 3, 130, 129, 64, 48),
+                                                     (1, 2, 65, 300, 128, 80), (2, 1, 1, 1, 64, 64)])
+def test_attention_reference_matches_autograd(B, heads, L, Lk, dh, d_true):
+    q, k, v, dO = _attn_inputs(B, heads, L, Lk, dh, d_true, "random")
+    ref = R.attention_ref(q, k, v, heads, dh, d_true ** -0.5, dO, max_elems=4096)   # several row chunks
+    o, lse, gq, gk, gv = _attn_autograd(q, k, v, dO, heads, dh, d_true ** -0.5)
+    for n, want in (("o", o), ("lse", lse), ("dq", gq), ("dk", gk), ("dv", gv)):
+        _close(ref[n][0], want)
+        assert (ref[n][1] >= 0).all() and torch.isfinite(ref[n][1]).all(), n
+    for n, rows in (("o", L), ("dq", L), ("dk", Lk), ("dv", Lk)):
+        assert (ref[n][0].view(B, rows, heads, dh)[..., d_true:] == 0).all(), n
+
+
+_EMU_WORST = {}
+
+
+@pytest.mark.parametrize("regime", ["random", "rising", "first_max", "one_hot", "negative", "constant"])
+@pytest.mark.parametrize("B,heads,L,Lk,dh,d_true", [(1, 2, 200, 300, 32, 32), (1, 1, 130, 520, 64, 64),
+                                                     (1, 1, 70, 77, 64, 48), (1, 1, 129, 257, 128, 128)])
+def test_attention_emulation_within_bound(B, heads, L, Lk, dh, d_true, regime):
+    """An f32 emulation of the kernels' arithmetic lies inside the float64 bound at every element, across the
+    logit regimes the GPU tests use.  The worst |err| / bound per output is printed (pytest -s)."""
+    q, k, v, dO = _attn_inputs(B, heads, L, Lk, dh, d_true, regime, seed=Lk)
+    scale = d_true ** -0.5
+    ref = R.attention_ref(q, k, v, heads, dh, scale, dO)
+    worst = _attn_check(_attn_emulate(q, k, v, dO, heads, dh, scale), ref)
+    print(f"EMU dh={dh} {regime}: " + " ".join(f"{n} {w:.3f}" for n, w in worst.items()))
+    for n, w in worst.items():
+        _EMU_WORST[n] = max(_EMU_WORST.get(n, 0.0), w)
+
+
+def _old_gates(got, ref):
+    """The relative-L2 / absolute lse checks the attention GPU tests used before the element-wise comparator."""
+    return (rel(got["o"], ref["o"][0]) < 1.5e-2 and (got["lse"] - ref["lse"][0]).abs().max().item() < 2e-2
+            and all(rel(got[n], ref[n][0]) < 2e-2 for n in ("dq", "dk", "dv")))
+
+
+@pytest.mark.parametrize("defect", ["leak", "drop_tile", "lse_off"])
+def test_attention_comparator_rejects_what_relative_l2_accepts(defect):
+    """Three confined attention defects, each accepted by the old gates and rejected element by element:
+    (a) a zero-filled tail key counted in l at Lk = 77 (seen through lse, and through O in the negative-logit
+    regime), (b) one CTA's query tile missing from dK and dV of the last key of a ragged key block (one head),
+    (c) the last row of a ragged query tile recomputing P from an lse that is off by 2^-3.  An offset of 2^-7
+    scales that row's P by 0.8 %, about two bf16 roundings of dS, which the kernels' own arithmetic may reach
+    (0.2 - 0.4 of the bound); 2^-4 lands at 1.0 - 1.5 depending on the inputs, 2^-3 clears it about twofold."""
+    heads, dh, L, Lk = 2, 64, 1000, 77
+    q, k, v, dO = _attn_inputs(1, heads, L, Lk, dh, dh, "random", seed=7)
+    scale = dh ** -0.5
+    ref = R.attention_ref(q, k, v, heads, dh, scale, dO)
+    _attn_check(_attn_emulate(q, k, v, dO, heads, dh, scale), ref)
+    kw = {"leak": dict(leak=True), "drop_tile": dict(drop_tile=(L - 1) // 128),
+          "lse_off": dict(lse_off=(L - 1, 2.0 ** -3))}
+    bad = _attn_emulate(q, k, v, dO, heads, dh, scale, **kw[defect])
+    assert _old_gates(bad, ref)                                  # what the relative-L2 tests accept ...
+    with pytest.raises(AssertionError, match="outside the bound"):
+        _attn_check(bad, ref)                                    # ... the element-wise comparator does not
+    if defect == "leak":
+        qn, kn, vn, dOn = _attn_inputs(1, heads, L, Lk, dh, dh, "negative", seed=7)
+        refn = R.attention_ref(qn, kn, vn, heads, dh, scale)
+        badn = _attn_emulate(qn, kn, vn, dOn, heads, dh, scale, leak=True)
+        with pytest.raises(AssertionError, match="outside the bound"):
+            _attn_check(badn, refn, ("o",))
+
+
+def test_attention_emulation_bound_is_not_vacuous():
+    """Runs after the emulation cases: somewhere the emulation comes within 2 % of the bound in every output
+    (bounds that no f32 arithmetic approaches would let real defects through)."""
+    if len(_EMU_WORST) < 5:
+        pytest.skip("the emulation cases did not run in this session")
+    print("EMU worst overall: " + " ".join(f"{n} {w:.3f}" for n, w in sorted(_EMU_WORST.items())))
+    assert all(w >= 0.02 for w in _EMU_WORST.values()), _EMU_WORST
