@@ -29,10 +29,18 @@ constexpr int kPixBytes = 2 * 128 * 128;     // two boxes of 128 pixels x 64 cha
 constexpr int kHaloBytes = 18 * 16 * 128;    // 16 x 18 pixel box
 constexpr int kXchgBytes = 32 * kLdT * 4;    // one warpgroup's exchange tile
 
-__host__ __device__ constexpr int stage_bytes(bool halo) { return halo ? 3 * kWBytes + kHaloBytes : kWBytes + kPixBytes; }
+// RES (halo at K = 64 only): the nine weight tiles stay resident after the ring, so a stage is the pixel box alone
+__host__ __device__ constexpr int stage_bytes(bool halo, bool res) {
+  return halo ? (res ? 0 : 3 * kWBytes) + kHaloBytes : kWBytes + kPixBytes;
+}
 __host__ __device__ constexpr int num_stages(bool halo) { return halo ? 3 : 5; }
-__host__ __device__ constexpr int smem_bytes(bool halo) { return num_stages(halo) * stage_bytes(halo) + 1024 + 256 + 2 * kXchgBytes; }
-static_assert(smem_bytes(true) <= 227 * 1024 && smem_bytes(false) <= 227 * 1024, "tct: shared memory");
+__host__ __device__ constexpr int wres_bytes(bool res) { return res ? 9 * kWBytes : 0; }
+__host__ __device__ constexpr int smem_bytes(bool halo, bool res) {
+  return num_stages(halo) * stage_bytes(halo, res) + wres_bytes(res) + 1024 + 256 + 2 * kXchgBytes;
+}
+static_assert(smem_bytes(true, false) <= 227 * 1024 && smem_bytes(true, true) <= 227 * 1024 &&
+              smem_bytes(false, false) <= 227 * 1024, "tct: shared memory");
+static_assert((num_stages(true) * stage_bytes(true, true)) % 1024 == 0, "tct: resident weights need 1024-byte alignment");
 
 struct TctDev {
   int nxb, nyb, nimg, W, H;
@@ -50,6 +58,26 @@ struct TctDev {
   const float* gn_ab;      // GNB kernels: [N][2][Ncols] GroupNorm coefficients a, b of the tensor `res` (= x)
 };
 
+// Tile t = (pixel block t / cblks, column block t % cblks).  CTA b runs tiles b, b + grid, b + 2 grid, ...; with
+// RES the grid is a multiple of cblks, so the column block (and the resident weights) of a CTA never changes.
+struct TileCoord { int cb, nb, x0, y0; };
+
+// 16-byte global load / store with the streaming cache policy (.cs: evict first, data touched once)
+__device__ __forceinline__ uint4 ld_stream_u4(const __nv_bfloat16* src) {
+  uint4 r;
+  asm volatile("ld.global.cs.v4.b32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(src));
+  return r;
+}
+__device__ __forceinline__ void st_stream_u4(__nv_bfloat16* dst, const uint4& v) {
+  asm volatile("st.global.cs.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
+               : "memory");
+}
+__device__ __forceinline__ TileCoord tile_coord(const TctDev& p, int tile) {
+  const int mt = tile / p.cblks;
+  return {tile % p.cblks, mt / (p.nxb * p.nyb), (mt % p.nxb) * 16, ((mt / p.nxb) % p.nyb) * 16};
+}
+
 // HALO = true (3x3 stride-1 only): with per-tap loads every (tap, K chunk) re-loads its 256 pixels, 40 KB of TMA
 // per 2.1 MFLOP = 52 FLOP per byte, so the layers are L2 -> shared-memory bandwidth bound.  ONE tall box of
 // 16 x 18 pixels (rows y0-1 .. y0+16) is loaded per (kx, K chunk); the three ky taps are 2048-byte row offsets
@@ -59,24 +87,33 @@ struct TctDev {
 // GroupNorm input (side input `res`) and z = a_c x + b_c the kernel stores dz = dy * silu'(z) instead of dy and
 // accumulates S0 = sum dz, S1 = sum dz * x per (image, channel) into the column-sum workspace, exactly as the
 // pixels-as-M engine's EPI_GN_BWD (fdx_epilogue.cuh).
-template <bool A_MN, bool HALO, bool GNB>
+// RES = true (HALO with one K chunk, K = 64): all nine 8 KB weight tiles of the CTA's column block are loaded
+// once per CTA, on their own mbarrier, into 72 KB after the ring; a stage then carries only the 36 KB pixel box.
+// Otherwise every tile re-fetched the same 72 KB of weights, 40 % of its 180 KB of L2 -> shared-memory traffic.
+// The MMAs and their order (kx, ky, k16) are those of the plain HALO path, so the outputs are bit-identical.
+template <bool A_MN, bool HALO, bool GNB, bool RES>
 __global__ void __launch_bounds__(kThreads, 1)
 fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapX,
                const __grid_constant__ TctDev p) {
-  constexpr int kStageBytes = stage_bytes(HALO);
+  static_assert(HALO || !RES, "tct: resident weights need the halo stage");
+  constexpr int kStageBytes = stage_bytes(HALO, RES);
   constexpr int S = num_stages(HALO);
+  constexpr int kRingBytes = S * kStageBytes + wres_bytes(RES);   // the ring, then the resident weights
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * kStageBytes);
+  uint8_t* wres = smem + S * kStageBytes;                          // RES: tap t at t * kWBytes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + S;
+  uint64_t* wfull = bars + 2 * S;                                  // RES: the resident weights have landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&mapW);
     tma_prefetch_desc(&mapX);
     for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
+    if constexpr (RES) mbar_init(wfull, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -87,32 +124,37 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
   if (warp >= 8) {
     producer_regs();
     if (warp == 8 && lane == 0) {
+      // A_MN: HWIO rows = (tap, ci), co contiguous: box (64 co, 64 k rows); else (k = Cout contiguous,
+      // rows = Cin, z1 = tap): box (64 k, 64 rows)
+      auto load_w = [&](uint8_t* dst, uint64_t* bar, int cb, int t, int kc) {
+        if constexpr (A_MN) tma_load_4d(dst, &mapW, bar, cb * 64, p.tap_b[t] + kc * 64, 0, 0);
+        else tma_load_4d(dst, &mapW, bar, kc * 64, cb * 64, p.tap_b[t], 0);
+      };
+      if constexpr (RES) {
+        mbar_arrive_expect_tx(wfull, 9 * kWBytes);
+#pragma unroll
+        for (int t = 0; t < 9; ++t) load_w(wres + t * kWBytes, wfull, tile_coord(p, blockIdx.x).cb, t, 0);
+      }
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-        const int cb = tile % p.cblks;
-        const int mt = tile / p.cblks;
-        const int xb = mt % p.nxb, yb = (mt / p.nxb) % p.nyb, nb = mt / (p.nxb * p.nyb);
-        const int x0 = xb * 16, y0 = yb * 16;
+        const TileCoord tc = tile_coord(p, tile);
         for (int q = 0; q < nst; ++q) {
           const int qt = q / p.kchunks, kc = q % p.kchunks;     // qt = kx (HALO) or the tap
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sw = smem + stage * kStageBytes;
           mbar_arrive_expect_tx(&full[stage], kStageBytes);
-          // A_MN: HWIO rows = (tap, ci), co contiguous: box (64 co, 64 k rows); else (k = Cout contiguous,
-          // rows = Cin, z1 = tap): box (64 k, 64 rows)
-          auto load_w = [&](uint8_t* dst, int t) {
-            if constexpr (A_MN) tma_load_4d(dst, &mapW, &full[stage], cb * 64, p.tap_b[t] + kc * 64, 0, 0);
-            else tma_load_4d(dst, &mapW, &full[stage], kc * 64, cb * 64, p.tap_b[t], 0);
-          };
           if constexpr (HALO) {
+            if constexpr (!RES) {
 #pragma unroll
-            for (int ky = 0; ky < 3; ++ky) load_w(sw + ky * kWBytes, ky * 3 + qt);
-            tma_load_4d(sw + 3 * kWBytes, &mapX, &full[stage], kc * 64, x0 + qt - 1, y0 - 1, nb);
+              for (int ky = 0; ky < 3; ++ky) load_w(sw + ky * kWBytes, &full[stage], tc.cb, ky * 3 + qt, kc);
+            }
+            tma_load_4d(sw + (RES ? 0 : 3 * kWBytes), &mapX, &full[stage], kc * 64, tc.x0 + qt - 1, tc.y0 - 1, tc.nb);
           } else {
-            load_w(sw, qt);
+            load_w(sw, &full[stage], tc.cb, qt, kc);
             uint8_t* sx = sw + kWBytes;
-            tma_load_4d(sx, &mapX, &full[stage], kc * 64, x0 + p.tap_dx[qt], y0 + p.tap_dy[qt], nb);
-            tma_load_4d(sx + 16384, &mapX, &full[stage], kc * 64, x0 + p.tap_dx[qt], y0 + 8 + p.tap_dy[qt], nb);
+            tma_load_4d(sx, &mapX, &full[stage], kc * 64, tc.x0 + p.tap_dx[qt], tc.y0 + p.tap_dy[qt], tc.nb);
+            tma_load_4d(sx + 16384, &mapX, &full[stage], kc * 64, tc.x0 + p.tap_dx[qt], tc.y0 + 8 + p.tap_dy[qt],
+                        tc.nb);
           }
           if (++stage == S) { stage = 0; phase ^= 1; }
         }
@@ -136,7 +178,7 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
     // ones, so no full[] barrier is ever waited on more than one phase ahead (a parity wait one phase early
     // would pass at once, on a stage not yet loaded).
     const int my_turn = 3 + wg, their_turn = 4 - wg;
-    float* xsT = reinterpret_cast<float*>(smem + S * kStageBytes + 256) + wg * (32 * kLdT);
+    float* xsT = reinterpret_cast<float*>(smem + kRingBytes + 256) + wg * (32 * kLdT);
     const int piece = lane >> 4, prow = lane & 15;
     const int srow = q * 16 + piece * 8;                 // exchange-tile row (channel) of this lane's first channel
     __nv_bfloat16* outp = static_cast<__nv_bfloat16*>(p.out);
@@ -147,22 +189,23 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
     // work on the current one (one 128-byte line per pixel).
     auto prefetch_res = [&](int t) {
       if (resp == nullptr || t >= p.ntiles) return;
-      const int cb_ = t % p.cblks, mt_ = t / p.cblks;
-      const int xb_ = mt_ % p.nxb, yb_ = (mt_ / p.nxb) % p.nyb, nb_ = mt_ / (p.nxb * p.nyb);
-      const __nv_bfloat16* base = resp + (long long)nb_ * p.rs_n + (long long)(yb_ * 16) * p.rs_y +
-                                  (long long)(xb_ * 16) * p.rs_x + cb_ * 64;
+      const TileCoord c = tile_coord(p, t);
+      const __nv_bfloat16* base = resp + (long long)c.nb * p.rs_n + (long long)c.y0 * p.rs_y +
+                                  (long long)c.x0 * p.rs_x + c.cb * 64;
       for (int pi = t128; pi < 256; pi += 128)
         asm volatile("prefetch.global.L2 [%0];" ::"l"(base + (long long)(pi >> 4) * p.rs_y + (long long)(pi & 15) * p.rs_x));
     };
     prefetch_res(blockIdx.x + wg * gridDim.x);
+    // every CTA has at least one tile, so the producer always issues the resident weights' loads
+    if constexpr (RES) mbar_wait(wfull, 0);
+    const uint32_t wres_u32 = smem_u32(wres);
     for (int i = wg, tile = blockIdx.x + wg * gridDim.x; tile < p.ntiles; i += 2, tile += 2 * gridDim.x) {
       prefetch_res(tile + 2 * gridDim.x);
-      const int cb = tile % p.cblks;
-      const int mt = tile / p.cblks;
-      const int xb = mt % p.nxb, yb = (mt / p.nxb) % p.nyb, nb = mt / (p.nxb * p.nyb);
-      const long long obase = (long long)nb * p.os_n + (long long)(yb * 16) * p.os_y + (long long)(xb * 16) * p.os_x;
-      const long long rbase = (long long)nb * p.rs_n + (long long)(yb * 16) * p.rs_y + (long long)(xb * 16) * p.rs_x;
-      const int ch = cb * 64 + srow;                       // read phase: this lane's first channel
+      const TileCoord tc = tile_coord(p, tile);
+      const int nb = tc.nb;
+      const long long obase = (long long)nb * p.os_n + (long long)tc.y0 * p.os_y + (long long)tc.x0 * p.os_x;
+      const long long rbase = (long long)nb * p.rs_n + (long long)tc.y0 * p.rs_y + (long long)tc.x0 * p.rs_x;
+      const int ch = tc.cb * 64 + srow;                    // read phase: this lane's first channel
       float add[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -189,12 +232,16 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
         mbar_wait(&full[stage], phase);
         wgmma_fence();
         const uint32_t sw = smem_u32(smem + stage * kStageBytes);
-        const uint32_t sx = sw + (HALO ? 3 : 1) * kWBytes;   // HALO: the 16 x 18 box; per-tap: two 16 x 8 boxes
+        // HALO: the 16 x 18 box; per-tap: two 16 x 8 boxes
+        const uint32_t sx = sw + (HALO ? (RES ? 0 : 3) : 1) * kWBytes;
+        // weight tile of (ky, this stage): RES, tap ky * 3 + kx of the resident set (kq = kx); else ky of the stage
+        const uint32_t wb = RES ? wres_u32 + kq * kWBytes : sw;
 #pragma unroll
         for (int ky = 0; ky < (HALO ? 3 : 1); ++ky) {
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
-            const uint32_t aw = A_MN ? sw + ky * kWBytes + k * 2048 : sw + ky * kWBytes + k * 32;
+            const uint32_t wt = wb + ky * (RES ? 3 : 1) * kWBytes;
+            const uint32_t aw = A_MN ? wt + k * 2048 : wt + k * 32;
             const uint64_t db = gmma_desc_sw128(sx + ky * 2048 + k * 32, 16, 1024);   // HALO: rows ky .. ky+15
             const uint64_t da = A_MN ? gmma_desc_sw128(aw, 8192, 1024) : gmma_desc_sw128(aw, 16, 1024);
             wgmma_m64n256k16<A_MN ? 1 : 0, 0>(acc, da, db);
@@ -213,19 +260,31 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
       float s0[8], s1[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) { s0[j] = 0.f; s1[j] = 0.f; }
+      // Side input of chunk c (pixel rows 2 c, 2 c + 1) into registers.  Chunk c + 1's is requested before
+      // chunk c is exchanged and stored, so each L2 round trip overlaps a whole chunk, not one exchange.  The
+      // per-tap GroupNorm-backward variant has no registers to spare for that (ptxas spills) and loads each
+      // chunk's side input at the start of the chunk.
+      // Side input and output are touched once: they are loaded and stored with the streaming (evict-first)
+      // policy, so they do not push the pixel boxes that neighbouring tiles still read out of L2.
+      constexpr int kDist = (HALO || !GNB) ? 1 : 0;
+      constexpr int kBufs = kDist + 1;
+      uint4 rbuf[kBufs][2];
+      auto load_res = [&](int c, uint4 (&r)[2]) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          r[k] = make_uint4(0, 0, 0, 0);
+          if (resp)
+            r[k] = ld_stream_u4(resp + rbase + (long long)(2 * c + k) * p.rs_y + (long long)prow * p.rs_x + ch);
+        }
+      };
+#pragma unroll
+      for (int c = 0; c < kDist; ++c) load_res(c, rbuf[c]);
       // Unrolled: the chunk index is a compile-time register index, and the 16 accumulator registers of a
       // chunk die once it is written out.
 #pragma unroll
       for (int ci = 0; ci < 8; ++ci) {
-        // The side input of this chunk is requested before the exchange so its latency overlaps it.
-        uint4 rcur[2];
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          rcur[k] = make_uint4(0, 0, 0, 0);
-          if (resp)
-            rcur[k] = *reinterpret_cast<const uint4*>(resp + rbase + (long long)(2 * ci + k) * p.rs_y +
-                                                      (long long)prow * p.rs_x + ch);
-        }
+        if (ci + kDist < 8) load_res(ci + kDist, rbuf[(ci + kDist) % kBufs]);
+        const uint4* rcur = rbuf[ci % kBufs];
         // ---- write phase: accumulator fragments of columns 32 ci .. 32 ci + 31 -> xsT[px][channel row] ----
         named_bar_sync(xbar, 128);                       // the previous chunk's reads are done
         {
@@ -268,7 +327,7 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
           uint4 o;
           o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]);
           o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
-          *reinterpret_cast<uint4*>(outp + obase + (long long)(2 * ci + k) * p.os_y + (long long)prow * p.os_x + ch) = o;
+          st_stream_u4(outp + obase + (long long)(2 * ci + k) * p.os_y + (long long)prow * p.os_x + ch, o);
           if (p.cs_ws) {
             const float2 h0 = unpack_bf16x2(o.x), h1 = unpack_bf16x2(o.y), h2 = unpack_bf16x2(o.z),
                          h3 = unpack_bf16x2(o.w);
@@ -299,21 +358,38 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
   }
 }
 
-template <bool A_MN, bool HALO, bool GNB = false>
-int launch_tct(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& d, cudaStream_t stream) {
-  constexpr int smem = smem_bytes(HALO);
+template <bool A_MN, bool HALO, bool GNB, bool RES>
+int launch_tct_grid(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& d, cudaStream_t stream) {
+  constexpr int smem = smem_bytes(HALO, RES);
   static bool attr_set = false;
   if (!attr_set) {
-    FDX_CUDA(cudaFuncSetAttribute(fdx_tct_kernel<A_MN, HALO, GNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    FDX_CUDA(cudaFuncSetAttribute(fdx_tct_kernel<A_MN, HALO, GNB, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  smem));
     attr_set = true;
   }
   int grid = fdx_num_sms();
   if (grid <= 0) return FDX_ERR_NO_DEVICE;
+  // RES: a whole number of column-block groups, so each CTA keeps one column block (tile_coord); ntiles is a
+  // multiple of cblks, so the clamp below keeps that.
+  if (RES) grid = (grid >= d.cblks ? grid / d.cblks : 1) * d.cblks;
   if (d.ntiles < grid) grid = d.ntiles;
-  fdx_tct_kernel<A_MN, HALO, GNB><<<grid, kThreads, smem, stream>>>(mW, mX, d);
+  fdx_tct_kernel<A_MN, HALO, GNB, RES><<<grid, kThreads, smem, stream>>>(mW, mX, d);
   fdx_note_kernel(FDX_KERNEL_TCT);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
+}
+
+// Halo launches with one K chunk keep their weights resident (RES); at K >= 128 the nine taps (147 KB and more)
+// do not fit beside the ring.  RES needs a grid of whole column-block groups; where that would leave SMs idle
+// (cblks = 5 on 132 SMs: 130 CTAs) the plain halo launch is the faster one, by about 1 % on an H100 SXM.
+template <bool A_MN, bool HALO, bool GNB = false>
+int launch_tct(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& d, cudaStream_t stream) {
+  if constexpr (HALO) {
+    const int sms = fdx_num_sms();
+    if (d.kchunks == 1 && std::min(d.ntiles, sms / d.cblks * d.cblks) == std::min(d.ntiles, sms))
+      return launch_tct_grid<A_MN, true, GNB, true>(mW, mX, d, stream);
+  }
+  return launch_tct_grid<A_MN, HALO, GNB, false>(mW, mX, d, stream);
 }
 
 }  // namespace
