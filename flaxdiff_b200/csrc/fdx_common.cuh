@@ -116,6 +116,40 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// L2 policy for data touched once (evict first): it does not push out lines that other CTAs still read
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ void tma_load_4d_hint(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                 int c2, int c3, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy)
+      : "memory");
+}
+// Bulk tensor store shared -> global.  The writing threads issue fence_proxy_async_smem() before the barrier
+// that precedes it; the source may be rewritten once bulk_wait_group_read shows the store's group has read it.
+__device__ __forceinline__ void tma_store_4d_hint(const CUtensorMap* m, const void* src, int c0, int c1, int c2,
+                                                  int c3, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group.L2::cache_hint"
+      " [%0, {%2, %3, %4, %5}], [%1], %6;" ::"l"(reinterpret_cast<uint64_t>(m)),
+      "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy)
+      : "memory");
+}
+// bulk async-groups belong to the thread that committed them: only it can wait on them
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
 
 // ----- wgmma ----------------------------------------------------------------------
 // One warpgroup (four consecutive warps, the first a multiple of four) computes D(64 x N, f32 registers)

@@ -15,7 +15,11 @@
 // consumer warpgroups that take alternate tiles of the CTA's persistent tile sequence.  Each owns its whole
 // tile (128 accumulator registers per thread), so warpgroup 0 runs the main loop of tile 2i while warpgroup 1
 // runs the epilogue of tile 2i - 1: output stores and side-input loads overlap the other tile's MMAs.
-// Geometry: stride 1, W and H multiples of 16.
+// The epilogue moves its HBM traffic by TMA as well: each warpgroup's leader requests the side input (residual,
+// accumulate source, or x of the fused GroupNorm backward) of a tile's first 32-pixel chunks when the tile's main
+// loop starts, into a ring of 4 KB chunk buffers, and stores each finished chunk from the same buffer with one
+// bulk tensor store, so neither direction waits on per-thread global round trips.
+// Geometry: stride 1, W and H multiples of 16; output and side input 16-byte aligned with 16-byte strides (TMA).
 #include "fdx_tc.cuh"
 #include "fdx_epilogue.cuh"
 #include <stdlib.h>
@@ -28,31 +32,40 @@ constexpr int kWBytes = 64 * 128;            // weight tile: 64 channels x 64 k 
 constexpr int kPixBytes = 2 * 128 * 128;     // two boxes of 128 pixels x 64 channels bf16
 constexpr int kHaloBytes = 18 * 16 * 128;    // 16 x 18 pixel box
 constexpr int kXchgBytes = 32 * kLdT * 4;    // one warpgroup's exchange tile
+constexpr int kChunkBytes = 32 * 128;        // one epilogue chunk: 32 pixels x 64 channels bf16 (one TMA box)
+constexpr int kCBufs = 3;                    // chunk buffers per consumer warpgroup
+constexpr int kEpiBytes = 2 * kCBufs * kChunkBytes;
+static_assert((2 * 4 + 1 + 2 * kCBufs) * 8 <= 256, "tct: barrier area");
 
 // RES (halo at K = 64 only): the nine weight tiles stay resident after the ring, so a stage is the pixel box alone
 __host__ __device__ constexpr int stage_bytes(bool halo, bool res) {
   return halo ? (res ? 0 : 3 * kWBytes) + kHaloBytes : kWBytes + kPixBytes;
 }
-__host__ __device__ constexpr int num_stages(bool halo) { return halo ? 3 : 5; }
+// per-tap: a fifth 40 KB stage does not fit beside the chunk buffers
+__host__ __device__ constexpr int num_stages(bool halo) { return halo ? 3 : 4; }
 __host__ __device__ constexpr int wres_bytes(bool res) { return res ? 9 * kWBytes : 0; }
-__host__ __device__ constexpr int smem_bytes(bool halo, bool res) {
-  return num_stages(halo) * stage_bytes(halo, res) + wres_bytes(res) + 1024 + 256 + 2 * kXchgBytes;
+__host__ __device__ constexpr int ring_bytes(bool halo, bool res) {
+  return num_stages(halo) * stage_bytes(halo, res) + wres_bytes(res);
 }
+// ring (+ resident weights), chunk buffers, barriers, exchange tiles; 1024 = alignment slack of the dynamic base
+__host__ __device__ constexpr int smem_bytes(bool halo, bool res) {
+  return ring_bytes(halo, res) + kEpiBytes + 1024 + 256 + 2 * kXchgBytes;
+}
+// halo and RES: 180 + 24 + 18.25 = 222.25 KB; per-tap: 160 + 24 + 18.25 = 202.25 KB
 static_assert(smem_bytes(true, false) <= 227 * 1024 && smem_bytes(true, true) <= 227 * 1024 &&
               smem_bytes(false, false) <= 227 * 1024, "tct: shared memory");
 static_assert((num_stages(true) * stage_bytes(true, true)) % 1024 == 0, "tct: resident weights need 1024-byte alignment");
+static_assert(ring_bytes(true, false) % 1024 == 0 && ring_bytes(true, true) % 1024 == 0 &&
+              ring_bytes(false, false) % 1024 == 0, "tct: 128-byte-swizzled chunk buffers need 1024-byte alignment");
 
 struct TctDev {
   int nxb, nyb, nimg, W, H;
   int ntaps, tap_dx[kTcMaxTaps], tap_dy[kTcMaxTaps], tap_b[kTcMaxTaps];
   int kchunks, K, Ncols, cblks, ntiles;
-  void* out;
-  long long os_x, os_y, os_n;
   float alpha;
   const float* bias;
   const float* rowvec;
-  const void* res;
-  long long rs_x, rs_y, rs_n;
+  int has_res;             // a side input (mapR) is added, or is x of the fused GroupNorm backward
   float* cs_ws;            // fused per-(image, channel) sums or null
   int cs_slots, cs_ld;
   const float* gn_ab;      // GNB kernels: [N][2][Ncols] GroupNorm coefficients a, b of the tensor `res` (= x)
@@ -62,17 +75,6 @@ struct TctDev {
 // RES the grid is a multiple of cblks, so the column block (and the resident weights) of a CTA never changes.
 struct TileCoord { int cb, nb, x0, y0; };
 
-// 16-byte global load / store with the streaming cache policy (.cs: evict first, data touched once)
-__device__ __forceinline__ uint4 ld_stream_u4(const __nv_bfloat16* src) {
-  uint4 r;
-  asm volatile("ld.global.cs.v4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(src));
-  return r;
-}
-__device__ __forceinline__ void st_stream_u4(__nv_bfloat16* dst, const uint4& v) {
-  asm volatile("st.global.cs.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-               : "memory");
-}
 __device__ __forceinline__ TileCoord tile_coord(const TctDev& p, int tile) {
   const int mt = tile / p.cblks;
   return {tile % p.cblks, mt / (p.nxb * p.nyb), (mt % p.nxb) * 16, ((mt / p.nxb) % p.nyb) * 16};
@@ -94,26 +96,31 @@ __device__ __forceinline__ TileCoord tile_coord(const TctDev& p, int tile) {
 template <bool A_MN, bool HALO, bool GNB, bool RES>
 __global__ void __launch_bounds__(kThreads, 1)
 fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapX,
+               const __grid_constant__ CUtensorMap mapR, const __grid_constant__ CUtensorMap mapO,
                const __grid_constant__ TctDev p) {
   static_assert(HALO || !RES, "tct: resident weights need the halo stage");
   constexpr int kStageBytes = stage_bytes(HALO, RES);
   constexpr int S = num_stages(HALO);
-  constexpr int kRingBytes = S * kStageBytes + wres_bytes(RES);   // the ring, then the resident weights
+  constexpr int kRingBytes = ring_bytes(HALO, RES);                // the ring, then the resident weights
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* wres = smem + S * kStageBytes;                          // RES: tap t at t * kWBytes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes + kEpiBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + S;
   uint64_t* wfull = bars + 2 * S;                                  // RES: the resident weights have landed
+  uint64_t* cfull = bars + 2 * S + 1;                              // [2][kCBufs]: a chunk's side input has landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&mapW);
     tma_prefetch_desc(&mapX);
+    tma_prefetch_desc(&mapO);
+    if (p.has_res) tma_prefetch_desc(&mapR);
     for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
     if constexpr (RES) mbar_init(wfull, 1);
+    for (int i = 0; i < 2 * kCBufs; ++i) mbar_init(&cfull[i], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -178,40 +185,56 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
     // ones, so no full[] barrier is ever waited on more than one phase ahead (a parity wait one phase early
     // would pass at once, on a stage not yet loaded).
     const int my_turn = 3 + wg, their_turn = 4 - wg;
-    float* xsT = reinterpret_cast<float*>(smem + kRingBytes + 256) + wg * (32 * kLdT);
+    float* xsT = reinterpret_cast<float*>(smem + kRingBytes + kEpiBytes + 256) + wg * (32 * kLdT);
     const int piece = lane >> 4, prow = lane & 15;
     const int srow = q * 16 + piece * 8;                 // exchange-tile row (channel) of this lane's first channel
-    __nv_bfloat16* outp = static_cast<__nv_bfloat16*>(p.out);
-    const __nv_bfloat16* resp = static_cast<const __nv_bfloat16*>(p.res);
     float acc[128];
-    // Side input (residual / accumulate source): each epilogue chunk loads its own pieces, which hides an L2
-    // hit, not HBM.  So the consumer threads pull the side input of the warpgroup's NEXT tile into L2 while they
-    // work on the current one (one 128-byte line per pixel).
-    auto prefetch_res = [&](int t) {
-      if (resp == nullptr || t >= p.ntiles) return;
-      const TileCoord c = tile_coord(p, t);
-      const __nv_bfloat16* base = resp + (long long)c.nb * p.rs_n + (long long)c.y0 * p.rs_y +
-                                  (long long)c.x0 * p.rs_x + c.cb * 64;
-      for (int pi = t128; pi < 256; pi += 128)
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(base + (long long)(pi >> 4) * p.rs_y + (long long)(pi & 15) * p.rs_x));
+    // Side input and output move by TMA through the warpgroup's kCBufs chunk buffers.  Chunk c of a tile is
+    // pixel rows 2 c, 2 c + 1 of its 16 x 16 block, 64 channels: one {64, 16, 2, 1} box, 128-byte swizzled, so
+    // the 16-byte pieces a quarter-warp reads (8 pixels, one channel piece) fall in 8 different bank groups.
+    // The warpgroup's n-th chunk (8 per tile) uses buffer n % kCBufs and barrier phase n / kCBufs.  The side
+    // input arrives in the buffer, each thread overwrites the pieces it read with its output, and one store
+    // sends the buffer back.  The leader thread issues all of it: bulk async-groups are per thread, so only the
+    // thread that committed a buffer's store can tell when its buffer may be refilled.  Side input and output
+    // are touched once and carry the evict-first L2 policy, so they do not push out the pixel boxes that
+    // neighbouring tiles still read.
+    uint8_t* cbuf = smem + kRingBytes + wg * kCBufs * kChunkBytes;
+    uint64_t* wg_cfull = cfull + wg * kCBufs;
+    auto load_chunk = [&](const TileCoord& c, int ci, int n) {
+      uint64_t* bar = &wg_cfull[n % kCBufs];
+      mbar_arrive_expect_tx(bar, kChunkBytes);
+      tma_load_4d_hint(cbuf + (n % kCBufs) * kChunkBytes, &mapR, bar, c.cb * 64, c.x0, c.y0 + 2 * ci, c.nb,
+                       l2_evict_first_policy());
     };
-    prefetch_res(blockIdx.x + wg * gridDim.x);
+    auto store_chunk = [&](const TileCoord& c, int ci, int n) {
+      tma_store_4d_hint(&mapO, cbuf + (n % kCBufs) * kChunkBytes, c.cb * 64, c.x0, c.y0 + 2 * ci, c.nb,
+                        l2_evict_first_policy());
+      bulk_commit_group();
+    };
     // every CTA has at least one tile, so the producer always issues the resident weights' loads
     if constexpr (RES) mbar_wait(wfull, 0);
     const uint32_t wres_u32 = smem_u32(wres);
     for (int i = wg, tile = blockIdx.x + wg * gridDim.x; tile < p.ntiles; i += 2, tile += 2 * gridDim.x) {
-      prefetch_res(tile + 2 * gridDim.x);
       const TileCoord tc = tile_coord(p, tile);
       const int nb = tc.nb;
-      const long long obase = (long long)nb * p.os_n + (long long)tc.y0 * p.os_y + (long long)tc.x0 * p.os_x;
-      const long long rbase = (long long)nb * p.rs_n + (long long)tc.y0 * p.rs_y + (long long)tc.x0 * p.rs_x;
+      const int n0 = (i >> 1) * 8;                         // the warpgroup's chunk count before this tile
+      // the side input of the first kCBufs chunks, requested before the main loop so that it has the main
+      // loop (and the wait for the tensor cores) to arrive from HBM; their buffers are free once the previous
+      // tile's stores have read them
+      if (p.has_res && wg_leader) {
+        bulk_wait_group_read<0>();
+#pragma unroll
+        for (int c = 0; c < kCBufs; ++c) load_chunk(tc, c, n0 + c);
+      }
       const int ch = tc.cb * 64 + srow;                    // read phase: this lane's first channel
       float add[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         add[j] = 0.f;
-        if (p.bias) add[j] += __ldg(p.bias + ch + j);
-        if (p.rowvec) add[j] += __ldg(p.rowvec + (long long)nb * p.Ncols + ch + j);
+        if constexpr (!GNB) {   // GNB launches have neither (fdx_tct_launch): the zeros then hold no registers
+          if (p.bias) add[j] += __ldg(p.bias + ch + j);
+          if (p.rowvec) add[j] += __ldg(p.rowvec + (long long)nb * p.Ncols + ch + j);
+        }
       }
       float ga[8], gb[8];
       if constexpr (GNB) {
@@ -257,36 +280,24 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
       wgmma_wait<0>();
       if (wg_leader) mbar_arrive(&empty[prev]);
 
+      // the tile's coordinates again: kept in registers across the main loop, they make the GroupNorm-backward
+      // variants spill
+      const TileCoord ec = tile_coord(p, tile);
       float s0[8], s1[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) { s0[j] = 0.f; s1[j] = 0.f; }
-      // Side input of chunk c (pixel rows 2 c, 2 c + 1) into registers.  Chunk c + 1's is requested before
-      // chunk c is exchanged and stored, so each L2 round trip overlaps a whole chunk, not one exchange.  The
-      // per-tap GroupNorm-backward variant has no registers to spare for that (ptxas spills) and loads each
-      // chunk's side input at the start of the chunk.
-      // Side input and output are touched once: they are loaded and stored with the streaming (evict-first)
-      // policy, so they do not push the pixel boxes that neighbouring tiles still read out of L2.
-      constexpr int kDist = (HALO || !GNB) ? 1 : 0;
-      constexpr int kBufs = kDist + 1;
-      uint4 rbuf[kBufs][2];
-      auto load_res = [&](int c, uint4 (&r)[2]) {
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          r[k] = make_uint4(0, 0, 0, 0);
-          if (resp)
-            r[k] = ld_stream_u4(resp + rbase + (long long)(2 * c + k) * p.rs_y + (long long)prow * p.rs_x + ch);
-        }
-      };
-#pragma unroll
-      for (int c = 0; c < kDist; ++c) load_res(c, rbuf[c]);
       // Unrolled: the chunk index is a compile-time register index, and the 16 accumulator registers of a
       // chunk die once it is written out.
 #pragma unroll
       for (int ci = 0; ci < 8; ++ci) {
-        if (ci + kDist < 8) load_res(ci + kDist, rbuf[(ci + kDist) % kBufs]);
-        const uint4* rcur = rbuf[ci % kBufs];
+        const int n = n0 + ci;
+        uint8_t* cb = cbuf + (n % kCBufs) * kChunkBytes;
         // ---- write phase: accumulator fragments of columns 32 ci .. 32 ci + 31 -> xsT[px][channel row] ----
-        named_bar_sync(xbar, 128);                       // the previous chunk's reads are done
+        named_bar_sync(xbar, 128);                       // the previous chunk's reads and buffer writes are done
+        if (wg_leader) {
+          if (ci > 0) store_chunk(ec, ci - 1, n - 1);
+          bulk_wait_group_read<kCBufs - 1>();            // this chunk's buffer has been read by its last store
+        }
         {
           const int w = t128 >> 5, l = t128 & 31;
 #pragma unroll
@@ -300,18 +311,29 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
           }
         }
         named_bar_sync(xbar, 128);
+        if (p.has_res) {
+          // refill the buffer the previous chunk's store (issued above) is reading: the side input of chunk
+          // ci + kCBufs - 1, two chunks before it is needed
+          if (wg_leader && ci > 0 && ci + kCBufs - 1 < 8) {
+            bulk_wait_group_read<0>();
+            load_chunk(ec, ci + kCBufs - 1, n + kCBufs - 1);
+          }
+          mbar_wait(&wg_cfull[n % kCBufs], (n / kCBufs) & 1);
+        }
         // ---- read phase: 16-byte channel pieces; columns 32 ci .. 32 ci + 31 = pixel rows 2 ci, 2 ci + 1 ----
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
-          const int j = prow + 16 * k;                     // pixel (column) within the chunk
+          const int j = prow + 16 * k;                     // pixel (column) within the chunk = box row
           const float4 a = *reinterpret_cast<const float4*>(xsT + j * kLdT + srow);
           const float4 b = *reinterpret_cast<const float4*>(xsT + j * kLdT + srow + 4);
           float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
           for (int e = 0; e < 8; ++e) f[e] = f[e] * p.alpha + add[e];
+          // this lane's 16-byte piece of box row j under the 128-byte swizzle (16-byte unit u -> u ^ (row % 8))
+          uint4* piece_p = reinterpret_cast<uint4*>(cb + j * 128 + (((srow >> 3) ^ (j & 7)) << 4));
           float xv[8];
-          if (resp) {
-            const uint4 r = rcur[k];
+          if (p.has_res) {
+            const uint4 r = *piece_p;
             const float2 r0 = unpack_bf16x2(r.x), r1 = unpack_bf16x2(r.y), r2 = unpack_bf16x2(r.z),
                          r3 = unpack_bf16x2(r.w);
             xv[0] = r0.x; xv[1] = r0.y; xv[2] = r1.x; xv[3] = r1.y;
@@ -327,7 +349,7 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
           uint4 o;
           o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]);
           o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
-          st_stream_u4(outp + obase + (long long)(2 * ci + k) * p.os_y + (long long)prow * p.os_x + ch, o);
+          *piece_p = o;
           if (p.cs_ws) {
             const float2 h0 = unpack_bf16x2(o.x), h1 = unpack_bf16x2(o.y), h2 = unpack_bf16x2(o.z),
                          h3 = unpack_bf16x2(o.w);
@@ -337,7 +359,10 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
             for (int e = 0; e < 8; ++e) { s0[e] += hv[e]; s1[e] = fmaf(hv[e], GNB ? xv[e] : hv[e], s1[e]); }
           }
         }
+        fence_proxy_async_smem();                        // the buffer's new contents, visible to the TMA store
       }
+      named_bar_sync(xbar, 128);
+      if (wg_leader) store_chunk(ec, 7, n0 + 7);
       if (p.cs_ws) {
         // the 16 lanes with the same piece (l / 16) hold the same 8 channels: combine them
 #pragma unroll
@@ -349,17 +374,21 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
           }
         }
         if (prow == 0) {
-          float* w = p.cs_ws + (((long long)(tile % p.cs_slots) * p.nimg + nb) * 2) * p.cs_ld + ch;
+          float* w = p.cs_ws + (((long long)(tile % p.cs_slots) * p.nimg + ec.nb) * 2) * p.cs_ld + ec.cb * 64 + srow;
 #pragma unroll
           for (int e = 0; e < 8; ++e) { atomicAdd(w + e, s0[e]); atomicAdd(w + p.cs_ld + e, s1[e]); }
         }
       }
     }
+    if (wg_leader) bulk_wait_group<0>();                 // every output store has completed
   }
 }
 
+// weights, pixels (the A operand), side input (unset without one) and output
+struct TctMaps { CUtensorMap w, x, r, o; };
+
 template <bool A_MN, bool HALO, bool GNB, bool RES>
-int launch_tct_grid(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& d, cudaStream_t stream) {
+int launch_tct_grid(const TctMaps& m, const TctDev& d, cudaStream_t stream) {
   constexpr int smem = smem_bytes(HALO, RES);
   static bool attr_set = false;
   if (!attr_set) {
@@ -373,7 +402,7 @@ int launch_tct_grid(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& 
   // multiple of cblks, so the clamp below keeps that.
   if (RES) grid = (grid >= d.cblks ? grid / d.cblks : 1) * d.cblks;
   if (d.ntiles < grid) grid = d.ntiles;
-  fdx_tct_kernel<A_MN, HALO, GNB, RES><<<grid, kThreads, smem, stream>>>(mW, mX, d);
+  fdx_tct_kernel<A_MN, HALO, GNB, RES><<<grid, kThreads, smem, stream>>>(m.w, m.x, m.r, m.o, d);
   fdx_note_kernel(FDX_KERNEL_TCT);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
@@ -383,13 +412,28 @@ int launch_tct_grid(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& 
 // do not fit beside the ring.  RES needs a grid of whole column-block groups; where that would leave SMs idle
 // (cblks = 5 on 132 SMs: 130 CTAs) the plain halo launch is the faster one, by about 1 % on an H100 SXM.
 template <bool A_MN, bool HALO, bool GNB = false>
-int launch_tct(const CUtensorMap& mW, const CUtensorMap& mX, const TctDev& d, cudaStream_t stream) {
+int launch_tct(const TctMaps& m, const TctDev& d, cudaStream_t stream) {
   if constexpr (HALO) {
     const int sms = fdx_num_sms();
     if (d.kchunks == 1 && std::min(d.ntiles, sms / d.cblks * d.cblks) == std::min(d.ntiles, sms))
-      return launch_tct_grid<A_MN, true, GNB, true>(mW, mX, d, stream);
+      return launch_tct_grid<A_MN, true, GNB, true>(m, d, stream);
   }
-  return launch_tct_grid<A_MN, HALO, GNB, false>(mW, mX, d, stream);
+  return launch_tct_grid<A_MN, HALO, GNB, false>(m, d, stream);
+}
+
+// TMA needs a 16-byte-aligned base and strides that are multiples of 16 bytes
+bool tma_view_ok(const void* base, long long sx, long long sy, long long sn) {
+  return reinterpret_cast<uintptr_t>(base) % 16 == 0 && sx % 8 == 0 && sy % 8 == 0 && sn % 8 == 0;
+}
+
+// the epilogue's TMA view of the output or side input: (channel, x, y, image), one chunk box {64, 16, 2, 1}
+int make_chunk_map(CUtensorMap* map, const void* base, const TcLaunch& L, long long sx, long long sy,
+                   long long sn) {
+  const uint64_t dims[4] = {(uint64_t)L.Ncols, (uint64_t)L.W, (uint64_t)L.H, (uint64_t)L.N};
+  const uint64_t str[3] = {(uint64_t)sx * 2, (uint64_t)sy * 2, (uint64_t)sn * 2};
+  const uint32_t box[4] = {64, 16, 2, 1};
+  const uint32_t est[4] = {1, 1, 1, 1};
+  return fdx_make_tmap_bf16(map, base, 4, dims, str, box, est, 1);
 }
 
 }  // namespace
@@ -403,6 +447,9 @@ int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
   // column counts the generic engine would have to cover with N < 256 tiles (64, 128, 192, 320, 384, ...)
   if (L.Ncols % 64 != 0 || L.Ncols % 256 == 0 || L.Ncols > 512) return FDX_ERR_UNSUPPORTED;
   if (L.W % 16 != 0 || L.H % 16 != 0 || L.K % 64 != 0) return FDX_ERR_UNSUPPORTED;
+  // the epilogue moves output and side input by TMA
+  if (!tma_view_ok(L.out, L.os_x, L.os_y, L.os_n) || (L.res && !tma_view_ok(L.res, L.rs_x, L.rs_y, L.rs_n)))
+    return FDX_ERR_UNSUPPORTED;
   TctDev d{};
   d.W = L.W; d.H = L.H; d.nimg = L.N;
   d.nxb = L.W / 16; d.nyb = L.H / 16;
@@ -411,9 +458,8 @@ int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
   d.K = L.K; d.kchunks = L.K / 64; d.Ncols = L.Ncols;
   d.cblks = L.Ncols / 64;
   d.ntiles = d.cblks * d.nxb * d.nyb * d.nimg;
-  d.out = L.out; d.os_x = L.os_x; d.os_y = L.os_y; d.os_n = L.os_n;
   d.alpha = L.alpha; d.bias = L.bias; d.rowvec = L.rowvec;
-  d.res = L.res; d.rs_x = L.rs_x; d.rs_y = L.rs_y; d.rs_n = L.rs_n;
+  d.has_res = L.res != nullptr;
   d.cs_ws = L.gn_ws; d.cs_slots = L.gn_slots > 0 ? L.gn_slots : 1; d.cs_ld = L.ws_ld > 0 ? L.ws_ld : L.Ncols;
   d.gn_ab = L.gn_ab;
 
@@ -424,14 +470,14 @@ int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
   const char* he = getenv("FDX_TCT_HALO");          // read per launch: the A/B tests toggle it in-process
   const int halo_env = (he && *he) ? atoi(he) : -1;
   if (halo_env >= 0 && halo_env != 64) halo = false;
-  CUtensorMap mW, mX;
+  TctMaps m{};
   {
     uint64_t dims[4], str[3];
     for (int i = 0; i < 4; ++i) dims[i] = L.A.dims[i];
     for (int i = 1; i < 4; ++i) str[i - 1] = L.A.strides[i] * 2;
     uint32_t box[4] = {64, 16, (uint32_t)(halo ? 18 : 8), 1};
     uint32_t est[4] = {1, 1, 1, 1};
-    int s = fdx_make_tmap_bf16(&mX, L.A.ptr, 4, dims, str, box, est, 1);
+    int s = fdx_make_tmap_bf16(&m.x, L.A.ptr, 4, dims, str, box, est, 1);
     if (s != FDX_OK) return s;
   }
   {
@@ -440,12 +486,14 @@ int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
     for (int i = 1; i < 4; ++i) str[i - 1] = L.B.strides[i] * 2;
     uint32_t box[4] = {64, 64, 1, 1};
     uint32_t est[4] = {1, 1, 1, 1};
-    int s = fdx_make_tmap_bf16(&mW, L.B.ptr, 4, dims, str, box, est, 1);
+    int s = fdx_make_tmap_bf16(&m.w, L.B.ptr, 4, dims, str, box, est, 1);
     if (s != FDX_OK) return s;
   }
-  if (L.mode == TC_KMN)
-    return halo ? launch_tct<true, true>(mW, mX, d, stream) : launch_tct<true, false>(mW, mX, d, stream);
+  int s = make_chunk_map(&m.o, L.out, L, L.os_x, L.os_y, L.os_n);
+  if (s != FDX_OK) return s;
+  if (L.res && (s = make_chunk_map(&m.r, L.res, L, L.rs_x, L.rs_y, L.rs_n)) != FDX_OK) return s;
+  if (L.mode == TC_KMN) return halo ? launch_tct<true, true>(m, d, stream) : launch_tct<true, false>(m, d, stream);
   if (L.gn_ab)   // fused GroupNorm backward
-    return halo ? launch_tct<false, true, true>(mW, mX, d, stream) : launch_tct<false, false, true>(mW, mX, d, stream);
-  return halo ? launch_tct<false, true>(mW, mX, d, stream) : launch_tct<false, false>(mW, mX, d, stream);
+    return halo ? launch_tct<false, true, true>(m, d, stream) : launch_tct<false, false, true>(m, d, stream);
+  return halo ? launch_tct<false, true>(m, d, stream) : launch_tct<false, false>(m, d, stream);
 }
