@@ -9,6 +9,10 @@
 //                  updates m, v, writes the un-scaled update u and accumulates per-tensor ||p||^2, ||u||^2
 //                  (segment = binary search of the element index in the layout's offset table), pass 2
 //                  applies p -= lr * ratio[seg] * u and the EMA / shadow refresh.
+//                  The per-tensor norms run over whole 64-element slots, so the alignment gaps between
+//                  tensors must be zero in p, g, m and v (then they stay zero in m, v and u): the trainer
+//                  zeroes the gradient buffer before every backward pass, and parameters and moments
+//                  start zero-filled.  A non-zero gap would enter its tensor's trust ratio.
 #include "fdx_common.cuh"
 #include "../../include/fdx.h"
 #include <math.h>
@@ -39,7 +43,9 @@ __device__ __forceinline__ GradScale grad_scale_of(float gscale, const float* __
     r.skip = gstats && gstats[1] > 0.f;
   }
   if (gstats && clip_norm > 0.f) {
-    const float nrm = sqrtf(gstats[0]) * r.mul;          // norm of the TRUE (averaged, unscaled) gradient
+    // gstats[0] = sum (g / loss scale)^2: fdx_grad_stats unscaled before squaring, so the norm stays finite
+    // at any loss scale; grad_scale is applied here
+    const float nrm = sqrtf(gstats[0]) * gscale;          // norm of the TRUE (averaged, unscaled) gradient
     if (nrm > clip_norm) r.mul *= clip_norm / nrm;
   }
   return r;
@@ -199,16 +205,19 @@ __global__ void ema_kernel(float* __restrict__ ema, const float* __restrict__ p,
   }
 }
 
-// out[0] += sum g^2, out[1] += number of non-finite elements
-__global__ void grad_stats_kernel(const float* __restrict__ g, long long n, float* __restrict__ out) {
+// out[0] += sum (g / dynscale[0])^2 (sum g^2 without dynscale), out[1] += number of non-finite elements of g
+__global__ void grad_stats_kernel(const float* __restrict__ g, long long n, const float* __restrict__ dynscale,
+                                  float* __restrict__ out) {
+  const float mul = dynscale ? 1.f / dynscale[0] : 1.f;
   float acc = 0.f, bad = 0.f;
   const long long n4 = n / 4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
        i += (long long)gridDim.x * blockDim.x) {
     const float4 v = reinterpret_cast<const float4*>(g)[i];
-    acc += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
-    const float t = v.x + v.y + v.z + v.w;     // non-finite iff any element is (inf - inf = nan included)
-    if (!(fabsf(t) <= 3.402823466e38f)) bad += 1.f;
+    const float x = v.x * mul, y = v.y * mul, z = v.z * mul, w = v.w * mul;
+    acc += x * x + y * y + z * z + w * w;
+    // element by element: finite values whose sum overflows are still finite
+    bad += (float)(!isfinite(v.x)) + (float)(!isfinite(v.y)) + (float)(!isfinite(v.z)) + (float)(!isfinite(v.w));
   }
   acc = warp_sum(acc);
   bad = warp_sum(bad);
@@ -294,18 +303,18 @@ int fdx_ema_update(float* ema, const float* p, long long n, float decay, void* s
   return FDX_OK;
 }
 
-int fdx_grad_stats(const float* g, long long n, float* out2, void* stream) {
+int fdx_grad_stats(const float* g, long long n, const float* dynscale, float* out2, void* stream) {
   FDX_REQUIRE(g && out2 && n > 0 && n % 4 == 0, "grad_stats: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   FDX_CUDA(cudaMemsetAsync(out2, 0, 2 * sizeof(float), st));
-  grad_stats_kernel<<<stream_grid(n / 4, 256), 256, 0, st>>>(g, n, out2);
+  grad_stats_kernel<<<stream_grid(n / 4, 256), 256, 0, st>>>(g, n, dynscale, out2);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
 }
 
 int fdx_sumsq(const float* g, long long n, float* out, void* stream) {
   // kept for callers that only need the norm: out[0] = sum g^2 (out must hold 2 floats: see fdx_grad_stats)
-  return fdx_grad_stats(g, n, out, stream);
+  return fdx_grad_stats(g, n, nullptr, out, stream);
 }
 
 int fdx_dynscale_update(float* state3, const float* gstats, float growth_factor, float backoff_factor,

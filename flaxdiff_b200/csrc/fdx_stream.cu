@@ -142,9 +142,9 @@ __global__ void affine_kernel(const AffineArgs p, int B, long long E) {
         }
       }
     }
-    if (p.clip) {
+    if (p.clip) {   // jnp.clip: a NaN propagates (fminf / fmaxf would turn it into clip_lo and hide it)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) o1[j] = fminf(fmaxf(o1[j], p.clip_lo), p.clip_hi);
+      for (int j = 0; j < 4; ++j) o1[j] = o1[j] < p.clip_lo ? p.clip_lo : (o1[j] > p.clip_hi ? p.clip_hi : o1[j]);
     }
     if (p.out1) reinterpret_cast<float4*>(p.out1)[i] = make_float4(o1[0], o1[1], o1[2], o1[3]);
     if (p.out2) reinterpret_cast<float4*>(p.out2)[i] = make_float4(o2[0], o2[1], o2[2], o2[3]);

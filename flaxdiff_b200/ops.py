@@ -400,10 +400,12 @@ def ema_update(ema: torch.Tensor, p: torch.Tensor, decay: float):
                                 stream_ptr()), "ema_update")
 
 
-def grad_stats(g: torch.Tensor) -> torch.Tensor:
-    """-> f32[2] = (sum g^2, number of non-finite elements)."""
+def grad_stats(g: torch.Tensor, dynscale: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """-> f32[2] = (sum (g / dynscale[0])^2 or sum g^2, number of non-finite elements of g).  Pass the same
+    DynamicScale state as to optimizer_step: its clip reads the norm with the loss scale removed."""
     out = torch.empty(2, dtype=torch.float32, device=g.device)
-    check(load().fdx_grad_stats(ptr(g), ctypes.c_longlong(g.numel()), ptr(out), stream_ptr()), "grad_stats")
+    check(load().fdx_grad_stats(ptr(g), ctypes.c_longlong(g.numel()), ptr(dynscale), ptr(out), stream_ptr()),
+          "grad_stats")
     return out
 
 

@@ -277,7 +277,8 @@ class TrainState:
         self._settle_count()
         count = self.opt_state["count"] + 1
         ds = self.dynamic_scale
-        gstats = ops.grad_stats(grads.flat) if (tx.clip_norm > 0 or ds is not None) else None
+        gstats = (ops.grad_stats(grads.flat, ds.state if ds is not None else None)
+                  if (tx.clip_norm > 0 or ds is not None) else None)
         lr = tx.lr_at(count - 1)
         if dyn is not None:
             host = torch.tensor([lr, 1 - tx.b1 ** count, 1 - tx.b2 ** count], dtype=torch.float32)

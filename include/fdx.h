@@ -195,7 +195,8 @@ int fdx_loss_fwd_bwd(const float* F, const float* x_t, const float* target, cons
                      float* loss_sum, float* dF, void* stream);
 /* out1 = sum_i coef1[i][b]*in_i ; out2 = sum_i coef2[i][b]*in_i ; out_bf16 = bf16(out1*scale[b]).
  * One pass for x0/eps recovery, CFG mixing (samplers/common.py:93-96) and every sampler update
- * (samplers/euler.py:8-18,39-56; heun_sampler.py:7-27; ddim.py:30-47; ddpm.py:6-15). */
+ * (samplers/euler.py:8-18,39-56; heun_sampler.py:7-27; ddim.py:30-47; ddpm.py:6-15).
+ * clip != 0 clamps out1 to [clip_lo, clip_hi] as jnp.clip does: a NaN stays NaN. */
 int fdx_affine_combine(int n_in, const float* const* inputs, const float* coef1, const float* coef2,
                        const float* bf16_scale, int B, long long E, float* out1, float* out2,
                        void* out_bf16, int clip, float clip_lo, float clip_hi, void* stream);
@@ -204,7 +205,9 @@ int fdx_affine_combine(int n_in, const float* const* inputs, const float* coef1,
  * (training.py:263-267,594-608; trainer/general_diffusion_trainer.py:311,327), fused with
  * TrainState.apply_ema (trainer/diffusion_trainer.py:31-37) and the refresh of the bf16 weight shadow the
  * tensor-core kernels read.  `ema` NULL = apply_gradients only.  The gradient the update sees is
- *   g * grad_scale [/ dynscale[0]] * min(1, clip_norm / ||.||)          (||.|| from gstats[0])
+ *   g * grad_scale [/ dynscale[0]] * min(1, clip_norm / ||.||)    (||.|| = sqrt(gstats[0]) * grad_scale)
+ * so with dynscale set, gstats must come from fdx_grad_stats called with the same dynscale: it then holds the
+ * squared norm of the gradient with the loss scale removed, which stays finite at any loss scale.
  * and with `dynscale` set the parameter / moment update is SKIPPED when gstats[1] > 0 (non-finite gradients,
  * general_diffusion_trainer.py:313-318) while the EMA still runs on the unchanged parameters.
  * lamb: seg_offsets = the nseg tensor start offsets (elements, ascending, first = 0, multiples of 4),
@@ -236,9 +239,11 @@ int fdx_adamw_ema_step(float* p, const float* g, float* m, float* v, float* ema,
                        void* stream);
 /* TrainState.apply_ema on its own: ema = decay*ema + (1-decay)*p (trainer/diffusion_trainer.py:31-37). */
 int fdx_ema_update(float* ema, const float* p, long long n, float decay, void* stream);
-/* out2[0] = sum g^2 (optax.clip_by_global_norm), out2[1] = number of non-finite elements (DynamicScale's
- * is_finite, flax/training/dynamic_scale.py via general_diffusion_trainer.py:308).  fdx_sumsq = same call. */
-int fdx_grad_stats(const float* g, long long n, float* out2, void* stream);
+/* out2[0] = sum (g / dynscale[0])^2, or sum g^2 with dynscale NULL (optax.clip_by_global_norm: the loss scale
+ * is removed before squaring, so the sum stays finite at any scale), out2[1] = number of non-finite elements of
+ * g, each tested on its own (DynamicScale's is_finite, flax/training/dynamic_scale.py via
+ * general_diffusion_trainer.py:308).  fdx_sumsq = fdx_grad_stats(g, n, NULL, out2). */
+int fdx_grad_stats(const float* g, long long n, const float* dynscale, float* out2, void* stream);
 int fdx_sumsq(const float* g, long long n, float* out2, void* stream);
 /* DynamicScale state update after a step: state3 = {scale, fin_steps, last_finite}; finite: after
  * growth_interval finite steps scale *= growth_factor; non-finite: scale = max(scale*backoff, minimum). */

@@ -71,7 +71,7 @@ def assert_elementwise(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor
     b = torch.as_tensor(bound, dtype=torch.float64, device=g.device).expand_as(r)
     assert g.shape == r.shape, (what, tuple(g.shape), tuple(r.shape))
     err = (g - r).abs()
-    frac = err / b
+    frac = torch.where(err == 0, torch.zeros_like(err), err / b)     # an exact element is 0 x even a zero bound
     bad = ~(err <= b) | ~torch.isfinite(g)            # NaN compares false: an unwritten NaN-prefilled element fails
     nbad = int(bad.sum())
     worst = torch.where(torch.isfinite(frac), frac, torch.full_like(frac, math.inf))
@@ -456,3 +456,249 @@ def attention_ref(q, k, v, heads: int, dh: int, scale: float, d_o=None, max_elem
                 val, err, mag = acc[n]
                 res[n][0][b, :, cs], res[n][1][b, :, cs] = val, err + TC_ADD * Lp * mag
     return res
+
+
+# ----------------------------------------------------------------------------------------------- training step
+# The kernels that run once per step over every parameter (csrc/fdx_optim.cu), the time embedding
+# (csrc/fdx_misc.cu) and the diffusion / loss / sampler streams (csrc/fdx_stream.cu).  Conventions as above;
+# in addition:
+#   * deltas here EXCLUDE the output's own rounding (f32_bound adds it); an intermediate that the kernel rounds
+#     and reuses enters downstream with its delta + u |value| (`_full`).
+#   * each product or sum of a formula rounds once (u on its absolute value); with FMA contraction some of
+#     these roundings disappear, so the same bound covers the fused and the unfused form.
+#   * TINY: one rounding into the subnormal range (the library is built without flush-to-zero) is off by at
+#     most 2^-150 absolute; every rounding of a value that can be that small adds TINY.
+#   * sqrtf is correctly rounded (no fast-math); sinf / cosf / tanhf are within 2 ulp (CUDA C Programming
+#     Guide, Mathematical Functions); atomics add in any order, so each atomic on an address is one level of
+#     summation depth.
+TINY = 2.0 ** -149
+TANHF = 4 * U32              # tanhf: 2 ulp of a result in [-1, 1], i.e. 4u relative
+
+
+def ulp_f32(ref: torch.Tensor) -> torch.Tensor:
+    """Spacing of f32 numbers at |ref| (2^(e-24) for |ref| in [2^(e-1), 2^e); 2^-149 below the smallest normal)."""
+    a = ref.abs().to(torch.float64).clamp_min(2.0 ** -126)
+    _, e = torch.frexp(a)
+    return torch.ldexp(torch.ones_like(a), (e - 24).to(torch.int32))
+
+
+def f32(x: float) -> float:
+    """x rounded to f32 (round to nearest), as a Python float."""
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def _full(val, delta):
+    """Error of an intermediate the kernel rounded to f32 and then reads again."""
+    return delta + U32 * val.abs() + TINY
+
+
+def adam_ref(p, g, m, v, *, lr, b1, b2, eps, wd, bc1, bc2, mul, rho_mul=0.0):
+    """One optax adam / adamw step (scale_by_adam -> add_decayed_weights -> -lr) as adam_kernel evaluates it:
+        gj = g mul;  m' = b1 m + (1 - b1) gj;  v' = b2 v + (1 - b2) gj gj
+        t = (m'/bc1) / (sqrt(v'/bc2) + eps) + wd p;  p' = p - lr t
+    p, g, m, v: float64 tensors of the f32 values; the hyperparameters are the f32 values the kernel uses
+    (lr, b1, b2, eps, wd, bc1, bc2); `mul` the exact gradient multiplier (grad_scale / loss scale times the
+    clip factor) and rho_mul the relative error of the kernel's f32 multiplier.  1 - b is exact for b in
+    [0.5, 1] (Sterbenz).  -> dict of (value, delta) for p, m, v and t (LAMB's update u, before -lr)."""
+    c1, c2 = 1.0 - b1, 1.0 - b2
+    gj = g * mul
+    e_gj = (U32 + rho_mul) * gj.abs() + TINY
+    m1 = b1 * m + c1 * gj
+    e_m = U32 * ((b1 * m).abs() + (c1 * gj).abs()) + c1 * e_gj + 2 * TINY
+    v1 = b2 * v + c2 * gj * gj
+    e_v = U32 * (b2 * v + 2 * c2 * gj * gj) + 2 * c2 * gj.abs() * e_gj + 3 * TINY
+    mh, vh = m1 / bc1, v1 / bc2
+    e_mh = _full(m1, e_m) / bc1 + U32 * mh.abs() + TINY
+    e_vh = _full(v1, e_v) / bc2 + U32 * vh + TINY
+    s = torch.sqrt(vh)
+    e_s = torch.where(s > 0, e_vh / (2 * s.clamp_min(1e-300)), torch.sqrt(e_vh)) + U32 * s
+    den = s + eps
+    e_den = e_s + U32 * den
+    q = mh / den
+    e_q = e_mh / den + q.abs() * e_den / den + U32 * q.abs() + TINY
+    t = q + wd * p
+    e_t = e_q + U32 * (wd * p).abs()
+    p1 = p - lr * t
+    e_p = lr * _full(t, e_t) + U32 * lr * t.abs()
+    return {"p": (p1, e_p), "m": (m1, e_m), "v": (v1, e_v), "t": (t, e_t)}
+
+
+def ema_ref(ema, p, decay, e_p=None):
+    """TrainState.apply_ema: ema' = decay ema + (1 - decay) p (decay and 1 - decay as the kernel's f32 values);
+    e_p: delta of the p the kernel reads (the fused step's p' before its rounding), None when p is exact."""
+    c = f32(1.0 - decay)
+    val = decay * ema + c * p
+    delta = U32 * ((decay * ema).abs() + (c * p).abs()) + 2 * TINY
+    if e_p is not None:
+        delta = delta + c * _full(p, e_p)
+    return val, delta
+
+
+def sumsq_ref(g, mul, depth: int):
+    """fdx_grad_stats' out[0] = sum (g mul)^2 over a buffer, with a summation depth `depth`; the kernel's
+    product g fl(mul) and the square add 3u relative to each (positive) term, the multiplier's rounding 1u."""
+    x = g * mul
+    val = (x * x).sum()
+    return val, gamma(depth + 4) * val
+
+
+def grad_stats_depth(n: int, sms: int) -> int:
+    """grad_stats_kernel: grid = min(ceil(n/4/256), 8 SMs) blocks of 256 threads; each thread adds one float4
+    (a 4-term chain) per grid-stride iteration to its running sum, then a warp tree (5), the 8 warps' tree (5)
+    and one atomic per block."""
+    n4 = n // 4
+    blocks = max(1, min(math.ceil(n4 / 256), 8 * sms))
+    iters = math.ceil(n4 / (blocks * 256))
+    return 4 + iters + 10 + blocks
+
+
+def lamb_ref(p, g, m, v, seg_start, seg_len, *, lr, b1, b2, eps, wd, bc1, bc2, mul, rho_mul=0.0):
+    """optax.lamb over a flat buffer of segments [seg_start, seg_start + seg_len) (tensor slots, 64-aligned,
+    zero gaps): u = adam's t, ratio = ||p|| / ||u|| per segment (1 where either is 0), p' = p - lr ratio u.
+    lamb_pass1_kernel sums each segment's p^2 and u^2 as 4-term fmaf chains, then a warp tree (5) and one
+    atomic per warp when the warp's 128 elements lie in one segment, per thread otherwise: at most
+    ceil(len/128) + 1 single-segment warps, 2 x 32 threads of warps that straddle a boundary and 32 of the
+    partial last warp.  -> dict of (value, delta) for p, m, v, u, and the per-segment norms (sum p^2, sum u^2)."""
+    r = adam_ref(p, g, m, v, lr=lr, b1=b1, b2=b2, eps=eps, wd=wd, bc1=bc1, bc2=bc2, mul=mul, rho_mul=rho_mul)
+    u, e_u = r["t"]
+    e_uf = _full(u, e_u)
+    nseg = seg_start.numel()
+    seg = torch.repeat_interleave(torch.arange(nseg, device=p.device), seg_len)
+
+    def ssum(x):
+        return torch.zeros(nseg, dtype=torch.float64, device=p.device).index_add_(0, seg, x)
+
+    D = torch.tensor([9 + math.ceil(int(n) / 128) + 1 + 96 for n in seg_len.tolist()], dtype=torch.float64,
+                     device=p.device)
+    gD = D * U32 / (1 - D * U32)
+    np2, nu2 = ssum(p * p), ssum(u * u)
+    e_np2 = gD * np2
+    e_nu2 = gD * nu2 + 2 * ssum(u.abs() * e_uf)
+    pn, un = torch.sqrt(np2), torch.sqrt(nu2)
+    one = (pn == 0) | (un == 0)
+    ratio = torch.where(one, torch.ones_like(pn), pn / torch.where(one, torch.ones_like(un), un))
+    rel = torch.where(one, torch.zeros_like(pn),
+                      e_np2 / (2 * np2.clamp_min(1e-300)) + e_nu2 / (2 * nu2.clamp_min(1e-300)) + 3 * U32)
+    a, rel_a = (lr * ratio)[seg], (rel + U32)[seg]
+    p1 = p - a * u
+    e_p = a * e_uf + (a * u).abs() * (rel_a + U32)
+    return {"p": (p1, e_p), "m": r["m"], "v": r["v"], "u": (u, e_u), "np2": (np2, e_np2), "nu2": (nu2, e_nu2)}
+
+
+# time embedding: gelu(tanh) with tanhf and the f32 constants of fdx_misc.cu
+GELU_K = math.sqrt(2 / math.pi)
+
+
+def gelu_f32_ref(x):
+    """gelu_tanh(x) = 0.5 x (1 + tanhf(k (x + a x^3))) -> (value, delta, t, e_t): the argument carries 7
+    roundings (x^3: 2, a x^3, the sum, k ( ), the f32 constants k and a) on k (|x| + a |x|^3)."""
+    inner = GELU_K * (x + GELU_A * x ** 3)
+    t = torch.tanh(inner)
+    e_in = 7 * U32 * GELU_K * (x.abs() + GELU_A * x.abs() ** 3)
+    e_t = TANHF * t.abs() + (1 - t * t) * e_in
+    y = 0.5 * x * (1 + t)
+    return y, 0.5 * x.abs() * (e_t + U32 * (1 + t).abs()), t, e_t
+
+
+def gelu_grad_f32_ref(x):
+    """gelu_tanh_grad: 0.5 (1 + t) + 0.5 x (1 - t^2) k (1 + 3 a x^2) -> (value, delta incl. its own rounding):
+    the error of t times d/dt = 1/2 - x t K, and 12 roundings on the absolute-value form."""
+    _, _, t, e_t = gelu_f32_ref(x)
+    K = GELU_K * (1 + 3 * GELU_A * x * x)
+    gp = 0.5 * (1 + t) + 0.5 * x * (1 - t * t) * K
+    gp_abs = 0.5 * (1 + t.abs()) + 0.5 * x.abs() * (1 + t * t) * K
+    return gp, (0.5 - x * t * K).abs() * e_t + 12 * U32 * gp_abs
+
+
+def time_phase_f32(t, freqs):
+    """The kernel's phase: fl(t fl(fl(2 pi) f)), in f32 (one correctly rounded product each) -> (B, D/2)."""
+    w = torch.tensor(2 * math.pi, dtype=torch.float32, device=freqs.device) * freqs.to(torch.float32)
+    return t.to(torch.float32)[:, None] * w[None, :]
+
+
+def time_embed_fwd_ref(ph, four, h1, h2, W1, b1, W2, b2):
+    """FourierEmbedding + TimeProjection, each stage from the f32 values the kernel stored before it (four, h1,
+    h2: float64 of the kernel's outputs).  Dense: a serial chain of D fmas onto the bias (gamma(D)).
+    -> dict of (value, bound): 'four' is bounded by 2 ulp of the float64 sine / cosine of the f32 phase; the
+    others are (value, delta) for f32_bound."""
+    D = W1.shape[0]
+    ph = ph.to(torch.float64)
+    fr = torch.cat([torch.sin(ph), torch.cos(ph)], 1)
+    out = {"four": (fr, 2 * ulp_f32(fr))}
+    out["h1"] = (b1 + four @ W1, gamma(D) * (b1.abs() + four.abs() @ W1.abs()))
+    g1, e_g1 = gelu_f32_ref(h1)[:2]
+    out["h2"] = (b2 + g1 @ W2, gamma(D) * (b2.abs() + g1.abs() @ W2.abs()) + _full(g1, e_g1) @ W2.abs())
+    out["emb"] = gelu_f32_ref(h2)[:2]
+    return out
+
+
+def wgrad_small_depth(B: int) -> int:
+    """dense_wgrad_small_kernel: batch slices bs = 16 / 4 / 1 for B >= 64 / >= 8 / < 8, a serial chain over
+    ceil(B / bs) samples each, then bs atomics onto the prior value."""
+    bs = 16 if B >= 64 else (4 if B >= 8 else 1)
+    return math.ceil(B / bs) + bs + 1
+
+
+def time_embed_bwd_ref(demb, four, h1, h2, dh1, dh2, W2, dW1_0, db1_0, dW2_0, db2_0):
+    """Backward of the time MLP, each stage from the kernel's stored f32 inputs (dh1, dh2: its workspaces):
+        dh2 = demb gelu'(h2);  dh1 = (dh2 W2^T) gelu'(h1);  dW2 += gelu(h1)^T dh2;  dW1 += four^T dh1;  db += sum_b
+    -> dict of (value, delta) for dh2, dh1, dW1, db1, dW2, db2."""
+    D, B = W2.shape[0], demb.shape[0]
+    gp2, e_gp2 = gelu_grad_f32_ref(h2)
+    gp1, e_gp1 = gelu_grad_f32_ref(h1)
+    out = {"dh2": (demb * gp2, demb.abs() * e_gp2)}
+    da1 = dh2 @ W2.T
+    e_da1 = gamma(D) * (dh2.abs() @ W2.abs().T)
+    out["dh1"] = (da1 * gp1, gp1.abs() * e_da1 + da1.abs() * e_gp1)
+    g1, e_g1 = gelu_f32_ref(h1)[:2]
+    gw = gamma(wgrad_small_depth(B))
+    out["dW2"] = (dW2_0 + g1.T @ dh2, gw * (dW2_0.abs() + g1.abs().T @ dh2.abs()) + _full(g1, e_g1).T @ dh2.abs())
+    out["db2"] = (db2_0 + dh2.sum(0), gw * (db2_0.abs() + dh2.abs().sum(0)))
+    out["dW1"] = (dW1_0 + four.T @ dh1, gw * (dW1_0.abs() + four.abs().T @ dh1.abs()))
+    out["db1"] = (db1_0 + dh1.sum(0), gw * (db1_0.abs() + dh1.abs().sum(0)))
+    return out
+
+
+def diffuse_ref(x0, eps, alpha, sigma, normalize: bool, kind: int):
+    """forward_diffusion + get_target of diffuse_forward_kernel: x = (x0 - 127.5) / 127.5 (one rounding) or x0;
+    x_t = a x + s eps; target x / eps / (a eps - s x) rsqrtf(a^2 + s^2).  x0, eps: (B, E) float64; alpha,
+    sigma: (B,) the f32 values.  -> dict of (value, delta) for x_t and target."""
+    a, s = alpha[:, None], sigma[:, None]
+    x = (x0 - 127.5) / 127.5 if normalize else x0
+    e_x = U32 * x.abs() if normalize else torch.zeros_like(x)
+    xt = a * x + s * eps
+    out = {"x_t": (xt, a.abs() * e_x + U32 * ((a * x).abs() + (s * eps).abs()))}
+    if kind == 0:
+        out["target"] = (x, torch.zeros_like(x))      # the normalising division is the output's own rounding
+    elif kind == 1:
+        out["target"] = (eps, torch.zeros_like(eps))
+    else:
+        inv = 1.0 / torch.sqrt(a * a + s * s)
+        rho = gamma(3) / 2 + RSQRT
+        d = a * eps - s * x
+        e_d = U32 * ((a * eps).abs() + (s * x).abs() + d.abs()) + s.abs() * e_x
+        out["target"] = (d * inv, inv * e_d + (d * inv).abs() * rho)
+    return out
+
+
+def loss_ref(F, x_t, target, c_out, c_skip, weight, depth: int):
+    """optax.l2_loss weighted and averaged (loss_kernel): d = c_out F + c_skip x_t - target (4 roundings on the
+    absolute-value sum), loss = sum 0.5 w d^2 / (B E), dF = w c_out d / (B E) with g = fl(fl(w c_out) fl(1/(BE)))
+    (3u).  The loss adds, per positive term, 4 roundings of the float4's squares, the product by w, the product by
+    1/(BE) and its rounding, and `depth` levels of summation.  -> dict of (value, delta) for loss and dF."""
+    B, E = F.shape
+    co, cs, w = c_out[:, None], c_skip[:, None], weight[:, None]
+    d = co * F + cs * x_t - target
+    e_d = gamma(4) * ((co * F).abs() + (cs * x_t).abs() + target.abs())
+    g = w * co / (B * E)
+    term = 0.5 * w * d * d / (B * E)
+    loss = term.sum()
+    e_loss = gamma(depth + 7) * loss + (w * d.abs() * e_d).sum() / (B * E)
+    return {"loss": (loss, e_loss), "dF": (g * d, g.abs() * e_d + 3 * U32 * (g * d).abs())}
+
+
+def affine_ref(inputs, coef):
+    """sum_k coef[k, b] in_k as a serial chain of n_in fmas from 0 (affine_kernel) -> (value, delta)."""
+    val = sum(c[:, None] * x for c, x in zip(coef, inputs))
+    mag = sum((c[:, None] * x).abs() for c, x in zip(coef, inputs))
+    return val, gamma(len(inputs)) * mag

@@ -380,3 +380,254 @@ def test_attention_emulation_bound_is_not_vacuous():
         pytest.skip("the emulation cases did not run in this session")
     print("EMU worst overall: " + " ".join(f"{n} {w:.3f}" for n, w in sorted(_EMU_WORST.items())))
     assert all(w >= 0.02 for w in _EMU_WORST.values()), _EMU_WORST
+
+
+# ----------------------------------------------------------------------------------------------- training step
+def _fl(t):
+    """Round a float64 tensor to f32 and back: one f32 rounding (how an FMA's single rounding is emulated)."""
+    return t.float().double()
+
+
+HP = dict(lr=R.f32(2.7e-4), b1=R.f32(0.9), b2=R.f32(0.999), eps=R.f32(1e-8), wd=R.f32(1e-4))
+
+
+def _opt_inputs(n=1 << 18, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    r = lambda s=1.0: torch.randn(n, generator=g, dtype=torch.float64) * s  # noqa: E731
+    p, gr, m = r(0.05), r(), r(0.1 / 8)
+    v = r(1 / 8) ** 2 * r().abs()
+    gr[100:600], m[100:600], v[100:600] = 0, 0, 0                 # unused parameters
+    gr[1000:1500] *= 1e-40                                       # subnormal
+    gr[2000:2500] *= 1e15                                        # large
+    return [_fl(t) for t in (p, gr, m, v)]
+
+
+def _adam_emulate(p, g, m, v, *, lr, b1, b2, eps, wd, bc1, bc2, mul, fused):
+    """adam_kernel in f32, with every product rounded (fused=False) or with the FMA contractions nvcc may make
+    (fused=True: a*b + c rounded once)."""
+    c1, c2 = 1.0 - b1, 1.0 - b2
+    if not fused:
+        f = lambda x: torch.tensor(x, dtype=torch.float32)  # noqa: E731
+        P, G, M, V = (t.float() for t in (p, g, m, v))
+        gj = G * f(mul)
+        M1 = f(b1) * M + f(c1) * gj
+        V1 = f(b2) * V + f(c2) * gj * gj
+        T = (M1 / f(bc1)) / (torch.sqrt(V1 / f(bc2)) + f(eps)) + f(wd) * P
+        return (P - f(lr) * T).double(), M1.double(), V1.double(), T.double()
+    gj = _fl(g * mul)
+    m1 = _fl(b1 * m + _fl(c1 * gj))
+    v1 = _fl(b2 * v + _fl(_fl(c2 * gj) * gj))
+    q = _fl(_fl(m1 / bc1) / _fl(_fl(torch.sqrt(_fl(v1 / bc2))) + eps))
+    t = _fl(wd * p + q)
+    return _fl(p - lr * t), m1, v1, t
+
+
+def test_optimizer_references_match_optax_restatement():
+    """adam_ref / lamb_ref / ema_ref / sumsq_ref against oracle/diffusion_ref.py (optax.adamw, optax.lamb,
+    clip_by_global_norm, apply_ema written out in numpy float64)."""
+    from oracle import diffusion_ref as O
+    p, g, m, v = _opt_inputs(4096)
+    step, mul = 7, 0.125
+    bc1, bc2 = 1 - HP["b1"] ** step, 1 - HP["b2"] ** step
+    r = R.adam_ref(p, g, m, v, bc1=bc1, bc2=bc2, mul=mul, **HP)
+    wp, wm, wv, we = O.adamw_ema(p.numpy(), mul * g.numpy(), m.numpy(), v.numpy(), p.numpy(), step, HP["lr"],
+                                 HP["b1"], HP["b2"], HP["eps"], HP["wd"], decay=0.999)
+    for k, w in (("p", wp), ("m", wm), ("v", wv)):
+        _close(r[k][0], torch.from_numpy(w), 1e-13)
+    _close(R.ema_ref(p, r["p"][0], 0.999)[0], torch.from_numpy(we), 1e-9)    # 1 - decay as the kernel's f32
+    # clip_by_global_norm then adam: the clipped multiplier
+    (gc,), nrm = O.clip_by_global_norm([(mul * g).numpy()], 1.0)
+    assert nrm > 1
+    r = R.adam_ref(p, g, m, v, bc1=bc1, bc2=bc2, mul=mul / nrm, **HP)
+    wp = O.adamw_ema(p.numpy(), gc.astype("float64"), m.numpy(), v.numpy(), p.numpy(), step, HP["lr"], HP["b1"],
+                     HP["b2"], HP["eps"], HP["wd"])[0]
+    _close(r["p"][0], torch.from_numpy(wp), 1e-6)              # the oracle rounds the clipped gradient to f32
+    val, _ = R.sumsq_ref(g, mul, 10)
+    _close(val, torch.tensor(nrm ** 2), 1e-12)
+    # lamb over three segments, the third with p = 0
+    lens = [128, 576, 64]
+    starts = torch.tensor([0, 128, 704])
+    p[704:768] = 0
+    r = R.lamb_ref(p[:768], g[:768], m[:768], v[:768], starts, torch.tensor(lens), bc1=bc1, bc2=bc2, mul=1.0,
+                   **HP)
+    sl = [slice(0, 128), slice(128, 704), slice(704, 768)]
+    wp, wm, wv = O.lamb_step([p[s].numpy() for s in sl], [g[s].numpy() for s in sl], [m[s].numpy() for s in sl],
+                             [v[s].numpy() for s in sl], step, HP["lr"], HP["b1"], HP["b2"], HP["eps"], HP["wd"])
+    for s, a, b, c in zip(sl, wp, wm, wv):
+        _close(r["p"][0][s], torch.from_numpy(a).double(), 1e-6)    # the oracle returns f32
+        _close(r["m"][0][s], torch.from_numpy(b).double(), 1e-6)
+        _close(r["v"][0][s], torch.from_numpy(c).double(), 1e-6)
+
+
+@pytest.mark.parametrize("fused", [False, True])
+@pytest.mark.parametrize("step", [1, 2, 1000, 10 ** 6])
+def test_adam_emulation_within_bound(step, fused):
+    p, g, m, v = _opt_inputs()
+    bc1, bc2 = R.f32(1 - HP["b1"] ** step), R.f32(1 - HP["b2"] ** step)
+    kw = dict(bc1=bc1, bc2=bc2, mul=0.125, **HP)
+    r = R.adam_ref(p, g, m, v, **kw)
+    ep, em, ev, et = _adam_emulate(p, g, m, v, fused=fused, **kw)
+    for got, k in ((ep, "p"), (em, "m"), (ev, "v"), (et, "t")):
+        R.assert_elementwise(got, r[k][0], R.f32_bound(*r[k]), k)
+    e, ed = R.ema_ref(p, r["p"][0], R.f32(0.999), r["p"][1])
+    d32 = torch.tensor(0.999, dtype=torch.float32)
+    emu = (d32 * p.float() + (1 - d32) * ep.float()).double()
+    R.assert_elementwise(emu, e, R.f32_bound(e, ed), "ema")
+
+
+def test_lamb_and_sumsq_emulation_within_bound():
+    p, g, m, v = _opt_inputs(64 * 300)
+    lens = torch.tensor([64, 64, 128, 1024, 64] + [64 * 59] * 3 + [64 * 102])
+    starts = torch.cat([torch.zeros(1, dtype=torch.long), lens.cumsum(0)[:-1]])
+    kw = dict(bc1=R.f32(1 - HP["b1"] ** 5), bc2=R.f32(1 - HP["b2"] ** 5), mul=1.0, **HP)
+    r = R.lamb_ref(p, g, m, v, starts, lens, **kw)
+    _, _, _, u = _adam_emulate(p, g, m, v, fused=False, **kw)
+    seg = torch.repeat_interleave(torch.arange(lens.numel()), lens)
+    np2 = torch.zeros(lens.numel(), dtype=torch.float32).index_add_(0, seg, (p.float() ** 2))
+    nu2 = torch.zeros(lens.numel(), dtype=torch.float32).index_add_(0, seg, (u.float() ** 2))
+    ratio = torch.sqrt(np2) / torch.sqrt(nu2)
+    a = torch.tensor(kw["lr"], dtype=torch.float32) * ratio
+    pe = (p.float() - a[seg] * u.float()).double()
+    R.assert_elementwise(np2.double(), r["np2"][0], R.f32_bound(*r["np2"]), "sum p^2")
+    R.assert_elementwise(nu2.double(), r["nu2"][0], R.f32_bound(*r["nu2"]), "sum u^2")
+    R.assert_elementwise(pe, r["p"][0], R.f32_bound(*r["p"]), "lamb p")
+    # grad stats: float4 chains, per-thread running sums over the grid-stride loop, then the rest
+    x = (g * 0.125).float()
+    q = (x * x).view(-1, 4).sum(1)                              # 4800 float4 groups: 8 blocks x 256 threads, 3 rounds
+    s = torch.cat([q, q.new_zeros(3 * 2048 - q.numel())]).view(3, 2048).sum(0).sum()
+    val, d = R.sumsq_ref(g, 0.125, R.grad_stats_depth(g.numel(), 1))
+    R.assert_elementwise(s.double().reshape(1), val.reshape(1), R.f32_bound(val, d).reshape(1), "sumsq")
+
+
+def _gelu32(x):
+    k, a = torch.tensor(R.GELU_K, dtype=torch.float32), torch.tensor(R.GELU_A, dtype=torch.float32)
+    return 0.5 * x * (1 + torch.tanh(k * (x + a * x * x * x)))
+
+
+def _gelu_grad32(x):
+    k, a = torch.tensor(R.GELU_K, dtype=torch.float32), torch.tensor(R.GELU_A, dtype=torch.float32)
+    th = torch.tanh(k * (x + a * x * x * x))
+    return 0.5 * (1 + th) + 0.5 * x * (1 - th * th) * k * (1 + 3 * a * x * x)
+
+
+def _temb_inputs(D, B, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    freqs = torch.randn(D // 2, generator=g) * 16
+    t = torch.cat([torch.rand(B // 2, generator=g) * 2.65 - 1.55, torch.randint(0, 1000, (B - B // 2,),
+                                                                               generator=g).float()])
+    W1, W2 = (torch.randn(D, D, generator=g) / math.sqrt(D) for _ in range(2))
+    b1, b2 = (torch.randn(D, generator=g) * 0.1 for _ in range(2))
+    return freqs, t, W1, b1, W2, b2, torch.randn(B, D, generator=g)
+
+
+def test_time_embedding_references_match_autograd():
+    """time_embed_fwd_ref / _bwd_ref against float64 autograd of FourierEmbedding + TimeProjection."""
+    D, B = 64, 9
+    freqs, t, W1, b1, W2, b2, demb = (x.double() for x in _temb_inputs(D, B))
+    ph = R.time_phase_f32(t, freqs).double()
+    four = torch.cat([torch.sin(ph), torch.cos(ph)], 1)
+    P = [x.clone().requires_grad_(True) for x in (W1, b1, W2, b2)]
+    gelu = lambda x: 0.5 * x * (1 + torch.tanh(R.GELU_K * (x + R.GELU_A * x ** 3)))  # noqa: E731
+    h1 = b1 + four @ P[0] + (P[1] - b1)
+    h1.retain_grad()
+    h2 = gelu(h1) @ P[2] + P[3]
+    h2.retain_grad()
+    emb = gelu(h2)
+    (emb * demb).sum().backward()
+    f = R.time_embed_fwd_ref(ph, four, h1.detach(), h2.detach(), W1, b1, W2, b2)
+    _close(f["four"][0], four, 1e-15)
+    _close(f["h1"][0], h1, 1e-13)
+    _close(f["h2"][0], h2, 1e-13)
+    _close(f["emb"][0], emb, 1e-13)
+    z = [torch.zeros_like(x) for x in (W1, b1, W2, b2)]
+    r = R.time_embed_bwd_ref(demb, four, h1.detach(), h2.detach(), h1.grad, h2.grad, W2, *z)
+    _close(r["dh2"][0], h2.grad, 1e-12)
+    _close(r["dh1"][0], h1.grad, 1e-12)
+    for k, x in (("dW1", P[0]), ("db1", P[1]), ("dW2", P[2]), ("db2", P[3])):
+        _close(r[k][0], x.grad, 1e-12)
+
+
+@pytest.mark.parametrize("B", [1, 8, 65])
+def test_time_embedding_emulation_within_bound(B):
+    D = 256
+    freqs, t, W1, b1, W2, b2, demb = _temb_inputs(D, B, 1)
+    ph = R.time_phase_f32(t, freqs)
+    four = torch.cat([torch.sin(ph), torch.cos(ph)], 1)
+    h1 = b1 + four @ W1
+    h2 = b2 + _gelu32(h1) @ W2
+    emb = _gelu32(h2)
+    d = lambda x: x.double()  # noqa: E731
+    f = R.time_embed_fwd_ref(ph, d(four), d(h1), d(h2), d(W1), d(b1), d(W2), d(b2))
+    R.assert_elementwise(d(four), f["four"][0], f["four"][1], "four")
+    for k, x in (("h1", h1), ("h2", h2), ("emb", emb)):
+        R.assert_elementwise(d(x), f[k][0], R.f32_bound(*f[k]), k)
+    dh2 = demb * _gelu_grad32(h2)
+    dh1 = (dh2 @ W2.T) * _gelu_grad32(h1)
+    pri = [torch.randn_like(x) * 0.3 for x in (W1, b1, W2, b2)]
+    got = {"dh2": dh2, "dh1": dh1, "dW1": pri[0] + four.T @ dh1, "db1": pri[1] + dh1.sum(0),
+           "dW2": pri[2] + _gelu32(h1).T @ dh2, "db2": pri[3] + dh2.sum(0)}
+    r = R.time_embed_bwd_ref(d(demb), d(four), d(h1), d(h2), d(dh1), d(dh2), d(W2), *[d(x) for x in pri])
+    for k, x in got.items():
+        R.assert_elementwise(d(x), r[k][0], R.f32_bound(*r[k]), k)
+
+
+@pytest.mark.parametrize("kind", [0, 1, 2])
+def test_diffuse_and_loss_references_and_emulation(kind):
+    """diffuse_ref / loss_ref against a float64 restatement (autograd for dF), and an f32 emulation of the
+    kernels inside their bounds."""
+    g = torch.Generator().manual_seed(kind)
+    B, E = 3, 4096
+    x0 = torch.randint(0, 256, (B, E), generator=g).double()
+    x0[:, :2] = torch.tensor([0.0, 255.0])
+    eps = _fl(torch.randn(B, E, generator=g, dtype=torch.float64))
+    sig = _fl(torch.rand(B, generator=g, dtype=torch.float64) * 3 + 0.01)
+    al = _fl(1 / torch.sqrt(1 + sig * sig))
+    r = R.diffuse_ref(x0, eps, al, sig, True, kind)
+    x = (x0 - 127.5) / 127.5
+    assert x[0, 0].item() == -1.0 and x[0, 1].item() == 1.0
+    want = [x, eps, (al[:, None] * eps - sig[:, None] * x) / torch.sqrt(al * al + sig * sig)[:, None]][kind]
+    _close(r["x_t"][0], al[:, None] * x + sig[:, None] * eps, 1e-14)
+    _close(r["target"][0], want, 1e-14)
+    a32, s32 = al.float()[:, None], sig.float()[:, None]
+    x32 = (x0.float() - 127.5) / 127.5
+    xt32 = a32 * x32 + s32 * eps.float()
+    tg32 = [x32, eps.float(), (a32 * eps.float() - s32 * x32) * torch.rsqrt(a32 * a32 + s32 * s32)][kind]
+    R.assert_elementwise(xt32.double(), r["x_t"][0], R.f32_bound(*r["x_t"]), "x_t")
+    R.assert_elementwise(tg32.double(), r["target"][0], R.f32_bound(*r["target"]), "target")
+    F = _fl(torch.randn(B, E, generator=g, dtype=torch.float64)).requires_grad_(True)
+    co, cs, w = (_fl(torch.rand(B, generator=g, dtype=torch.float64) + 0.2) for _ in range(3))
+    xt, tg = xt32.double(), tg32.double()
+    lr_ = R.loss_ref(F.detach(), xt, tg, co, cs, w, 20)
+    loss = (0.5 * w[:, None] * (co[:, None] * F + cs[:, None] * xt - tg) ** 2).mean()
+    loss.backward()
+    _close(lr_["loss"][0], loss.detach(), 1e-13)
+    _close(lr_["dF"][0], F.grad, 1e-13)
+    d32 = co.float()[:, None] * F.detach().float() + cs.float()[:, None] * xt32 - tg32
+    l32 = (0.5 * w.float()[:, None] * d32 * d32).sum() * torch.tensor(1 / (B * E), dtype=torch.float32)
+    g32 = w.float()[:, None] * co.float()[:, None] * torch.tensor(1 / (B * E), dtype=torch.float32)
+    R.assert_elementwise(l32.double().reshape(1), lr_["loss"][0].reshape(1),
+                         R.f32_bound(*lr_["loss"]).reshape(1), "loss")
+    R.assert_elementwise((g32 * d32).double(), lr_["dF"][0], R.f32_bound(*lr_["dF"]), "dF")
+
+
+def test_training_comparator_rejects_what_relative_l2_accepts():
+    """One parameter of the optimiser's output off by 2^-12 relative, or one DDPM sample's time embedding
+    computed from a phase one f32 ulp off: relative L2 (1e-6, 1e-2) lets them through, the element-wise bound
+    does not."""
+    p, g, m, v = _opt_inputs()
+    kw = dict(bc1=R.f32(1 - HP["b1"] ** 3), bc2=R.f32(1 - HP["b2"] ** 3), mul=0.125, **HP)
+    r = R.adam_ref(p, g, m, v, **kw)
+    got = _adam_emulate(p, g, m, v, fused=False, **kw)[0]
+    got[12345] *= 1 + 2.0 ** -12
+    assert rel(got, r["p"][0]) < 1e-6
+    with pytest.raises(AssertionError, match="outside the bound"):
+        R.assert_elementwise(got, r["p"][0], R.f32_bound(*r["p"]))
+    freqs, t, *_ = _temb_inputs(256, 8, 2)
+    ph = R.time_phase_f32(t, freqs)
+    bad = ph.clone()
+    bad[5] = torch.nextafter(bad[5], torch.tensor(math.inf))
+    four = torch.cat([torch.sin(bad.double()), torch.cos(bad.double())], 1)
+    ref = torch.cat([torch.sin(ph.double()), torch.cos(ph.double())], 1)
+    assert rel(four, ref) < 1e-2
+    with pytest.raises(AssertionError, match="outside the bound"):
+        R.assert_elementwise(four, ref, 2 * R.ulp_f32(ref))
