@@ -364,6 +364,56 @@ def affine_combine(inputs, coef1: torch.Tensor, coef2: Optional[torch.Tensor] = 
     return out1, out2, outb
 
 
+# --------------------------------------------------------------------------- jax.random's threefry streams
+def _random(entry: str, key, shape, dtype, device, out, *args):
+    """Common part of the random_* wrappers.  `key`: two host ints, or a (2,) int32 CUDA tensor holding the two
+    words (read by the kernel when it runs: the form a captured graph takes)."""
+    shape = (shape,) if isinstance(shape, int) else tuple(int(d) for d in shape)
+    if any(d < 0 for d in shape):
+        raise _lib.FdxError(f"{entry}: negative dimension in shape {shape}")
+    n = 1
+    for d in shape:
+        n *= d
+    if out is None:
+        device = torch.device("cuda" if device is None else device)
+        if device.type != "cuda":
+            raise _lib.FdxError(f"{entry}: expected a CUDA device (flaxdiff_b200 has no CPU path)")
+        out = torch.empty(shape, dtype=dtype, device=device)
+    elif out.dtype != dtype or out.numel() != n or not out.is_contiguous():
+        raise _lib.FdxError(f"{entry}: out must be a contiguous {dtype} tensor of {n} elements")
+    if isinstance(key, torch.Tensor):
+        if key.dtype != torch.int32 or key.numel() != 2 or not key.is_contiguous():
+            raise _lib.FdxError(f"{entry}: a device key is a contiguous (2,) int32 tensor")
+        k0, k1, key_dev = 0, 0, ptr(key)
+    else:
+        k0, k1, key_dev = int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF, ptr(None)
+    check(getattr(load(), "fdx_" + entry)(ctypes.c_uint32(k0), ctypes.c_uint32(k1), key_dev, ctypes.c_longlong(n),
+                                          *args, ptr(out), stream_ptr()), entry)
+    return out
+
+
+def random_bits(key, shape, device=None, out=None) -> torch.Tensor:
+    """jax.random.bits(key, shape, uint32); the words are returned in an int32 tensor (same bits)."""
+    return _random("random_bits", key, shape, torch.int32, device, out)
+
+
+def random_uniform(key, shape, minval: float = 0.0, maxval: float = 1.0, device=None, out=None) -> torch.Tensor:
+    """jax.random.uniform(key, shape, float32, minval, maxval)."""
+    return _random("random_uniform", key, shape, torch.float32, device, out,
+                   ctypes.c_float(minval), ctypes.c_float(maxval))
+
+
+def random_normal(key, shape, device=None, out=None) -> torch.Tensor:
+    """jax.random.normal(key, shape, float32)."""
+    return _random("random_normal", key, shape, torch.float32, device, out)
+
+
+def random_randint(key, shape, minval: int, maxval: int, device=None, out=None) -> torch.Tensor:
+    """jax.random.randint(key, shape, minval, maxval, int32), minval < maxval."""
+    return _random("random_randint", key, shape, torch.int32, device, out,
+                   ctypes.c_int(int(minval)), ctypes.c_int(int(maxval)))
+
+
 def adamw_ema_step(p, g, m, v, ema, shadow, lr, b1, b2, eps, weight_decay, step, ema_decay,
                    grad_scale: float = 1.0, gnorm_sq=None, clip_norm: float = 0.0, dyn=None):
     check(load().fdx_adamw_ema_step(ptr(p), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(shadow),

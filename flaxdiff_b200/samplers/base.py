@@ -68,6 +68,17 @@ class _GraphedEval:
         return tuple(o.clone() for o in outs)
 
 
+class _DeviceKeyState:
+    """The RandomMarkovState a whole-step capture hands to `take_next_step`: every subkey it gives out is the key
+    held in `words` (a (2,) int32 device tensor) at replay time.  One draw per step (see _noise_per_step)."""
+
+    def __init__(self, words: torch.Tensor):
+        self.words = words
+
+    def get_random_key(self):
+        return self, utils.DeviceKey(self.words)
+
+
 class DiffusionSampler:
     def __init__(self, model, noise_schedule: NoiseScheduler,
                  model_output_transform: DiffusionPredictionTransform, input_config=None,
@@ -126,8 +137,14 @@ class DiffusionSampler:
     # captures the WHOLE step - model evaluation(s) + the (B,)-sized coefficient algebra + the update kernel -
     # in one CUDA graph with (x, current_step, next_step) as inputs, so a denoise step is one replay instead
     # of a replay plus ~30 tiny un-graphed launches (the reference runs them as un-jitted XLA dispatches,
-    # SURVEY.md $3.2).  Samplers that draw noise or keep Python-side history use the per-evaluation graph.
+    # SURVEY.md $3.2).  Samplers that keep Python-side history use the per-evaluation graph.
     _whole_step_graph = False
+    # Update rules that draw exactly one noise tensor per step (EulerAncestral, DDPM, SimpleDDPM, DDIM eta>0) set
+    # this.  With a `utils.ThreefryKey` in the RandomMarkovState they take the whole-step graph too: the noise is
+    # an fdx_random_normal launch inside the graph that reads its key from 8 bytes of device memory; the host runs
+    # the `split` chain of the eager steps ahead of the loop and each replay is handed its subkey.  A plain
+    # tuple key draws from a torch.Generator, which a graph cannot re-seed: per-evaluation graph, as before.
+    _noise_per_step = False
     MAX_GRAPHS = 4      # captured graphs kept per sampler (each owns a private memory pool)
     MAX_TREES = 2       # flax-tree -> FlatParams conversions kept per sampler
 
@@ -173,24 +190,28 @@ class DiffusionSampler:
             self._graphs.move_to_end(key)
         return ge(x_t, t, *conditioning_inputs)
 
-    def _graphed_step(self, fp, x, cur, nxt, conds):
-        """One full sampler step through a captured graph (see _whole_step_graph)."""
-        key = ("step", id(fp), tuple(x.shape), tuple((tuple(c.shape), c.dtype) for c in conds))
+    def _graphed_step(self, fp, x, cur, nxt, conds, key_words=None):
+        """One full sampler step through a captured graph (see _whole_step_graph).  `key_words`: the subkey this
+        step's noise is drawn from, as a (2,) int32 device tensor (see _noise_per_step); None for a deterministic
+        update rule."""
+        keyed = [] if key_words is None else [key_words]
+        key = ("step", id(fp), tuple(x.shape), len(keyed), tuple((tuple(c.shape), c.dtype) for c in conds))
         ge = self._graphs.get(key)
         fp.shadow()
         if ge is None:
-            def fn(a, c, n, *cc):
+            def fn(a, c, n, *rest):
                 def smf(x_t, t, *add):
                     return self.sample_model(fp, x_t, t, *add)
-                out, _ = self.sample_step(smf, a, c, list(cc), next_step=n, state=None)
+                state, cc = (_DeviceKeyState(rest[0]), rest[1:]) if keyed else (None, rest)
+                out, _ = self.sample_step(smf, a, c, list(cc), next_step=n, state=state)
                 return out
-            ge = _GraphedEval(fn, [x, cur, nxt, *conds])
+            ge = _GraphedEval(fn, [x, cur, nxt, *keyed, *conds])
             self._graphs[key] = ge
             while len(self._graphs) > self.MAX_GRAPHS:
                 self._graphs.popitem(last=False)
         else:
             self._graphs.move_to_end(key)
-        return ge(x, cur, nxt, *conds, clone=False)[0]
+        return ge(x, cur, nxt, *keyed, *conds, clone=False)[0]
 
     def post_process(self, samples: torch.Tensor) -> torch.Tensor:
         ones = torch.ones((1, samples.shape[0]), dtype=torch.float32, device=samples.device)
@@ -279,16 +300,25 @@ class DiffusionSampler:
         steps = steps_override if steps_override is not None else self.get_steps(start_step, end_step, diffusion_steps)
         steps = [float(s) for s in np.asarray(steps).tolist()]
         n = len(steps)
-        whole = self.use_cuda_graph and self._whole_step_graph and n > 1
+        keyed = self._noise_per_step and isinstance(getattr(rngstate, "rng", None), utils.ThreefryKey)
+        whole = self.use_cuda_graph and (self._whole_step_graph or keyed) and n > 1
         if whole:
             # per-step (B,) step tensors, built once: rows are views, no per-step fill kernels
             tab = torch.tensor([self.scale_steps(s) for s in steps] + [self.scale_steps(0)], dtype=torch.float32,
                                device=device).unsqueeze(1).expand(n + 1, samples.shape[0]).contiguous()
+        if whole and keyed:
+            # the subkeys of all steps, in one upload: row i is what step i's take_next_step would split off
+            subkeys = []
+            for _ in range(n - 1):
+                rngstate, subkey = rngstate.get_random_key()
+                subkeys.append(subkey)
+            keytab = torch.from_numpy(np.asarray(subkeys, dtype=np.uint32).view(np.int32)).to(device)
         for i in range(n):
             current_step = self.scale_steps(steps[i])
             next_step = self.scale_steps(steps[i + 1] if i + 1 < n else 0)
             if i != n - 1 and whole:
-                samples = self._graphed_step(params, samples, tab[i], tab[i + 1], tuple(model_conditioning_inputs))
+                samples = self._graphed_step(params, samples, tab[i], tab[i + 1], tuple(model_conditioning_inputs),
+                                             keytab[i] if keyed else None)
             elif i != n - 1:
                 samples, rngstate = self.sample_step(sample_model_fn, samples, current_step,
                                                      model_conditioning_inputs, next_step=next_step, state=rngstate)

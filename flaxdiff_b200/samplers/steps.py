@@ -52,6 +52,8 @@ class SimplifiedEulerSampler(DiffusionSampler):
 
 
 class EulerAncestralSampler(DiffusionSampler):
+    _noise_per_step = True
+
     def take_next_step(self, current_samples, reconstructed_samples, model_conditioning_inputs, pred_noise,
                        current_step, state: RandomMarkovState, sample_model_fn, next_step=1):
         ca, cs = _rates(self.noise_schedule, current_step)
@@ -88,7 +90,8 @@ class DDIMSampler(DiffusionSampler):
     def __init__(self, *args, eta=0.0, **kwargs):
         super().__init__(*args, **kwargs)
         self.eta = eta
-        self._whole_step_graph = (eta == 0)      # eta > 0 draws noise per step
+        self._whole_step_graph = (eta == 0)
+        self._noise_per_step = (eta > 0)
 
     def take_next_step(self, current_samples, reconstructed_samples, model_conditioning_inputs, pred_noise,
                        current_step, state: RandomMarkovState, sample_model_fn, next_step=1):
@@ -105,6 +108,8 @@ class DDIMSampler(DiffusionSampler):
 
 
 class DDPMSampler(DiffusionSampler):
+    _noise_per_step = True
+
     def take_next_step(self, current_samples, reconstructed_samples, model_conditioning_inputs, pred_noise,
                        current_step, state: RandomMarkovState, sample_model_fn, next_step=1):
         c0, ct = self.noise_schedule.get_posterior_coeffs(current_step)
@@ -120,6 +125,8 @@ class DDPMSampler(DiffusionSampler):
 
 
 class SimpleDDPMSampler(DiffusionSampler):
+    _noise_per_step = True
+
     def take_next_step(self, current_samples, reconstructed_samples, model_conditioning_inputs, pred_noise,
                        current_step, state: RandomMarkovState, sample_model_fn, next_step=1):
         state, rng = state.get_random_key()

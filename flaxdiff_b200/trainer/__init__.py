@@ -454,8 +454,10 @@ class GeneralDiffusionTrainer:
         self.distributed_training = (self.world_size > 1) if distributed_training is None else distributed_training
         if isinstance(rngs, int):
             rngs = utils.PRNGKey(rngs)
-        self.rngstate = RandomMarkovState(tuple(rngs))
-        self.state, self.best_state = self.generate_states(optimizer, tuple(rngs), model=model,
+        if not isinstance(rngs, utils.ThreefryKey):      # a ThreefryKey keeps its type: it selects JAX's streams
+            rngs = tuple(rngs)
+        self.rngstate = RandomMarkovState(rngs)
+        self.state, self.best_state = self.generate_states(optimizer, rngs, model=model,
                                                            use_dynamic_scale=use_dynamic_scale)
         self.best_loss = 1e9
         self.latest_step = 0
@@ -598,7 +600,7 @@ class GeneralDiffusionTrainer:
             if self.input_config.conditions:
                 # per-sample unconditional mask (bernoulli p = unconditional_prob) and null-embedding mixing
                 # (general_diffusion_trainer.py:266-275; inputs/__init__.py:123-146)
-                mask = utils.device_uniform(uncond_key, (B,), dev) < self.unconditional_prob
+                mask = utils.device_bernoulli(uncond_key, self.unconditional_prob, (B,), dev)
                 ctx = self.input_config.process_conditioning(batch, uncond_mask=mask)[0]
                 ctx = ctx.to(device=dev, dtype=torch.float32).contiguous()
             noise_level, local = self.noise_schedule.generate_timesteps(B, local)
@@ -851,7 +853,8 @@ class GeneralDiffusionTrainer:
         if isinstance(r, dict):
             r = r.get("rng")
         if r is not None:
-            self.rngstate = RandomMarkovState(tuple(int(x) for x in np.asarray(r).reshape(-1)[:2]))
+            # the checkpoint holds the words; which stream they draw from is this trainer's choice (its `rngs`)
+            self.rngstate = RandomMarkovState(utils.key_like(self.rngstate.rng, np.asarray(r).reshape(-1)[:2]))
         self.best_loss = float(np.asarray(ck["best_loss"]))
         if self.best_loss == 0:
             self.best_loss = 1e9

@@ -4,9 +4,19 @@
 trainer and samplers.  Keys here are threefry2x32 keys with JAX's `split` / `fold_in`
 semantics (jax/_src/prng.py; JAX is not installable here, so the construction is a
 restatement checked against the published Random123 known-answer vectors in
-tests/test_prng.py).  Bulk device noise is drawn with a torch.Generator seeded from the
-key: statistically equivalent, not bit-identical, to `jax.random.normal` - parity tests
-therefore inject identical (x0, eps, t) tensors on both sides, as SURVEY.md $8(c) says.
+tests/test_prng.py).
+
+Which stream a key draws from is chosen where the key is made, by its type:
+  * a plain tuple (`PRNGKey(seed)`, the default everywhere) draws bulk device tensors with a
+    torch.Generator seeded from the key: statistically equivalent, not bit-identical, to
+    `jax.random.normal` - parity tests therefore inject identical (x0, eps, t) tensors on both
+    sides, as SURVEY.md $8(c) says;
+  * a `ThreefryKey` (`jax_key(seed)`, same two words) draws them with the libfdx kernels of
+    csrc/fdx_random.cu, which restate jax.random.{bits, uniform, normal, randint, bernoulli} of
+    JAX 0.4.28 (jax_threefry_partitionable=False).  `split`, `fold_in` and
+    `RandomMarkovState.get_random_key` return the type they were given, so the choice flows through
+    samplers, schedulers and the trainer.  `uniform`, `normal_f32`, `randint` and `bernoulli` below
+    are the host restatements those kernels are held to, bit for bit.
 """
 from __future__ import annotations
 
@@ -15,6 +25,9 @@ from typing import Tuple
 
 import numpy as np
 import torch
+
+from . import ops
+from ._lib import FdxError
 
 _U32 = np.uint32
 _ROT = ((13, 15, 26, 6), (17, 29, 16, 24))
@@ -54,14 +67,37 @@ def PRNGKey(seed: int) -> Tuple[int, int]:
     return ((seed >> 32) & 0xFFFFFFFF, seed & 0xFFFFFFFF)
 
 
+class ThreefryKey(tuple):
+    """A threefry key (two uint32 words) whose device draws are jax.random's own streams."""
+    __slots__ = ()
+
+    def __new__(cls, words):
+        k0, k1 = (int(w) & 0xFFFFFFFF for w in words)
+        return super().__new__(cls, (k0, k1))
+
+    def __repr__(self):
+        return f"ThreefryKey(({self[0]}, {self[1]}))"
+
+
+def jax_key(seed: int) -> ThreefryKey:
+    """`jax.random.PRNGKey(seed)`: the words of `PRNGKey(seed)`, drawing from JAX's streams."""
+    return ThreefryKey(PRNGKey(seed))
+
+
+def key_like(key, words):
+    """A key with `words`, of the stream `key` draws from."""
+    words = (int(words[0]), int(words[1]))
+    return ThreefryKey(words) if isinstance(key, ThreefryKey) else words
+
+
 def split(key: Tuple[int, int], num: int = 2):
     bits = _random_bits32(key, 2 * num).reshape(num, 2)
-    return [(int(r[0]), int(r[1])) for r in bits]
+    return [key_like(key, r) for r in bits]
 
 
 def fold_in(key: Tuple[int, int], data: int) -> Tuple[int, int]:
     a, b = threefry2x32(key, np.array([0], dtype=_U32), np.array([int(data) & 0xFFFFFFFF], dtype=_U32))
-    return (int(a[0]), int(b[0]))
+    return key_like(key, (a[0], b[0]))
 
 
 def uniform01(key: Tuple[int, int], n: int) -> np.ndarray:
@@ -81,26 +117,120 @@ def normal(key: Tuple[int, int], n: int) -> np.ndarray:
     return (np.float32(np.sqrt(2.0)) * erfinv(u.astype(np.float64)).astype(np.float32)).astype(np.float32)
 
 
+# ---------------------------------------------------------------------------------------------------------
+# host restatements of jax.random's draws (JAX 0.4.28): the specification of csrc/fdx_random.cu
+# ---------------------------------------------------------------------------------------------------------
+_F32 = np.float32
+_NORMAL_LO = np.nextafter(_F32(-1.0), _F32(0.0))
+# Giles (2010), "Approximating the erfinv function", single precision, as XLA's erf_inv evaluates it
+_ERFINV_CENTRAL = (2.81022636e-08, 3.43273939e-07, -3.5233877e-06, -4.39150654e-06, 0.00021858087,
+                   -0.00125372503, -0.00417768164, 0.246640727, 1.50140941)
+_ERFINV_TAIL = (-0.000200214257, 0.000100950558, 0.00134934322, -0.00367342844, 0.00573950773,
+                -0.0076224613, 0.00943887047, 1.00167406, 2.83297682)
+
+
+def uniform(key: Tuple[int, int], n: int, minval=0.0, maxval=1.0) -> np.ndarray:
+    """jax.random.uniform(key, (n,), float32, minval, maxval): every operation rounded to float32."""
+    minval, maxval = _F32(minval), _F32(maxval)
+    return np.maximum(minval, uniform01(key, n) * _F32(maxval - minval) + minval).astype(_F32)
+
+
+def erfinv_f32(u: np.ndarray) -> np.ndarray:
+    """XLA's float32 erf_inv for |u| < 1, one float32 rounding per operation (no fused multiply-add)."""
+    u = np.asarray(u, dtype=_F32)
+    w = -np.log1p(-u * u).astype(_F32)
+    central = w < _F32(5.0)
+    with np.errstate(invalid="ignore"):
+        w = np.where(central, w - _F32(2.5), np.sqrt(w) - _F32(3.0)).astype(_F32)
+    p = np.where(central, _F32(_ERFINV_CENTRAL[0]), _F32(_ERFINV_TAIL[0])).astype(_F32)
+    for c, t in zip(_ERFINV_CENTRAL[1:], _ERFINV_TAIL[1:]):
+        p = (np.where(central, _F32(c), _F32(t)).astype(_F32) + p * w).astype(_F32)
+    return (p * u).astype(_F32)
+
+
+def normal_f32(key: Tuple[int, int], n: int) -> np.ndarray:
+    """jax.random.normal(key, (n,), float32) with XLA's float32 erf_inv polynomial instead of SciPy's float64
+    erfinv (`normal` above): what the device kernel computes."""
+    return (_F32(np.sqrt(2.0)) * erfinv_f32(uniform(key, n, _NORMAL_LO, 1.0))).astype(_F32)
+
+
+def randint(key: Tuple[int, int], n: int, minval: int, maxval: int) -> np.ndarray:
+    """jax.random.randint(key, (n,), minval, maxval, int32) for minval < maxval: two 32-bit draws combined so
+    that the modulo bias is that of a 64-bit draw.  Restated from jax/_src/random.py; no JAX was at hand to pin
+    it against."""
+    if not minval < maxval:
+        raise ValueError(f"randint: minval={minval} must be below maxval={maxval}")
+    k1, k2 = split(key)
+    hi, lo = _random_bits32(k1, n), _random_bits32(k2, n)
+    span = _U32((int(maxval) - int(minval)) & 0xFFFFFFFF)
+    mult = _U32(65536) % span
+    with np.errstate(over="ignore"):
+        mult = _U32(mult * mult) % span
+        off = ((hi % span) * mult + (lo % span)).astype(_U32) % span
+        return (off + _U32(int(minval) & 0xFFFFFFFF)).astype(_U32).view(np.int32)
+
+
+def bernoulli(key: Tuple[int, int], p: float, n: int) -> np.ndarray:
+    """jax.random.bernoulli(key, p, (n,)) = uniform(key, (n,)) < p."""
+    return uniform(key, n) < _F32(p)
+
+
 def key_to_seed(key: Tuple[int, int]) -> int:
     return ((int(key[0]) << 32) | int(key[1])) & 0x7FFFFFFFFFFFFFFF
 
 
+class DeviceKey:
+    """The two words of a `ThreefryKey` in device memory (a (2,) int32 tensor): a captured CUDA graph draws
+    from whatever key those 8 bytes hold when it is replayed."""
+
+    def __init__(self, words: torch.Tensor):
+        self.words = words
+
+
+def _threefry_words(key):
+    """The `ops.random_*` key argument for a key that draws from JAX's streams, else None."""
+    if isinstance(key, DeviceKey):
+        return key.words
+    return key if isinstance(key, ThreefryKey) else None
+
+
+def _f32_only(dtype):
+    if dtype != torch.float32:
+        raise FdxError(f"a ThreefryKey draws float32 only, not {dtype}")
+
+
 def device_normal(key: Tuple[int, int], shape, device, dtype=torch.float32) -> torch.Tensor:
+    words = _threefry_words(key)
+    if words is not None:
+        _f32_only(dtype)
+        return ops.random_normal(words, shape, device=device)
     g = torch.Generator(device=device)
     g.manual_seed(key_to_seed(key))
     return torch.randn(shape, generator=g, device=device, dtype=dtype)
 
 
 def device_uniform(key: Tuple[int, int], shape, device, dtype=torch.float32) -> torch.Tensor:
+    words = _threefry_words(key)
+    if words is not None:
+        _f32_only(dtype)
+        return ops.random_uniform(words, shape, device=device)
     g = torch.Generator(device=device)
     g.manual_seed(key_to_seed(key))
     return torch.rand(shape, generator=g, device=device, dtype=dtype)
 
 
 def device_randint(key: Tuple[int, int], shape, low: int, high: int, device) -> torch.Tensor:
+    words = _threefry_words(key)
+    if words is not None:
+        return ops.random_randint(words, shape, low, high, device=device)
     g = torch.Generator(device=device)
     g.manual_seed(key_to_seed(key))
     return torch.randint(low, high, shape, generator=g, device=device, dtype=torch.int32)
+
+
+def device_bernoulli(key: Tuple[int, int], p: float, shape, device) -> torch.Tensor:
+    """jax.random.bernoulli: `uniform < p`, on the stream `key` draws from."""
+    return device_uniform(key, shape, device) < p
 
 
 class MarkovState:

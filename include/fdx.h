@@ -200,6 +200,27 @@ int fdx_loss_fwd_bwd(const float* F, const float* x_t, const float* target, cons
 int fdx_affine_combine(int n_in, const float* const* inputs, const float* coef1, const float* coef2,
                        const float* bf16_scale, int B, long long E, float* out1, float* out2,
                        void* out_bf16, int clip, float clip_lo, float clip_hi, void* stream);
+/* ---- jax.random's threefry streams (fdx_random.cu) ---------------------------------------------
+ * The draws of jax.random.{bits, uniform, normal, randint} for a threefry2x32 key, as JAX 0.4.28 lays them out with
+ * jax_threefry_partitionable=False: x_T and the per-step noise of the samplers (samplers/common.py:253-260,
+ * euler.py:39-56, ddpm.py:6-37), the trainer's noise, timesteps and unconditional mask
+ * (trainer/general_diffusion_trainer.py:266-283).  A draw of any shape is the flat draw of n elements, row-major.
+ * The key is (k0, k1), or - when key_dev is non-null - the two words at key_dev in device memory, read by the
+ * kernel: a captured graph is replayed with a new key by overwriting those 8 bytes.  0 <= n <= 2^31-1; `out` needs
+ * 4-byte alignment only.  split / fold_in stay on the host (two threefry blocks).
+ *   bits:    m = ceil(n/2); threefry2x32(key, [0..m), [m..2m)), the two outputs concatenated, first n words.
+ *   uniform: f = bitcast((bits >> 9) | 0x3F800000) - 1; max(minval, f*(maxval-minval) + minval), every
+ *            operation rounded to f32 on its own.  minval < maxval.
+ *   normal:  sqrt(2) * erfinv(uniform(nextafter(-1, 0), 1)) with XLA's f32 erf_inv polynomial (Giles 2010).
+ *   randint: k1, k2 = split(key); hi = bits(k1), lo = bits(k2); span = maxval - minval;
+ *            mult = (2^16 mod span)^2 mod span; minval + ((hi mod span)*mult + lo mod span) mod span in wrapping
+ *            uint32 arithmetic.  minval < maxval. */
+int fdx_random_bits(uint32_t k0, uint32_t k1, const uint32_t* key_dev, long long n, uint32_t* out, void* stream);
+int fdx_random_uniform(uint32_t k0, uint32_t k1, const uint32_t* key_dev, long long n, float minval, float maxval,
+                       float* out, void* stream);
+int fdx_random_normal(uint32_t k0, uint32_t k1, const uint32_t* key_dev, long long n, float* out, void* stream);
+int fdx_random_randint(uint32_t k0, uint32_t k1, const uint32_t* key_dev, long long n, int minval, int maxval,
+                       int32_t* out, void* stream);
 /* ---- optimiser / EMA / loss scaling over ONE flat f32 buffer (fdx_optim.cu) -------------------- */
 /* optax.adam / adamw / lamb (+ optax.clip_by_global_norm) as flax TrainState.apply_gradients does them
  * (training.py:263-267,594-608; trainer/general_diffusion_trainer.py:311,327), fused with
