@@ -224,15 +224,309 @@ def gn_backward_ref(x, dy, gamma_, beta_, G, eps, silu, dy_delta=None):
     return out
 
 
-def conv3x3_dgrad_ref(dy, w_hwio):
-    """d/dx of a 3x3 SAME cross-correlation (HWIO weights), NHWC -> (value, delta of the tensor-core engine):
-    K = 9 Cout exact products accumulated in f32 (TC_ADD each), plus <= 16 split-K / epilogue additions."""
-    W = w_hwio.to(torch.float64).permute(3, 2, 0, 1)       # (Cout, Cin, 3, 3)
+# ----------------------------------------------------------------------------------------------- convolutions
+# The convolution and GEMM engines (fdx_tc.cu, fdx_tct.cu, fdx_wgrad9.cu, fdx_upconv.cu, the 3-channel paths of
+# ops.py).  Every reference returns (value, delta) with delta = depth TC_ADD mag: mag is the same operation on
+# |inputs| (the sum of |terms| of each output), depth the longest chain of f32 additions the kernel makes:
+#   * the K-long accumulation of one tile (9 Cin taps forward, taps x Cout data gradient, the pixels of one split
+#     of a weight gradient), counted from the launch code below;
+#   * EPI = 16 further roundings: the epilogue's alpha, bias, row vector, residual or prior.  A split-K reduction
+#     adds one level per split (red.global.add / atomics in any order) and a prior that is accumulated onto, one.
+# Where an operand is rounded to bf16 before the tensor cores read it (the packed sub-pixel weights, the master
+# weights of the 3-channel convolutions, conv_out's loss gradient), delta has U_BF16 on that operand explicitly.
+# The references run in float64 on the device, over chunks of `chunk` images.
+EPI = 16
+
+
+def _pads(stride: int, H: int, W: int):
+    """flax SAME for a 3x3 kernel, low side (the high side is 1): (1, 1) at stride 1; at stride 2, 0 on even and
+    1 on odd sizes (fdx_api_tc.cu)."""
+    if stride == 1:
+        return 1, 1
+    return (0 if H % 2 == 0 else 1), (0 if W % 2 == 0 else 1)
+
+
+def _conv(x, w_hwio, stride):
+    """float64 3x3 SAME cross-correlation, NHWC x HWIO -> NHWC."""
+    ph, pw = _pads(stride, x.shape[1], x.shape[2])
+    xp = Fnn.pad(x.to(torch.float64).permute(0, 3, 1, 2), (pw, 1, ph, 1))
+    return Fnn.conv2d(xp, w_hwio.to(torch.float64).permute(3, 2, 0, 1), stride=stride).permute(0, 2, 3, 1)
+
+
+def _dconv(dy, w_hwio, stride, H, W):
+    """Adjoint of _conv onto an (H, W) input."""
+    ph, pw = _pads(stride, H, W)
     d = dy.to(torch.float64).permute(0, 3, 1, 2)
-    val = Fnn.conv_transpose2d(d, W, padding=1).permute(0, 2, 3, 1)
-    mag = Fnn.conv_transpose2d(d.abs(), W.abs(), padding=1).permute(0, 2, 3, 1)
-    K = 9 * w_hwio.shape[-1]
-    return val, (K + 16) * TC_ADD * mag
+    full = Fnn.conv_transpose2d(d, w_hwio.to(torch.float64).permute(3, 2, 0, 1), stride=stride)
+    return full[:, :, ph:ph + H, pw:pw + W].permute(0, 2, 3, 1)
+
+
+def _chunks(N, chunk):
+    return [slice(i, min(N, i + chunk)) for i in range(0, N, chunk)]
+
+
+def _plus(val, mag, *terms):
+    """Add epilogue terms (bias, row vector, residual, prior; None skipped) to a value and its magnitude."""
+    for t in terms:
+        if t is not None:
+            t = t.to(torch.float64)
+            val, mag = val + t, mag + t.abs()
+    return val, mag
+
+
+def conv3x3_fwd_ref(x, w_hwio, stride: int = 1, bias=None, rowvec=None, res=None, chunk: int = 64):
+    """fdx_conv3x3_fwd: y = conv(x, w) + bias + rowvec[n] + res, NHWC / HWIO.  One accumulator chains all nine
+    taps: depth 9 Cin + EPI."""
+    N = x.shape[0]
+    val = torch.cat([_conv(x[s], w_hwio, stride) for s in _chunks(N, chunk)])
+    mag = torch.cat([_conv(x[s].abs(), w_hwio.abs(), stride) for s in _chunks(N, chunk)])
+    rv = None if rowvec is None else rowvec.reshape(N, 1, 1, -1)
+    val, mag = _plus(val, mag, bias, rv, res)
+    return val, (9 * x.shape[-1] + EPI) * TC_ADD * mag
+
+
+def conv3x3_dgrad_ref(dy, w_hwio, stride: int = 1, prior=None, chunk: int = 64):
+    """d/dx of a 3x3 SAME cross-correlation (HWIO weights), NHWC -> (value, delta of the tensor-core engine).
+    Stride 1: one launch of K = 9 Cout.  Stride 2 (even input sizes): four output-parity launches with 4, 2, 2
+    and 1 taps, the longest K = 4 Cout.  `prior`: the bf16 dx that accumulate=True adds to."""
+    N, Ho, Wo, Cout = dy.shape
+    H, W = Ho * stride, Wo * stride
+    val = torch.cat([_dconv(dy[s], w_hwio, stride, H, W) for s in _chunks(N, chunk)])
+    mag = torch.cat([_dconv(dy[s].abs(), w_hwio.abs(), stride, H, W) for s in _chunks(N, chunk)])
+    val, mag = _plus(val, mag, prior)
+    K = (9 if stride == 1 else 4) * Cout
+    return val, (K + EPI) * TC_ADD * mag
+
+
+def _wgrad(x, dy, stride, absolute, chunk):
+    """sum over images and output pixels of x[n, s oy + ky - ph, s ox + kx - pw, ci] dy[n, oy, ox, co]."""
+    N, Ho, Wo, Co = dy.shape
+    Ci = x.shape[-1]
+    ph, pw = _pads(stride, x.shape[1], x.shape[2])
+    out = torch.zeros(3, 3, Ci, Co, dtype=torch.float64, device=dy.device)
+    for s in _chunks(N, chunk):
+        xs, d = x[s].to(torch.float64), dy[s].to(torch.float64).reshape(-1, Co)
+        if absolute:
+            xs, d = xs.abs(), d.abs()
+        xp = Fnn.pad(xs, (0, 0, pw, 1, ph, 1))
+        for ky in range(3):
+            for kx in range(3):
+                tap = xp[:, ky:ky + stride * (Ho - 1) + 1:stride, kx:kx + stride * (Wo - 1) + 1:stride]
+                out[ky, kx] += tap.reshape(-1, Ci).T @ d
+    return out
+
+
+def conv3x3_wgrad_ref(x, dy, depth: int, stride: int = 1, prior=None, chunk: int = 16):
+    """fdx_conv3x3_wgrad: dw (f32 HWIO) = prior + sum_pixels x (shifted by the tap) dy.  `depth` from
+    wgrad9_depth or mnmn_depth (it includes the prior)."""
+    val, mag = _plus(_wgrad(x, dy, stride, False, chunk), _wgrad(x, dy, stride, True, chunk), prior)
+    return val, depth * TC_ADD * mag
+
+
+def split_count(sms: int, base_tiles: int, kblocks: int) -> int:
+    """The wave-aware split-K count of fdx_tc.cu (TC_MNMN) and fdx_wgrad9.cu: the split whose tile total fills
+    w = 1..4 waves of `sms` SMs best, more waves only for > 3 % more fill; at most one split per pixel block."""
+    best, splits = -1.0, 1
+    for w in range(1, 5):
+        sp = min(max(1, (sms * w) // base_tiles), kblocks)
+        tiles = base_tiles * sp
+        eff = tiles / (math.ceil(tiles / sms) * sms)
+        if eff > best + 0.03:
+            best, splits = eff, sp
+    return min(splits, kblocks)
+
+
+def wgrad9_depth(N: int, H: int, W: int, Cin: int, Cout: int, sms: int) -> int:
+    """fdx_wgrad9_launch: 64-pixel blocks (TW = 16 for W >= 16, else 8), split over the pixel blocks; each split
+    chains 64 products per block, then one red.global.add per split onto the prior."""
+    TW = 16 if W >= 16 else 8
+    kblocks = (W // TW) * (H // (64 // TW)) * N
+    splits = split_count(sms, math.ceil(Cin / 64) * math.ceil(Cout / 64), kblocks)
+    return 64 * math.ceil(kblocks / splits) + splits + 1
+
+
+def _pow2_floor(v: int) -> int:
+    return 1 << (max(1, v).bit_length() - 1)
+
+
+def tc_bn(ncols: int) -> int:
+    """fdx_tc_launch's column tile: the first of 256 / 128 / 64 minimising ceil(ncols / bn) (bn + 64)."""
+    return min((256, 128, 64), key=lambda bn: math.ceil(ncols / bn) * (bn + 64))
+
+
+def mnmn_depth(W: int, H: int, N: int, M: int, Ncols: int, ntaps: int, sms: int, gemm: bool = False,
+               b_view: bool = False, splits: int = 0, mn_batched: bool = False) -> int:
+    """fdx_tc_launch in TC_MNMN (the generic weight gradient and the GEMM_MNMN reductions): 64-row pixel tiles
+    (a TW x TH x TN box for convolutions, 64 rows of K for GEMMs), split over the pixel blocks (`splits` 0 =
+    the wave-aware count); depth = rows per split + one level per split + the prior."""
+    if gemm:
+        TW, TH, TN = 64, 1, 1
+    else:
+        TW = _pow2_floor(min(W, 16))
+        TH = _pow2_floor(min(H, 64 // TW))
+        TN = 64 // TW // TH
+    nxb, nyb, nnb = math.ceil(W / TW), math.ceil(H / TH), math.ceil(N / TN)
+    tpp = 2 if (M <= 64 and ntaps > 1 and not b_view) else 1
+    base = math.ceil(ntaps / tpp) * math.ceil(M / 128) * math.ceil(Ncols / tc_bn(Ncols))
+    kblocks = nxb if mn_batched else nxb * nyb * nnb
+    nbz = nyb * nnb if mn_batched else 1
+    sp = split_count(sms, base * nbz, kblocks) if splits <= 0 else min(splits, kblocks)
+    return 64 * math.ceil(kblocks / sp) + sp + 1
+
+
+def gemm_ref(a, b, depth: int, alpha: float = 1.0, bias=None, res=None, prior=None):
+    """fdx_gemm: D = alpha a @ b + bias + res (+ the prior of an atomic D), a (..., M, K), b (..., K, N) float64
+    views of the operands in any GEMM_KK / GEMM_KMN / GEMM_MNMN layout.  depth: K + EPI, or mnmn_depth."""
+    a, b = a.to(torch.float64), b.to(torch.float64)
+    val, mag = _plus(alpha * (a @ b), abs(alpha) * (a.abs() @ b.abs()), bias, res, prior)
+    return val, depth * TC_ADD * mag
+
+
+# sub-pixel upsample convolution (fdx_upconv.cu): output parity (py, px) reads low-resolution row
+# i + (slot - 1 + py) through the sum of the 3x3 taps that land on the same source pixel
+def up_slot(parity: int, k: int) -> int:
+    return (1 if k >= 1 else 0) if parity == 0 else (1 if k == 2 else 0)
+
+
+def upconv_pack_ref(w_hwio):
+    """upconv_pack_kernel restated: per parity (py, px), the f32 taps added in (ky, kx) order into slot
+    (up_slot(py, ky), up_slot(px, kx)) from +0, then rounded to bf16 (round to nearest even) -> bf16 [16][Cin][Cout]."""
+    t = w_hwio.to(torch.float32)
+    out = []
+    for ph in range(4):
+        py, px = ph >> 1, ph & 1
+        acc = [torch.zeros_like(t[0, 0]) for _ in range(4)]
+        for ky in range(3):
+            for kx in range(3):
+                s = up_slot(py, ky) * 2 + up_slot(px, kx)
+                acc[s] = acc[s] + t[ky, kx]
+        out += acc
+    return torch.stack(out).to(torch.bfloat16)
+
+
+# the packed weight: fl(sum of <= 4 f32 taps) rounded to bf16 is within PACK times the sum of the taps' |w|
+# of the exact tap sum (u_bf16 on the sum, gamma(3) on the f32 additions)
+PACK = U_BF16 + gamma(3) * (1 + U_BF16)
+
+
+def upconv_fwd_ref(x, w_hwio, bias=None, chunk: int = 16):
+    """fdx_upconv3x3_fwd = conv3x3(nearest 2x(x)) + bias with the f32 master weights; each parity launch chains
+    4 taps x Cin products of the packed bf16 weights (PACK on the weight operand)."""
+    up = upsample2x_ref(x.to(torch.float64))
+    val, mag = conv3x3_fwd_ref(up, w_hwio, 1, chunk=chunk)[0], conv3x3_fwd_ref(up.abs(), w_hwio.abs(), chunk=chunk)[0]
+    val, mag = _plus(val, mag, bias)
+    return val, ((4 * x.shape[-1] + EPI) * TC_ADD * (1 + PACK) + PACK) * mag
+
+
+def upconv_dgrad_ref(dy, w_hwio, prior=None, chunk: int = 16):
+    """fdx_upconv3x3_dgrad: the adjoint of upconv_fwd_ref onto the low-resolution x (one launch of 16 taps,
+    K = 16 Cout), plus the bf16 prior of accumulate=True."""
+    val = upsample2x_bwd_ref(conv3x3_dgrad_ref(dy, w_hwio, chunk=chunk)[0])
+    mag = upsample2x_bwd_ref(conv3x3_dgrad_ref(dy.abs(), w_hwio.abs(), chunk=chunk)[0])
+    val, mag = _plus(val, mag, prior)
+    return val, ((16 * dy.shape[-1] + EPI) * TC_ADD * (1 + PACK) + PACK) * mag
+
+
+def upconv_wgrad_depth(N: int, h: int, w: int, Cin: int, Cout: int, sms: int) -> int:
+    """fdx_upconv3x3_wgrad: a TC_MNMN launch of 16 taps over the low-resolution pixels (B a stride-2 view), then
+    upconv_fold_kernel adds the 4 parity slabs of each tap from 0 and adds that onto the prior."""
+    return mnmn_depth(w, h, N, Cin, Cout, 16, sms, b_view=True) + 4
+
+
+def upconv_wgrad_ref(x, dy, depth: int, prior=None, chunk: int = 16):
+    """d/dw of upconv_fwd_ref (f32 HWIO) = prior + the 3x3 weight gradient of the upsampled x."""
+    return conv3x3_wgrad_ref(upsample2x_ref(x.to(torch.float64)), dy, depth, prior=prior, chunk=chunk)
+
+
+# 3-channel first and last convolutions (ops.conv_in_* / conv_out_*): im2col3 + one tensor-core GEMM (+ col2im3)
+def im2col3_ref(src, sgn: int, ones_col: bool):
+    """fdx_im2col3x3_c3: col[p][3 t + k] = src[p + sgn d(t)][k] (0 outside the image) as bf16 (round to nearest
+    even from the f32 / bf16 source), column 27 = 1 with ones_col, columns 28..31 = 0 -> (N H W, 32) bf16."""
+    N, H, W, _ = src.shape
+    sp = Fnn.pad(src.to(torch.float32), (0, 0, 1, 1, 1, 1))
+    cols = []
+    for ky in range(3):
+        for kx in range(3):
+            oy, ox = 1 + sgn * (ky - 1), 1 + sgn * (kx - 1)
+            cols.append(sp[:, oy:oy + H, ox:ox + W])
+    extra = torch.zeros(N, H, W, 5, dtype=torch.float32, device=src.device)
+    if ones_col:
+        extra[..., 0] = 1
+    return torch.cat(cols + [extra], -1).reshape(N * H * W, 32).to(torch.bfloat16)
+
+
+def col2im3_ref(col, bias, N: int, H: int, W: int):
+    """fdx_col2im3x3_c3 restated in f32: y[p][k] = bias[k], then + col[p + d(t)][3 t + k] for the taps inside the
+    image in (ky, kx) order -> (N, H, W, 3) f32."""
+    c = Fnn.pad(col.to(torch.float32).reshape(N, H, W, 32), (0, 0, 1, 1, 1, 1))
+    inside = Fnn.pad(torch.ones(N, H, W, 1, dtype=torch.bool, device=col.device), (0, 0, 1, 1, 1, 1))
+    y = bias.to(torch.float32).reshape(1, 1, 1, 3).expand(N, H, W, 3).clone()
+    for ky in range(3):
+        for kx in range(3):
+            t = ky * 3 + kx
+            ok = inside[:, ky:ky + H, kx:kx + W]
+            y = torch.where(ok, y + c[:, ky:ky + H, kx:kx + W, 3 * t:3 * t + 3], y)
+    return y
+
+
+def conv_in_fwd_ref(x, w_hwio, bias, chunk: int = 64):
+    """ops.conv_in_fwd: bf16 im2col of x (exact) times bf16(w) (U_BF16 on the weights), K = 27, with the bias."""
+    val, d = conv3x3_fwd_ref(x, w_hwio, 1, bias=bias, chunk=chunk)
+    mag = d / ((9 * x.shape[-1] + EPI) * TC_ADD)
+    return val, ((27 + EPI) * TC_ADD * (1 + U_BF16) + U_BF16) * mag
+
+
+def conv_in_wgrad_ref(x, dy, depth: int, dw_prior=None, db_prior=None, chunk: int = 16):
+    """ops.conv_in_wgrad: im2col(x)^T dY (with the ones column for the bias) by a GEMM_MNMN reduce over the pixels
+    into a zeroed f32 (32, Cout), then added onto the priors: depth = mnmn_depth + 1."""
+    dw = conv3x3_wgrad_ref(x, dy, depth, prior=dw_prior, chunk=chunk)
+    s = dy.to(torch.float64).sum((0, 1, 2))
+    db = _plus(s, dy.to(torch.float64).abs().sum((0, 1, 2)), db_prior)
+    return dw, (db[0], depth * TC_ADD * db[1])
+
+
+def conv_out_fwd_ref(x, w_hwio, bias, chunk: int = 64):
+    """ops.conv_out_fwd: GEMM (pixels x Cin)(Cin x 27) of bf16(w) into f32 columns (K = Cin), then col2im3 adds
+    the bias and the nine taps' columns in f32 (10 more levels)."""
+    val, d = conv3x3_fwd_ref(x, w_hwio, 1, bias=bias, chunk=chunk)
+    mag = d / ((9 * x.shape[-1] + EPI) * TC_ADD)
+    return val, ((x.shape[-1] + EPI + 10) * TC_ADD * (1 + U_BF16) + U_BF16) * mag
+
+
+def conv_out_dgrad_ref(dF, w_hwio, chunk: int = 64):
+    """ops.conv_out_dgrad: im2col of dF rounded to bf16 (U_BF16 on dF) times bf16(w) (U_BF16 on w), K = 27."""
+    val, d = conv3x3_dgrad_ref(dF, w_hwio, 1, chunk=chunk)
+    mag = d / ((27 + EPI) * TC_ADD)
+    rho = 2 * U_BF16 + U_BF16 ** 2
+    return val, ((27 + EPI) * TC_ADD * (1 + rho) + rho) * mag
+
+
+def conv_out_wgrad_ref(x, dF, depth: int, dw_prior=None, db_prior=None, chunk: int = 16):
+    """ops.conv_out_wgrad: x^T im2col(dF) (dF rounded to bf16: U_BF16) by a GEMM_MNMN reduce into a zeroed f32
+    (Cin, 32), then added onto the prior (depth = mnmn_depth + 1); the bias gradient is fdx_colsum over the
+    bf16 centre-tap columns (depth: the number of pixels, which bounds any order) plus the prior."""
+    val, d = conv3x3_wgrad_ref(x, dF, depth, prior=dw_prior, chunk=chunk)
+    mag = d / (depth * TC_ADD)
+    dw = (val, (depth * TC_ADD * (1 + U_BF16) + U_BF16) * mag)
+    f = dF.to(torch.float64)
+    P = f.numel() // f.shape[-1]
+    s, m = _plus(f.sum((0, 1, 2)), f.abs().sum((0, 1, 2)), db_prior)
+    return dw, (s, (gamma(P + 1) * (1 + U_BF16) + U_BF16) * m)
+
+
+def exact_case_ok(mag) -> bool:
+    """Precondition of the exact integer cases: with integer operands and every output's sum of |terms| below
+    2^24, every partial sum is an integer of at most 24 bits, so any f32 summation order, truncating or
+    rounding, is exact."""
+    return bool((mag < 2.0 ** 24).all())
+
+
+def assert_guard_intact(buf, lo: int, C: int, sentinel: float):
+    """The channels of an NHWC buffer outside the slot [lo, lo + C) still hold `sentinel`, bit for bit."""
+    side = torch.cat([buf[..., :lo], buf[..., lo + C:]], -1)
+    ref = torch.full_like(side, sentinel)
+    bits = torch.int16 if side.element_size() == 2 else torch.int32
+    assert torch.equal(side.view(bits), ref.view(bits)), "a kernel wrote outside its channel slot"
 
 
 def conv_gn_backward_ref(x, dy, w_hwio, gamma_, beta_, G, eps):

@@ -631,3 +631,212 @@ def test_training_comparator_rejects_what_relative_l2_accepts():
     assert rel(four, ref) < 1e-2
     with pytest.raises(AssertionError, match="outside the bound"):
         R.assert_elementwise(four, ref, 2 * R.ulp_f32(ref))
+
+
+# ----------------------------------------------------------------------------------------------- convolutions
+def _flax_same(x, w, stride):
+    """conv2d with flax SAME written from its definition: total padding max((out - 1) s + 3 - size, 0), the
+    smaller half first."""
+    pads = []
+    for size in (x.shape[2], x.shape[1]):
+        out = -(-size // stride)
+        tot = max((out - 1) * stride + 3 - size, 0)
+        pads += [tot // 2, tot - tot // 2]
+    return Fnn.conv2d(Fnn.pad(x.permute(0, 3, 1, 2), pads), w.permute(3, 2, 0, 1), stride=stride).permute(0, 2, 3, 1)
+
+
+def _ints(shape, g, lo=-2, hi=2):
+    return torch.randint(lo, hi + 1, shape, generator=g).double()
+
+
+@pytest.mark.parametrize("stride,H,W", [(1, 5, 7), (1, 8, 8), (2, 8, 12), (2, 7, 9)])
+def test_conv_references_match_autograd(stride, H, W):
+    g = torch.Generator().manual_seed(7)
+    x = _bf(torch.randn(2, H, W, 16, generator=g, dtype=torch.float64))
+    w = _bf(torch.randn(3, 3, 16, 24, generator=g, dtype=torch.float64) / 12)
+    xr, wr = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
+    y = _flax_same(xr, wr, stride)
+    _close(R.conv3x3_fwd_ref(x, w, stride)[0], y)
+    dy = _bf(torch.randn(tuple(y.shape), generator=g, dtype=torch.float64))
+    y.backward(dy)
+    _close(R.conv3x3_wgrad_ref(x, dy, 100, stride)[0], wr.grad)
+    prior = torch.randn(3, 3, 16, 24, generator=g, dtype=torch.float64)
+    _close(R.conv3x3_wgrad_ref(x, dy, 100, stride, prior=prior)[0], wr.grad + prior)
+    if stride == 1 or (H % 2 == 0 and W % 2 == 0):       # the stride-2 data gradient needs even sizes
+        _close(R.conv3x3_dgrad_ref(dy, w, stride)[0], xr.grad)
+    # every delta is depth TC_ADD times the same operation on |inputs|
+    _, d = R.conv3x3_fwd_ref(x, w, stride)
+    _close(d, (9 * 16 + R.EPI) * R.TC_ADD * _flax_same(x.abs(), w.abs(), stride))
+
+
+def test_gemm_upconv_and_3channel_references_match_autograd():
+    g = torch.Generator().manual_seed(8)
+    a, b = torch.randn(3, 5, 7, generator=g, dtype=torch.float64), torch.randn(3, 7, 4, generator=g, dtype=torch.float64)
+    bias, res = torch.randn(4, generator=g, dtype=torch.float64), torch.randn(3, 5, 4, generator=g, dtype=torch.float64)
+    v, d = R.gemm_ref(a, b, 7 + R.EPI, alpha=0.5, bias=bias, res=res)
+    _close(v, 0.5 * torch.bmm(a, b) + bias + res)
+    _close(d, (7 + R.EPI) * R.TC_ADD * (0.5 * torch.bmm(a.abs(), b.abs()) + bias.abs() + res.abs()))
+    # nearest 2x + conv3x3 and its gradients
+    x = _bf(torch.randn(2, 4, 6, 8, generator=g, dtype=torch.float64))
+    w = torch.randn(3, 3, 8, 16, generator=g, dtype=torch.float64).float().double()
+    xr, wr = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
+    up = Fnn.interpolate(xr.permute(0, 3, 1, 2), scale_factor=2, mode="nearest").permute(0, 2, 3, 1)
+    y = _flax_same(up, wr, 1) + bias.repeat(4)
+    _close(R.upconv_fwd_ref(x, w, bias.repeat(4))[0], y)
+    dy = _bf(torch.randn(tuple(y.shape), generator=g, dtype=torch.float64))
+    y.backward(dy)
+    _close(R.upconv_dgrad_ref(dy, w)[0], xr.grad)
+    _close(R.upconv_wgrad_ref(x, dy, 100)[0], wr.grad)
+    # the pack: bf16 of the f32 sums, within one rounding of the exact sums; an integer kernel packs exactly
+    weff = R.upconv_pack_ref(w).double()
+    ex, ex_abs = torch.zeros_like(weff), torch.zeros_like(weff)
+    for ph in range(4):
+        for ky in range(3):
+            for kx in range(3):
+                ex[ph * 4 + R.up_slot(ph >> 1, ky) * 2 + R.up_slot(ph & 1, kx)] += w[ky, kx]
+                ex_abs[ph * 4 + R.up_slot(ph >> 1, ky) * 2 + R.up_slot(ph & 1, kx)] += w[ky, kx].abs()
+    assert ((weff - ex).abs() <= R.PACK * ex_abs).all()
+    wi = _ints((3, 3, 8, 16), g)
+    assert torch.equal(R.upconv_pack_ref(wi).double(), torch.stack([
+        sum(wi[ky, kx] for ky in range(3) for kx in range(3)
+            if R.up_slot(ph >> 1, ky) * 2 + R.up_slot(ph & 1, kx) == s) for ph in range(4) for s in range(4)]))
+    # 3-channel convolutions: im2col3 / GEMM / col2im3 restate the convolution
+    x3 = _bf(torch.randn(2, 5, 6, 3, generator=g, dtype=torch.float64))
+    w3 = torch.randn(3, 3, 3, 8, generator=g, dtype=torch.float64)
+    col = R.im2col3_ref(x3, +1, True).double()
+    assert torch.equal(col[:, 27], torch.ones(60, dtype=torch.float64)) and not col[:, 28:].any()
+    _close((col[:, :27] @ w3.reshape(27, 8)).reshape(2, 5, 6, 8), R.conv_in_fwd_ref(x3, w3, None)[0])
+    xo = _bf(torch.randn(2, 5, 6, 8, generator=g, dtype=torch.float64))
+    wo = torch.randn(3, 3, 8, 3, generator=g, dtype=torch.float64)
+    bo = torch.randn(3, generator=g, dtype=torch.float64)
+    colo = xo.reshape(-1, 8) @ Fnn.pad(wo.reshape(9, 8, 3).permute(1, 0, 2).reshape(8, 27), (0, 5))
+    yo = R.col2im3_ref(colo.float(), bo.float(), 2, 5, 6).double()
+    _close(yo, R.conv_out_fwd_ref(xo, wo, bo)[0], 1e-6)
+    xor, wor, bor = (t.clone().requires_grad_(True) for t in (xo, wo, bo))
+    (_flax_same(xor, wor, 1) + bor).backward(_bf(dF := torch.randn(2, 5, 6, 3, generator=g, dtype=torch.float64)))
+    dFb = _bf(dF)
+    _close(R.conv_out_dgrad_ref(dFb, wo)[0], xor.grad)
+    (dw, _), (db, _) = R.conv_out_wgrad_ref(xo, dFb, 100)
+    _close(dw, wor.grad)
+    _close(db, bor.grad)
+    # conv_out's data gradient is im2col3(dF, -1) times the re-arranged kernel
+    colf = R.im2col3_ref(dFb, -1, False).double()[:, :27]
+    _close((colf @ wo.reshape(9, 8, 3).permute(0, 2, 1).reshape(27, 8)).reshape(2, 5, 6, 8), xor.grad)
+
+
+@pytest.mark.parametrize("sms", [132, 114])
+def test_split_counts_follow_the_sm_count(sms):
+    # C2's 64 x 64 weight gradient: one (ci, co) block, 16384 pixel blocks: one split per SM
+    assert R.wgrad9_depth(256, 64, 64, 64, 64, sms) == 64 * math.ceil(16384 / sms) + sms + 1
+    # 1024 channels: 256 blocks, two waves on 132 SMs at one split, so no split-K
+    assert R.split_count(sms, 256, 4) == 1
+    assert R.tc_bn(64) == 64 and R.tc_bn(128) == 128 and R.tc_bn(256) == 256 and R.tc_bn(320) == 128
+
+
+def _trunc32(v):
+    """v (float64) rounded to f32 toward zero."""
+    f = v.float()
+    over = f.double().abs() > v.abs()
+    return torch.where(over, torch.nextafter(f, torch.zeros_like(f)), f)
+
+
+def test_conv_emulation_within_bound():
+    """The weight gradient as wgrad9 computes it, in f32: per split a truncating chain over its 64-pixel blocks,
+    then the splits added onto the prior in a random order; and a truncating 9 Cin forward chain rounded to
+    bf16.  Both stay inside the bound; the exact integer case is exact."""
+    g = torch.Generator().manual_seed(9)
+    sms = 12
+    N, H, W, Ci, Co = 3, 16, 16, 8, 8
+    for kind in ("dense", "exact"):
+        if kind == "dense":
+            x = _bf(torch.randn(N, H, W, Ci, generator=g, dtype=torch.float64))
+            dy = _bf(torch.randn(N, H, W, Co, generator=g, dtype=torch.float64))
+            prior = torch.randn(3, 3, Ci, Co, generator=g, dtype=torch.float64).float().double()
+        else:
+            x, dy, prior = _ints((N, H, W, Ci), g), _ints((N, H, W, Co), g), _ints((3, 3, Ci, Co), g)
+        depth = R.wgrad9_depth(N, H, W, Ci, Co, sms)
+        val, delta = R.conv3x3_wgrad_ref(x, dy, depth, prior=prior)
+        TW, TH = 16, 4
+        nxb, nyb = W // TW, H // TH
+        kb = nxb * nyb * N
+        splits = R.split_count(sms, 1, kb)
+        xp = Fnn.pad(x, (0, 0, 1, 1, 1, 1))
+        parts = []
+        for s in range(splits):
+            acc = torch.zeros(3, 3, Ci, Co, dtype=torch.float32)
+            for pb in range(kb * s // splits, kb * (s + 1) // splits):
+                xb, yb, nb = pb % nxb, (pb // nxb) % nyb, pb // (nxb * nyb)
+                for py in range(yb * TH, yb * TH + TH):
+                    for px in range(xb * TW, xb * TW + TW):
+                        t = xp[nb, py:py + 3, px:px + 3, :, None] * dy[nb, py, px]
+                        acc = _trunc32(acc.double() + t)
+            parts.append(acc)
+        out = prior.float()
+        for s in torch.randperm(splits, generator=g).tolist():
+            out = out + parts[s]
+        if kind == "exact":
+            assert R.exact_case_ok(R.conv3x3_wgrad_ref(x.abs(), dy.abs(), depth, prior=prior.abs())[0])
+            assert torch.equal(out.double(), val)
+        R.assert_elementwise(out, val, R.f32_bound(val, delta), "emulated wgrad9 " + kind)
+    # forward: 9 Cin terms in one truncating chain, then bf16
+    w = _bf(torch.randn(3, 3, Ci, Co, generator=g, dtype=torch.float64) / 8)
+    val, delta = R.conv3x3_fwd_ref(x, w)
+    xp = Fnn.pad(x, (0, 0, 1, 1, 1, 1))
+    acc = torch.zeros(N, H, W, Co, dtype=torch.float32)
+    for ky in range(3):
+        for kx in range(3):
+            for ci in range(Ci):
+                acc = _trunc32(acc.double() + xp[:, ky:ky + H, kx:kx + W, ci, None] * w[ky, kx, ci])
+    R.assert_elementwise(acc.bfloat16(), val, R.bf16_bound(val, delta), "emulated forward")
+
+
+def test_conv_comparator_rejects_what_relative_l2_accepts():
+    """Four faults of the convolution engines, each inside the relative-L2 tolerances of the existing tests, each
+    caught: a dropped pixel block (rel < 1e-4, the f32 tolerance) and a skipped split (rel < 5e-3, the tolerance of
+    the full-size checks) by the exact integer case at C2's full weight-gradient reduction (256 images of
+    64 x 64), a missing border tap by the element-wise bound, a write into the neighbouring channel slot by the
+    sentinels."""
+    g = torch.Generator().manual_seed(10)
+    sms = 132
+    N, H, W, C = 256, 64, 64, 8
+    # non-negative integers: the sums grow with the pixel count, so that one block is 64 / 2^20 of them
+    x, dy = _ints((N, H, W, C), g, 0, 2), _ints((N, H, W, C), g, 0, 2)
+    depth = R.wgrad9_depth(N, H, W, C, C, sms)
+    exact, _ = R.conv3x3_wgrad_ref(x, dy, depth, chunk=64)
+    assert R.exact_case_ok(exact)
+    pb = ((torch.arange(N)[:, None, None] * (H // 4) + torch.arange(H)[None, :, None] // 4) * (W // 16)
+          + torch.arange(W)[None, None, :] // 16)                     # wgrad9's pixel block of every pixel
+    kb = N * (H // 4) * (W // 16)
+    splits = R.split_count(sms, 1, kb)
+
+    def without(mask):
+        return exact - R.conv3x3_wgrad_ref(x, dy * mask[..., None], depth, chunk=64)[0]
+
+    dropped = without(pb == 1000)
+    assert rel(dropped, exact) < 1e-4
+    # a skipped split (1/132 of the pixels), in a gradient accumulated onto an earlier micro-batch's
+    prior = exact.flip(2)
+    s0, s1 = kb * 7 // splits, kb * 8 // splits
+    skipped = without((pb >= s0) & (pb < s1)) + prior
+    assert R.exact_case_ok(exact + prior) and rel(skipped, exact + prior) < 5e-3
+    for got, ref in ((dropped, exact), (skipped, exact + prior)):
+        assert not torch.equal(got, ref)                             # the exact integer case sees both
+    # one border tap missing at one pixel of a bf16 forward
+    xd = _bf(torch.randn(4, 16, 16, 64, generator=g, dtype=torch.float64))
+    wd = _bf(torch.randn(3, 3, 64, 64, generator=g, dtype=torch.float64) / 24)
+    val, delta = R.conv3x3_fwd_ref(xd, wd)
+    bad = val.clone()
+    bad[2, 15, 0, 5] -= (xd[2, 14, 0] * wd[0, 1, :, 5]).sum()        # tap (ky, kx) = (0, 1) of the bottom-left pixel
+    got = _bf(bad)
+    assert rel(got, val) < 5e-3
+    with pytest.raises(AssertionError, match="outside the bound"):
+        R.assert_elementwise(got, val, R.bf16_bound(val, delta))
+    R.assert_elementwise(_bf(val), val, R.bf16_bound(val, delta))
+    # a write into the neighbouring slot: the slot itself is right
+    buf = torch.full((2, 4, 4, 8 + 64 + 16), -1234.0, dtype=torch.bfloat16)
+    buf[..., 8:72] = _bf(val[:2, :4, :4]).bfloat16()
+    R.assert_guard_intact(buf, 8, 64, -1234.0)
+    buf[1, 3, 3, 72] = buf[1, 3, 3, 71]
+    assert rel(buf[..., 8:72], val[:2, :4, :4]) < 5e-3
+    with pytest.raises(AssertionError, match="outside its channel slot"):
+        R.assert_guard_intact(buf, 8, 64, -1234.0)
