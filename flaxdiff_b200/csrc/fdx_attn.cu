@@ -2,8 +2,8 @@
 // NormalAttention (flaxdiff/models/attention.py:156-177, softmax(q k^T / sqrt(d)) v, self- and cross-attention
 // to the 77 x 768 text context) and its backward (jax.value_and_grad, trainer/general_diffusion_trainer.py:321).
 //
-// The round-1 path ran QK^T, softmax, PV as separate launches with the f32 logits S and the bf16 probabilities
-// P round-tripping HBM ((B, h, L, Lk): 2.1 GB + 1 GB per block at 256x256).  Here S and P never leave the SM:
+// As separate QK^T, softmax and PV launches, the f32 logits S and the bf16 probabilities P would round-trip HBM
+// ((B, h, L, Lk): 2.1 GB + 1 GB per block at 256x256).  Here S and P never leave the SM:
 //
 //   forward  (one CTA per 128 queries x head x image; flash-style loop over 128-key blocks)
 //     warp 4      TMA: Q tile once, K_j / V_j tiles through an mbarrier ring (128B-swizzled boxes of
@@ -27,7 +27,6 @@
 #include "../../include/fdx.h"
 #include <math.h>
 #include <type_traits>
-#include <stdlib.h>
 
 namespace {
 
@@ -898,7 +897,7 @@ int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
   d.scale = a->scale; d.scale_log2 = a->scale * kLog2e;
   d.o = (__nv_bfloat16*)a->o; d.o_ld = a->o_ld; d.o_bs = a->o_bs;
   d.lse = a->lse;
-  const bool short_keys = a->Lk <= 128 && !getenv("FDX_ATTN_NO_SHORT");
+  const bool short_keys = a->Lk <= 128;
   if (a->dh == 128) {
     const int smem128 = (2 + 2 * (short_keys ? 1 : 2)) * kWTile + 1024 + 64;
     dim3 grid128((a->L + 127) / 128, a->heads, a->B);

@@ -17,7 +17,6 @@
 //               atomics for the split-K weight gradient).
 #include "fdx_tc.cuh"
 #include "fdx_epilogue.cuh"
-#include <stdlib.h>
 
 namespace {
 
@@ -443,7 +442,7 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
 
   // Few output columns (Ncols = 64 / 128): the transposed formulation (fdx_tct.cu) issues M x 256 x 16 MMAs
   // instead of 128 x Ncols x 16 ones; faster on every such layer (profiles/layers_r01_tct.txt).
-  if (L.mode != TC_MNMN && !getenv("FDX_NO_TCT")) {
+  if (L.mode != TC_MNMN) {
     const int rt = fdx_tct_launch(L, stream);
     if (rt != FDX_ERR_UNSUPPORTED) return rt;
   }

@@ -22,7 +22,6 @@
 // Geometry: stride 1, W and H multiples of 16; output and side input 16-byte aligned with 16-byte strides (TMA).
 #include "fdx_tc.cuh"
 #include "fdx_epilogue.cuh"
-#include <stdlib.h>
 
 namespace {
 
@@ -85,7 +84,7 @@ __device__ __forceinline__ TileCoord tile_coord(const TctDev& p, int tile) {
 // 16 x 18 pixels (rows y0-1 .. y0+16) is loaded per (kx, K chunk); the three ky taps are 2048-byte row offsets
 // into it (swizzle-aligned views, exactly as in the nine-tap weight gradient), so a stage carries three weight
 // tiles + 36 KB of pixels and feeds twelve MMAs: 96 -> 36 KB of pixel traffic per three taps.
-// GNB = true (data gradient only): the first pass of the GroupNorm(+SiLU) backward in the epilogue - with x = the
+// GNB = true (HALO data gradient only): the first pass of the GroupNorm(+SiLU) backward in the epilogue - with x = the
 // GroupNorm input (side input `res`) and z = a_c x + b_c the kernel stores dz = dy * silu'(z) instead of dy and
 // accumulates S0 = sum dz, S1 = sum dz * x per (image, channel) into the column-sum workspace, exactly as the
 // pixels-as-M engine's EPI_GN_BWD (fdx_epilogue.cuh).
@@ -442,8 +441,11 @@ int make_chunk_map(CUtensorMap* map, const void* base, const TcLaunch& L, long l
 int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
   if (L.mode == TC_MNMN || L.gemm_like || L.es != 1 || L.out_f32 || L.out_atomic || L.b_batched)
     return FDX_ERR_UNSUPPORTED;
-  // fused GroupNorm-backward first pass: data gradient with x as the side input and the sums workspace
-  if (L.gn_ab && (L.mode != TC_KK || !L.res || !L.gn_ws || L.bias || L.rowvec)) return FDX_ERR_UNSUPPORTED;
+  // halo-sharing variant: standard 3x3 stride-1 tap set in (ky, kx) order
+  bool halo = L.ntaps == 9;
+  for (int t = 0; t < 9 && halo; ++t) halo = (L.tap_dx[t] == t % 3 - 1) && (L.tap_dy[t] == t / 3 - 1);
+  // fused GroupNorm-backward first pass: halo data gradient with x as the side input and the sums workspace
+  if (L.gn_ab && (!halo || L.mode != TC_KK || !L.res || !L.gn_ws || L.bias || L.rowvec)) return FDX_ERR_UNSUPPORTED;
   // column counts the generic engine would have to cover with N < 256 tiles (64, 128, 192, 320, 384, ...)
   if (L.Ncols % 64 != 0 || L.Ncols % 256 == 0 || L.Ncols > 512) return FDX_ERR_UNSUPPORTED;
   if (L.W % 16 != 0 || L.H % 16 != 0 || L.K % 64 != 0) return FDX_ERR_UNSUPPORTED;
@@ -463,13 +465,6 @@ int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
   d.cs_ws = L.gn_ws; d.cs_slots = L.gn_slots > 0 ? L.gn_slots : 1; d.cs_ld = L.ws_ld > 0 ? L.ws_ld : L.Ncols;
   d.gn_ab = L.gn_ab;
 
-  // halo-sharing variant: standard 3x3 stride-1 tap set in (ky, kx) order.  FDX_TCT_HALO=0 disables it, and so
-  // does any other value but 64 (the tile's channel count).
-  bool halo = L.ntaps == 9;
-  for (int t = 0; t < 9 && halo; ++t) halo = (L.tap_dx[t] == t % 3 - 1) && (L.tap_dy[t] == t / 3 - 1);
-  const char* he = getenv("FDX_TCT_HALO");          // read per launch: the A/B tests toggle it in-process
-  const int halo_env = (he && *he) ? atoi(he) : -1;
-  if (halo_env >= 0 && halo_env != 64) halo = false;
   TctMaps m{};
   {
     uint64_t dims[4], str[3];
@@ -493,7 +488,6 @@ int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
   if (s != FDX_OK) return s;
   if (L.res && (s = make_chunk_map(&m.r, L.res, L, L.rs_x, L.rs_y, L.rs_n)) != FDX_OK) return s;
   if (L.mode == TC_KMN) return halo ? launch_tct<true, true>(m, d, stream) : launch_tct<true, false>(m, d, stream);
-  if (L.gn_ab)   // fused GroupNorm backward
-    return halo ? launch_tct<false, true, true>(m, d, stream) : launch_tct<false, false, true>(m, d, stream);
+  if (L.gn_ab) return launch_tct<false, true, true>(m, d, stream);   // fused GroupNorm backward
   return halo ? launch_tct<false, true>(m, d, stream) : launch_tct<false, false>(m, d, stream);
 }

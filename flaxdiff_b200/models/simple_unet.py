@@ -44,12 +44,9 @@ ATTN_EPS = 1e-4     # TransformerBlock.norm_epsilon, models/attention.py:319
 
 
 def _attn_width(d: int) -> int:
-    """Stored head width for the fused attention kernels: 32, 64 or 128 (narrower heads are zero-padded).
-    FDX_ATTN_PAD64=1 stores every head of up to 64 channels 64 wide (one head per 128-byte swizzle row)."""
+    """Stored head width for the fused attention kernels: 32, 64 or 128 (narrower heads are zero-padded)."""
     if d > 64:
         return 128
-    if os.environ.get("FDX_ATTN_PAD64"):
-        return 64
     return 32 if d <= 32 else 64
 
 
@@ -549,10 +546,7 @@ class Unet:
         77 x 768) or from xn itself.  q / k / v / out projections are tensor-core GEMMs; the attention core is ONE
         fused kernel (fdx_attention_fwd: logits and probabilities stay in registers / shared memory).  Heads
         narrower than 32 are zero-padded to 32, and heads of 65 - 127 channels to 128 (the kernel stores heads
-        32, 64 or 128 wide).
-        FDX_ATTN_UNFUSED=1 selects the round-1 path (separate QK^T / softmax / PV launches)."""
-        if os.environ.get("FDX_ATTN_UNFUSED"):
-            return self._attn_fwd_unfused(name, xin, dst, heads, W, W16, ctx16)
+        32, 64 or 128 wide)."""
         x = xin.t
         Bn, hh, ww, C = x.shape
         L = hh * ww
@@ -582,50 +576,6 @@ class Unet:
         out2 = dst.t
         ops.gemm(GEMM_KMN, o, wo, out2, Bn * L, C, HD, HD, C, out2.stride(2), res=xn, r_ld=C)
         return ("attn", name, xin, dst, heads, xn, q, k, v, lse, o, ctx if ctx16 is not None else None,
-                (wq, wk, wv, wo), Lk)
-
-    def _attn_fwd_unfused(self, name, xin: Node, dst: Node, heads, W, W16, ctx16=None):
-        """Round-1 attention path (FDX_ATTN_UNFUSED=1): xn = RMSNorm(x);
-        out = xn + to_out(softmax(q k^T / sqrt(d)) v); keys/values come from `textcontext`
-        (cross-attention, e.g. 77 x 768) or from xn itself (self-attention).  Heads narrower than 32
-        and key counts that are not multiples of 32 are zero-padded for the tensor-core tiles."""
-        x = xin.t
-        Bn, hh, ww, C = x.shape
-        L = hh * ww
-        d = C // heads
-        dp = max(32, d)
-        HD = heads * dp
-        base = f"{name}/Attention/Attention2"
-        dev = x.device
-        xn = ops.rmsnorm_fwd(x, W[f"{name}/RMSNorm_0/scale"], ATTN_EPS)
-        x2 = xn.view(Bn * L, C)
-        if ctx16 is None:
-            ctx, Lk, Cc = xn.view(Bn, L, C), L, C
-        else:
-            ctx, Lk, Cc = ctx16, ctx16.shape[1], ctx16.shape[2]
-        Lkp = (Lk + 31) // 32 * 32
-        wq = self._pad_heads(W16[f"{base}/to_q/kernel"], 2, d, dp).reshape(C, HD)
-        wk = self._pad_heads(W16[f"{base}/to_k/kernel"], 2, d, dp).reshape(Cc, HD)
-        wv = self._pad_heads(W16[f"{base}/to_v/kernel"], 2, d, dp).reshape(Cc, HD)
-        wo = self._pad_heads(W16[f"{base}/to_out_0/kernel"], 1, d, dp).reshape(HD, C)
-        q = ops.linear_fwd(x2, wq)                                        # [B*L, h*dp]
-        alloc = torch.zeros if Lkp != Lk else torch.empty
-        k = alloc((Bn, Lkp, HD), dtype=BF16, device=dev)
-        v = alloc((Bn, Lkp, HD), dtype=BF16, device=dev)
-        for w_, o_ in ((wk, k), (wv, v)):
-            ops.gemm(GEMM_KMN, ctx, w_, o_, Lk, HD, Cc, Cc, HD, HD, batch2=Bn,
-                     a_s=(0, Lk * Cc), d_s=(0, Lkp * HD))
-        S = torch.empty((Bn, heads, L, Lkp), dtype=F32, device=dev)
-        ops.gemm(GEMM_KK, q, k, S, L, Lkp, dp, HD, HD, Lkp, batch1=heads, batch2=Bn,
-                 a_s=(dp, L * HD), b_s=(dp, Lkp * HD), d_s=(L * Lkp, heads * L * Lkp), alpha=d ** -0.5)
-        P = ops.softmax_fwd(S, valid=Lk)
-        del S
-        o = torch.empty((Bn * L, HD), dtype=BF16, device=dev)
-        ops.gemm(GEMM_KMN, P, v, o, L, dp, Lkp, Lkp, HD, HD, batch1=heads, batch2=Bn,
-                 a_s=(L * Lkp, heads * L * Lkp), b_s=(dp, Lkp * HD), d_s=(dp, L * HD))
-        out2 = dst.t
-        ops.gemm(GEMM_KMN, o, wo, out2, Bn * L, C, HD, HD, C, out2.stride(2), res=xn, r_ld=C)
-        return ("attn_unfused", name, xin, dst, heads, xn, q, k, v, P, o, ctx if ctx16 is not None else None,
                 (wq, wk, wv, wo), Lk)
 
 
@@ -915,8 +865,6 @@ class Unet:
                     mark_children_written(xin, children[id(xin)])
             elif kind == "attn":
                 self._attn_bwd(rec, W, W16, Gd, want, grad_of)
-            elif kind == "attn_unfused":
-                self._attn_bwd_unfused(rec, W, W16, Gd, want, grad_of)
             elif kind == "tblock":
                 self._tblock_bwd(rec, W, W16, Gd, want, grad_of)
             elif kind == "conv":
@@ -1079,78 +1027,5 @@ class Unet:
         if not cross:
             for dy_, w_ in ((dk2, wk), (dv2, wv)):
                 ops.gemm(GEMM_KK, dy_, w_, dxn2, M, C, HD, HD, HD, C, res=dxn2, r_ld=C)
-        dx, acc = want(xin)
-        ops.rmsnorm_bwd(x, dxn, W[f"{name}/RMSNorm_0/scale"], ATTN_EPS, dx, Gd[f"{name}/RMSNorm_0/scale"], acc)
-
-    def _attn_bwd_unfused(self, rec, W, W16, Gd, want, grad_of):
-        _, name, xin, dst, heads, xn, q, k, v, P, o, ctx, (wq, wk, wv, wo), Lk = rec
-        x = xin.t
-        Bn, hh, ww, C = x.shape
-        L = hh * ww
-        d = C // heads
-        dp = max(32, d)
-        HD = heads * dp
-        Lkp = k.shape[1]
-        cross = ctx is not None
-        kv_src = ctx if cross else xn.view(Bn, L, C)
-        Cc = kv_src.shape[2]
-        base = f"{name}/Attention/Attention2"
-        dout = grad_of(dst)                      # [B,h,w,C] view
-        M = Bn * L
-        dev = x.device
-        alpha = d ** -0.5
-
-        def grad_target(pname, shape_p):
-            """(buffer to accumulate into, finisher): padded heads go through a scratch buffer."""
-            g = Gd[pname]
-            if dp == d:
-                return g.view(shape_p), None
-            return torch.zeros(shape_p, dtype=F32, device=dev), g
-
-        def finish(tmp, g, axis_view, sl):
-            if g is not None:
-                g.add_(tmp.view(axis_view)[sl])
-
-        # out = xn + o @ Wo
-        t_o, g_o = grad_target(f"{base}/to_out_0/kernel", (HD, C))
-        ops.gemm(GEMM_MNMN, o, dout, t_o, HD, C, M, HD, dout.stride(2), C, atomic=True, reduce_batch=True)
-        finish(t_o, g_o, (heads, dp, C), (slice(None), slice(0, d), slice(None)))
-        do = torch.empty((M, HD), dtype=BF16, device=dev)
-        ops.gemm(GEMM_KK, dout, wo, do, M, HD, C, dout.stride(2), C, HD)
-        # o = P v
-        dv = torch.empty((Bn, Lkp, HD), dtype=BF16, device=dev)
-        ops.gemm(GEMM_MNMN, P, do, dv, Lkp, dp, L, Lkp, HD, HD, batch1=heads, batch2=Bn,
-                 a_s=(L * Lkp, heads * L * Lkp), b_s=(dp, L * HD), d_s=(dp, Lkp * HD))
-        dP = torch.empty((Bn, heads, L, Lkp), dtype=F32, device=dev)
-        ops.gemm(GEMM_KK, do, v, dP, L, Lkp, dp, HD, HD, Lkp, batch1=heads, batch2=Bn,
-                 a_s=(dp, L * HD), b_s=(dp, Lkp * HD), d_s=(L * Lkp, heads * L * Lkp))
-        dS = ops.softmax_bwd(P, dP, alpha, valid=Lk)
-        del dP
-        dq = torch.empty((M, HD), dtype=BF16, device=dev)
-        ops.gemm(GEMM_KMN, dS, k, dq, L, dp, Lkp, Lkp, HD, HD, batch1=heads, batch2=Bn,
-                 a_s=(L * Lkp, heads * L * Lkp), b_s=(dp, Lkp * HD), d_s=(dp, L * HD))
-        dk = torch.empty((Bn, Lkp, HD), dtype=BF16, device=dev)
-        ops.gemm(GEMM_MNMN, dS, q, dk, Lkp, dp, L, Lkp, HD, HD, batch1=heads, batch2=Bn,
-                 a_s=(L * Lkp, heads * L * Lkp), b_s=(dp, L * HD), d_s=(dp, Lkp * HD))
-        del dS
-        # projection weight gradients: y = src @ W  ->  dW = src^T dy (reduced over tokens and images)
-        x2 = xn.view(M, C)
-        t_q, g_q = grad_target(f"{base}/to_q/kernel", (C, HD))
-        ops.gemm(GEMM_MNMN, x2, dq, t_q, C, HD, M, C, HD, HD, atomic=True, reduce_batch=True)
-        finish(t_q, g_q, (C, heads, dp), (slice(None), slice(None), slice(0, d)))
-        for nm, dy_ in (("to_k", dk), ("to_v", dv)):
-            t_w, g_w = grad_target(f"{base}/{nm}/kernel", (Cc, HD))
-            ops.gemm(GEMM_MNMN, kv_src, dy_, t_w, Cc, HD, Lk, Cc, HD, HD, batch2=Bn,
-                     a_s=(0, Lk * Cc), b_s=(0, Lkp * HD), atomic=True, reduce_batch=True)
-            finish(t_w, g_w, (Cc, heads, dp), (slice(None), slice(None), slice(0, d)))
-        # d(xn) = dout (residual) + dq Wq^T (+ dk Wk^T + dv Wv^T for self-attention)
-        dxn = torch.empty((Bn, hh, ww, C), dtype=BF16, device=dev)
-        dxn2 = dxn.view(M, C)
-        ops.gemm(GEMM_KK, dq, wq, dxn2, M, C, HD, HD, HD, C, res=dout, r_ld=dout.stride(2))
-        if not cross:
-            for dy_, w_ in ((dk, wk), (dv, wv)):
-                # rows of the padded [B, Lkp, HD] buffers map to tokens batch by batch
-                ops.gemm(GEMM_KK, dy_, w_, dxn2, L, C, HD, HD, HD, C, batch2=Bn, a_s=(0, Lkp * HD),
-                         d_s=(0, L * C), res=dxn2, r_ld=C, r_s=(0, L * C))
         dx, acc = want(xin)
         ops.rmsnorm_bwd(x, dxn, W[f"{name}/RMSNorm_0/scale"], ATTN_EPS, dx, Gd[f"{name}/RMSNorm_0/scale"], acc)

@@ -511,48 +511,7 @@ class GeneralDiffusionTrainer:
     # ------------------------------------------------------------------ the step
     def _fwd_bwd(self, images, noise, noise_level, ctx=None):
         """noise-add -> UNet fwd -> loss -> UNet bwd [-> bucketed gradient exchange]; returns the loss tensor
-        (f32[1]); gradients land in self._grads.  FDX_MICROBATCH=2 processes the batch as two micro-batches
-        on two streams; measured slower than one batch with side-stream weight gradients, hence opt-in."""
-        B = images.shape[0]
-        nmb = int(os.environ.get("FDX_MICROBATCH", "1"))
-        if nmb < 2 or B % nmb != 0 or B // nmb < 2:
-            return self._fwd_bwd_one(images, noise, noise_level, ctx, self._grads, exchange=True)
-        if getattr(self, "_mb_grads", None) is None or len(self._mb_grads) != nmb:
-            self._mb_grads = [self.state.params.zeros_like() for _ in range(nmb)]
-            self._mb_streams = [torch.cuda.Stream() for _ in range(nmb)]
-        main = torch.cuda.current_stream()
-        ev = torch.cuda.Event()
-        ev.record(main)
-        losses = []
-        step = B // nmb
-        for h in range(nmb):
-            sl = slice(h * step, (h + 1) * step)
-            self._mb_streams[h].wait_event(ev)
-            with torch.cuda.stream(self._mb_streams[h]):
-                losses.append(self._fwd_bwd_one(images[sl], noise[sl], noise_level[sl],
-                                                None if ctx is None else ctx[sl], self._mb_grads[h]))
-        for h in range(nmb):
-            main.wait_stream(self._mb_streams[h])
-        g = self._grads.flat
-        if nmb == 2:
-            torch.lerp(self._mb_grads[0].flat, self._mb_grads[1].flat, 0.5, out=g)
-        else:
-            torch.add(self._mb_grads[0].flat, self._mb_grads[1].flat, out=g)
-            for h in range(2, nmb):
-                g.add_(self._mb_grads[h].flat)
-            g.mul_(1.0 / nmb)
-        loss = losses[0]
-        for h in range(1, nmb):
-            loss = loss + losses[h]
-        loss = loss / nmb
-        if self._overlap:
-            self._gbuf[-64:-63].copy_(loss)
-            self._exchange.begin()
-            self._exchange.finish([torch.cuda.current_stream()])
-            loss = self._gbuf[-64:-63]
-        return loss
-
-    def _fwd_bwd_one(self, images, noise, noise_level, ctx, grads, exchange=False):
+        (f32[1]); gradients land in self._grads."""
         sched, tr, st = self.noise_schedule, self.model_output_transform, self.state
         B = images.shape[0]
         rates = sched.get_rates(noise_level, shape=(-1,))
@@ -569,9 +528,9 @@ class GeneralDiffusionTrainer:
         if ds is not None:
             # DynamicScale.value_and_grad differentiates loss * scale (the optimiser divides it back out)
             dF, _, _ = ops.affine_combine([dF], ds.state[0:1].expand(1, B))
+        grads = self._grads
         grads.flat.zero_()
-        overlap = exchange and self._overlap
-        if overlap:
+        if self._overlap:
             self._gbuf[-64:-63].copy_(loss)
             self._exchange.begin()
             self.model.backward(st.params, saved, dF, grads, on_ready=self._exchange.ready)

@@ -1,24 +1,18 @@
 """GPU probe for attention at head width 128 (run directly on a GPU machine; not a pytest file).
 
-Prints the card's name and power limit, then:
-  1. the fused kernels (fdx_attention_fwd / fdx_attention_bwd at stored width 128) and the unfused path (QK^T GEMM,
-     f32 logits and bf16 probabilities in HBM, softmax, PV GEMM; the backward of FDX_ATTN_UNFUSED=1) at
-     (B=32, h=8, L=Lk=1024), (32, 8, 256, 256) and (32, 8, 1024, 77): milliseconds per call as min / median / max
-     over repeated CUDA-event windows, TFLOP/s from true-width FLOPs (forward 4 B h L Lk d; backward 10 B h L Lk d,
-     the FlashAttention count that includes the recomputed logits) and the peak memory each call adds over its
-     inputs and outputs, next to the size of the (B, h, L, Lk) f32 logits;
-  2. one training step of the README gallery UNet (feature_depths 128 / 256 / 512 / 1024, 8-head attention at the
-     last three levels, 128 x 128 images) fused against FDX_ATTN_UNFUSED=1, the two alternating; where the
-     unfused path runs out of memory the batch is halved until both fit.
+Prints the card's name and power limit, then the fused kernels (fdx_attention_fwd / fdx_attention_bwd at stored
+width 128) and an unfused attention core (QK^T GEMM, f32 logits and bf16 probabilities in HBM, softmax, PV GEMM, and
+its backward) at (B=32, h=8, L=Lk=1024), (32, 8, 256, 256) and (32, 8, 1024, 77): milliseconds per call as
+min / median / max over repeated CUDA-event windows, TFLOP/s from true-width FLOPs (forward 4 B h L Lk d; backward
+10 B h L Lk d, the FlashAttention count that includes the recomputed logits) and the peak memory each call adds over
+its inputs and outputs, next to the size of the (B, h, L, Lk) f32 logits.
 
-usage: python tests/gpu_probe_attn_wide.py [--batch 32] [--steps 10] [--rounds 3] [--skip-train]"""
+usage: python tests/gpu_probe_attn_wide.py [--iters 20] [--rounds 3]"""
 import argparse
-import gc
 import os
 import statistics
 import subprocess
 import sys
-import time
 
 import torch
 
@@ -68,7 +62,7 @@ def peak_extra(fn):
 
 
 def unfused_fwd(q, k, v, heads, dp, scale):
-    """The FDX_ATTN_UNFUSED=1 attention core (Unet._attn_fwd_unfused): S f32 and P in HBM."""
+    """Attention as separate launches: S f32 and P in HBM."""
     Bn, L, HD = q.shape
     Lkp = k.shape[1]
     S = torch.empty((Bn, heads, L, Lkp), dtype=F32, device=dev)
@@ -83,7 +77,7 @@ def unfused_fwd(q, k, v, heads, dp, scale):
 
 
 def unfused_bwd(q, k, v, P, do, heads, dp, scale, valid):
-    """The attention core of Unet._attn_bwd_unfused: dP f32 and dS in HBM."""
+    """The backward of unfused_fwd: dP f32 and dS in HBM."""
     Bn, L, HD = q.shape
     Lkp = k.shape[1]
     dv = torch.empty((Bn, Lkp, HD), dtype=BF16, device=dev)
@@ -117,7 +111,7 @@ def kernels(args, info):
         tb = timed(lambda: ops.attention_bwd(q, k, v, o, lse, do, h, d, scale), args.iters, args.rounds)
         mf = peak_extra(lambda: ops.attention_fwd(q, k, v, h, d, scale))
         mb = peak_extra(lambda: ops.attention_bwd(q, k, v, o, lse, do, h, d, scale))
-        # unfused: keys zero-padded to a multiple of 32, as Unet._attn_fwd_unfused stores them
+        # unfused: keys zero-padded to a multiple of 32 for the tensor-core tiles
         Lkp = (Lk + 31) // 32 * 32
         kp = torch.zeros(B, Lkp, HD, device=dev, dtype=BF16)
         vp = torch.zeros(B, Lkp, HD, device=dev, dtype=BF16)
@@ -140,95 +134,14 @@ def kernels(args, info):
         torch.cuda.empty_cache()
 
 
-def train(args, info, B):
-    from flaxdiff_b200.inputs import DiffusionInputConfig
-    from flaxdiff_b200.models.simple_unet import Unet
-    from flaxdiff_b200.predictors import KarrasPredictionTransform
-    from flaxdiff_b200.schedulers import EDMNoiseScheduler
-    from flaxdiff_b200.trainer import GeneralDiffusionTrainer, adamw
-    res = 128
-    model = Unet(feature_depths=(128, 256, 512, 1024), attention_configs=(None, {"heads": 8}, {"heads": 8},
-                                                                           {"heads": 8}), dtype=torch.bfloat16)
-    trainer = GeneralDiffusionTrainer(model, adamw(1e-4), EDMNoiseScheduler(1, sigma_max=80, rho=7, sigma_data=0.5),
-                                      DiffusionInputConfig("image", (res, res, 3), []), rngs=4,
-                                      model_output_transform=KarrasPredictionTransform(0.5), device=dev,
-                                      use_cuda_graph=False)
-    step_fn = trainer._define_train_step(B)
-    img = torch.randint(0, 256, (B, res, res, 3), dtype=torch.uint8)
-    batch = {"image": img}
-
-    def run(unfused, n):
-        if unfused:
-            os.environ["FDX_ATTN_UNFUSED"] = "1"
-        else:
-            os.environ.pop("FDX_ATTN_UNFUSED", None)
-        try:
-            torch.cuda.synchronize()
-            torch.cuda.empty_cache()                   # the two paths fragment the allocator differently
-            t0 = time.perf_counter()
-            for _ in range(n):
-                trainer.state, loss, trainer.rngstate = step_fn(trainer.state, trainer.rngstate, batch, 0)
-            torch.cuda.synchronize()
-            return (time.perf_counter() - t0) * 1e3 / n, loss.item()
-        finally:
-            os.environ.pop("FDX_ATTN_UNFUSED", None)
-
-    def oom(unfused):
-        try:
-            run(unfused, 2)                            # warm-up
-            return False
-        except torch.cuda.OutOfMemoryError as e:
-            print(f"[{info}] gallery UNet training step 128x128 B={B} {'unfused' if unfused else 'fused'}: out of "
-                  f"memory ({str(e).splitlines()[0][:90]})", flush=True)
-            return True
-
-    if oom(False):
-        return False
-    times = {False: [], True: []}
-    if oom(True):                                      # the fused path alone at this batch
-        for _ in range(args.rounds):
-            times[False].append(run(False, args.steps)[0])
-        t = times[False]
-        print(f"[{info}] gallery UNet training step 128x128 B={B} fused  : {min(t):.1f} / {statistics.median(t):.1f} / "
-              f"{max(t):.1f} ms per step (min/median/max of {args.rounds} rounds x {args.steps} steps)", flush=True)
-        return False
-    try:
-        for _ in range(args.rounds):
-            for unfused in (False, True):
-                times[unfused].append(run(unfused, args.steps)[0])
-    except torch.cuda.OutOfMemoryError as e:
-        print(f"[{info}] gallery UNet training step 128x128 B={B} unfused: out of memory while timing "
-              f"({str(e).splitlines()[0][:90]})", flush=True)
-        return False
-    for unfused in (False, True):
-        t = times[unfused]
-        print(f"[{info}] gallery UNet training step 128x128 B={B} {'unfused' if unfused else 'fused  '}: "
-              f"{min(t):.1f} / {statistics.median(t):.1f} / {max(t):.1f} ms per step (min/median/max of "
-              f"{args.rounds} rounds x {args.steps} steps, alternating)", flush=True)
-    print(f"[{info}] gallery UNet training step B={B} speed-up "
-          f"{statistics.median(times[True]) / statistics.median(times[False]):.2f}x", flush=True)
-    return True
-
-
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--batch", type=int, default=32)
-    ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--skip-train", action="store_true")
     args = ap.parse_args()
     info = card()
     print(f"card: {info}", flush=True)
     kernels(args, info)
-    B = args.batch
-    while not args.skip_train and B >= 4:
-        # where the unfused path runs out of memory, halve the batch until both paths fit
-        if train(args, info, B):
-            break
-        B //= 2
-        gc.collect()
-        torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":

@@ -119,7 +119,6 @@ def record_step(B):
     images = torch.randint(0, 256, (B, res, res, 3), dtype=torch.uint8, generator=gen).to(dev)
     noise = torch.randn(B, res, res, 3, device=dev)
     t = torch.randn(B, device=dev)
-    os.environ["FDX_MICROBATCH"] = "1"
     os.environ["FDX_NO_SIDE"] = "1"
     trainer._overlap = False
     trainer._fwd_bwd(images, noise, t)                 # warm-up: module load, first launches

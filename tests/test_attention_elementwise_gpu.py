@@ -82,12 +82,10 @@ def inputs(B, heads, L, Lk, dh, d_true, regime, seed):
     return out
 
 
-def run(B, heads, L, Lk, dh, d_true, regime="random", seed=0, no_short=False, monkeypatch=None):
+def run(B, heads, L, Lk, dh, d_true, regime="random", seed=0):
     q, k, v, dO = inputs(B, heads, L, Lk, dh, d_true, regime, seed)
     HD = heads * dh
     scale = d_true ** -0.5
-    if no_short:
-        monkeypatch.setenv("FDX_ATTN_NO_SHORT", "1")
     n_st = B * heads * L
     lse_buf = torch.full((n_st + 64,), SENTINEL, dtype=torch.float32, device=dev)
     lse = lse_buf[:n_st].view(B, heads, L)
@@ -109,7 +107,7 @@ def run(B, heads, L, Lk, dh, d_true, regime="random", seed=0, no_short=False, mo
     assert torch.equal(lse_buf[n_st:].view(torch.int32), torch.full_like(lse_buf[n_st:], SENTINEL).view(torch.int32)), \
         "lse: a kernel wrote past its end"
     ref = R.attention_ref(*(t.to(F64) for t in (q, k, v)), heads, dh, scale, dO.to(F64))
-    tag = f"dh={dh} B={B} heads={heads} L={L} Lk={Lk} d={d_true} {regime}" + (" no_short" if no_short else "")
+    tag = f"dh={dh} B={B} heads={heads} L={L} Lk={Lk} d={d_true} {regime}"
     got = {"o": o, "lse": lse, "dq": dq, "dk": dk, "dv": dv}
     for n, t in got.items():
         val, d = ref[n]
@@ -140,10 +138,8 @@ def edge_cases():
 
 
 @pytest.mark.parametrize("B,heads,L,Lk,dh,d_true", edge_cases())
-def test_attention_tile_edges_elementwise(B, heads, L, Lk, dh, d_true, monkeypatch):
+def test_attention_tile_edges_elementwise(B, heads, L, Lk, dh, d_true):
     run(B, heads, L, Lk, dh, d_true, seed=L * 7 + Lk)
-    if Lk <= 128:                                    # the forward's K/V-ring arrangement for short key sequences
-        run(B, heads, L, Lk, dh, d_true, seed=L * 7 + Lk, no_short=True, monkeypatch=monkeypatch)
 
 
 @pytest.mark.parametrize("B,heads,L,Lk,dh,d_true", [
@@ -160,9 +156,7 @@ def test_attention_unet_shapes_elementwise(B, heads, L, Lk, dh, d_true):
 
 @pytest.mark.parametrize("regime", ["rising", "first_max", "one_hot", "negative", "constant"])
 @pytest.mark.parametrize("dh", [32, 64, 128])
-def test_attention_logit_regimes_elementwise(dh, regime, monkeypatch):
+def test_attention_logit_regimes_elementwise(dh, regime):
     heads = 2 if dh == 32 else 1
     run(1, heads, 257, 1024, dh, dh, regime, seed=dh)            # eight key blocks: the online softmax
     run(1, heads, 200, 77, dh, dh, regime, seed=dh + 1)          # 51 zero-filled tail keys in the one block
-    if regime == "negative":
-        run(1, heads, 200, 77, dh, dh, regime, seed=dh + 1, no_short=True, monkeypatch=monkeypatch)

@@ -77,24 +77,6 @@ def test_attention_strided_views_and_determinism():
                                  {"o": o1, "lse": lse1, "dq": g1[0], "dk": g1[1], "dv": g1[2]}, d_o)
 
 
-@pytest.mark.parametrize("B,heads,L,Lk,dh", [(2, 8, 1024, 1024, 64), (1, 4, 200, 300, 32), (2, 8, 384, 77, 64)])
-def test_attention_kernel_arrangements_agree(B, heads, L, Lk, dh, monkeypatch):
-    """The forward's single-stage arrangement for key sequences that fit one 128-key block against the K/V ring
-    (FDX_ATTN_NO_SHORT, read per launch).  Same arithmetic in the same order per element, so the results are
-    bit-identical."""
-    torch.manual_seed(2)
-    HD = heads * dh
-    q, k, v, d_o = (torch.randn(B, n, HD, device=dev).bfloat16() for n in (L, Lk, Lk, L))
-    o, lse = ops.attention_fwd(q, k, v, heads, dh, dh ** -0.5)
-    g = ops.attention_bwd(q, k, v, o, lse, d_o, heads, dh, dh ** -0.5)
-    monkeypatch.setenv("FDX_ATTN_NO_SHORT", "1")
-    o1, lse1 = ops.attention_fwd(q, k, v, heads, dh, dh ** -0.5)
-    g1 = ops.attention_bwd(q, k, v, o, lse, d_o, heads, dh, dh ** -0.5)
-    torch.cuda.synchronize()
-    assert torch.equal(o, o1) and torch.equal(lse, lse1)
-    assert all(torch.equal(a, b) for a, b in zip(g, g1))
-
-
 def test_attention_rejects_unsupported_head_width():
     from flaxdiff_b200._lib import FdxError
     q = torch.zeros(1, 8, 8 * 16, device=dev, dtype=torch.bfloat16)

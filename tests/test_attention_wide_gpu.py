@@ -64,23 +64,6 @@ def test_wide_attention_strided_views_and_determinism():
                                  {"o": o1, "lse": lse1, "dq": g1[0], "dk": g1[1], "dv": g1[2]}, d_o)
 
 
-@pytest.mark.parametrize("B,heads,L,Lk", [(2, 8, 256, 77), (1, 4, 200, 128), (2, 2, 1024, 5)])
-def test_wide_attention_kernel_arrangements_agree(B, heads, L, Lk, monkeypatch):
-    """At <= 128 keys the single-stage forward equals the K/V ring (FDX_ATTN_NO_SHORT) bit for bit."""
-    torch.manual_seed(2)
-    dh = 128
-    HD = heads * dh
-    q, k, v, d_o = (torch.randn(B, n, HD, device=dev).bfloat16() for n in (L, Lk, Lk, L))
-    o, lse = ops.attention_fwd(q, k, v, heads, dh, dh ** -0.5)
-    g = ops.attention_bwd(q, k, v, o, lse, d_o, heads, dh, dh ** -0.5)
-    monkeypatch.setenv("FDX_ATTN_NO_SHORT", "1")
-    o1, lse1 = ops.attention_fwd(q, k, v, heads, dh, dh ** -0.5)
-    g1 = ops.attention_bwd(q, k, v, o, lse, d_o, heads, dh, dh ** -0.5)
-    torch.cuda.synchronize()
-    assert torch.equal(o, o1) and torch.equal(lse, lse1)
-    assert all(torch.equal(a, b) for a, b in zip(g, g1))
-
-
 def test_attention_still_rejects_other_head_widths():
     from flaxdiff_b200._lib import FdxError
     q = torch.zeros(1, 8, 2 * 96, device=dev, dtype=torch.bfloat16)

@@ -149,45 +149,42 @@ def f64(t):
 
 
 # ----------------------------------------------------------------------------------------------- conv3x3 forward
-# (N, H, W, Cin, Cout, stride, epilogue, halo)
+# (N, H, W, Cin, Cout, stride, epilogue)
 FWD = [
-    (256, 64, 64, 64, 64, 1, "bias", True),            # C2 64 x 64
-    (256, 32, 32, 128, 128, 1, "bias+res", True),      # C2 32 x 32
-    (256, 16, 16, 256, 256, 1, "", True),              # C2 16 x 16
-    (2, 256, 256, 64, 64, 1, "bias", True),            # C3 256 x 256
-    (4, 16, 16, 64, 128, 1, "", True),
-    (4, 16, 16, 64, 192, 1, "", True),
-    (4, 16, 16, 64, 320, 1, "", True),                 # 20 tiles: resident
-    (32, 16, 16, 64, 320, 1, "", True),                # 160 tiles: five column blocks do not divide the grid
-    (4, 16, 16, 64, 384, 1, "", True),
-    (8, 16, 16, 64, 448, 1, "bias", True),
-    (4, 16, 16, 128, 128, 1, "bias+res+rowvec", True),
-    (4, 32, 32, 64, 128, 1, "bias", False),            # FDX_TCT_HALO=0: per-tap loads
-    (2, 16, 16, 1024, 1024, 1, "bias", True),          # gallery 16 x 16
-    (4, 8, 8, 1024, 1024, 1, "", True),                # gallery 8 x 8
-    (8, 8, 8, 64, 64, 1, "bias", True),
-    (8, 8, 8, 128, 128, 1, "res", True),
-    (8, 8, 8, 128, 512, 1, "", True),
-    (16, 2, 2, 64, 64, 1, "bias+res+rowvec", True),    # 2 x 2 images: many images per tile
-    (8, 32, 32, 64, 64, 2, "bias", True),              # stride 2, pad (0, 1)
-    (4, 64, 64, 128, 128, 2, "", True),
-    (4, 15, 15, 64, 64, 2, "bias", True),              # stride 2 on odd sizes, pad (1, 1)
+    (256, 64, 64, 64, 64, 1, "bias"),                  # C2 64 x 64
+    (256, 32, 32, 128, 128, 1, "bias+res"),            # C2 32 x 32
+    (256, 16, 16, 256, 256, 1, ""),                    # C2 16 x 16
+    (2, 256, 256, 64, 64, 1, "bias"),                  # C3 256 x 256
+    (4, 16, 16, 64, 128, 1, ""),
+    (4, 16, 16, 64, 192, 1, ""),
+    (4, 16, 16, 64, 320, 1, ""),                       # 20 tiles: resident
+    (32, 16, 16, 64, 320, 1, ""),                      # 160 tiles: five column blocks do not divide the grid
+    (4, 16, 16, 64, 384, 1, ""),
+    (8, 16, 16, 64, 448, 1, "bias"),
+    (4, 16, 16, 128, 128, 1, "bias+res+rowvec"),
+    (2, 16, 16, 1024, 1024, 1, "bias"),                # gallery 16 x 16
+    (4, 8, 8, 1024, 1024, 1, ""),                      # gallery 8 x 8
+    (8, 8, 8, 64, 64, 1, "bias"),
+    (8, 8, 8, 128, 128, 1, "res"),
+    (8, 8, 8, 128, 512, 1, ""),
+    (16, 2, 2, 64, 64, 1, "bias+res+rowvec"),          # 2 x 2 images: many images per tile
+    (8, 32, 32, 64, 64, 2, "bias"),                    # stride 2, pad (0, 1)
+    (4, 64, 64, 128, 128, 2, ""),
+    (4, 15, 15, 64, 64, 2, "bias"),                    # stride 2 on odd sizes, pad (1, 1)
 ]
 
 
 def _fwd_id(c):
-    N, H, W, Ci, Co, s, epi, halo = c
+    N, H, W, Ci, Co, s, epi = c
     Ho, Wo = -(-H // s), -(-W // s)
-    r = launch_route(Wo, Ho, N, Ci, Co, s, halo and s == 1)
+    r = launch_route(Wo, Ho, N, Ci, Co, s, s == 1)
     return f"{r}-B{N}-{H}x{W}-{Ci}to{Co}-s{s}" + (f"-{epi}" if epi else "")
 
 
 @pytest.mark.parametrize("kind", KINDS)
 @pytest.mark.parametrize("case", FWD, ids=[_fwd_id(c) for c in FWD])
-def test_conv3x3_fwd(case, kind, monkeypatch):
-    N, H, W, Ci, Co, s, epi, halo = case
-    if not halo:
-        monkeypatch.setenv("FDX_TCT_HALO", "0")
+def test_conv3x3_fwd(case, kind):
+    N, H, W, Ci, Co, s, epi = case
     g = gen(1)
     Ho, Wo = -(-H // s), -(-W // s)
     x = draw((N, H, W, Ci), kind, g)
@@ -205,36 +202,33 @@ def test_conv3x3_fwd(case, kind, monkeypatch):
 
 
 # ----------------------------------------------------------------------------------------------- conv3x3 data gradient
-# (N, H, W, Cin, Cout, stride, accumulate, halo), (H, W) of dx
+# (N, H, W, Cin, Cout, stride, accumulate), (H, W) of dx
 DGRAD = [
-    (256, 64, 64, 64, 64, 1, False, True),             # C2 64 x 64
-    (256, 32, 32, 128, 128, 1, True, True),            # C2 32 x 32
-    (8, 32, 32, 192, 64, 1, False, True),              # the up path's concat inputs
-    (8, 32, 32, 384, 128, 1, True, True),
-    (8, 16, 16, 128, 128, 1, False, True),
-    (4, 32, 32, 128, 64, 1, True, False),              # FDX_TCT_HALO=0
-    (4, 16, 16, 1024, 1024, 1, False, True),           # gallery 16 x 16
-    (4, 8, 8, 1024, 1024, 1, True, True),              # gallery 8 x 8
-    (8, 8, 8, 64, 64, 1, True, True),
-    (16, 2, 2, 64, 128, 1, False, True),
-    (256, 64, 64, 64, 64, 2, False, True),             # C2 downsample: four parity launches of 4, 2, 2, 1 taps
-    (8, 32, 32, 64, 64, 2, True, True),
-    (8, 16, 16, 128, 128, 2, True, True),              # 8 x 8 dy: pixels-as-M engine
+    (256, 64, 64, 64, 64, 1, False),                   # C2 64 x 64
+    (256, 32, 32, 128, 128, 1, True),                  # C2 32 x 32
+    (8, 32, 32, 192, 64, 1, False),                    # the up path's concat inputs
+    (8, 32, 32, 384, 128, 1, True),
+    (8, 16, 16, 128, 128, 1, False),
+    (4, 16, 16, 1024, 1024, 1, False),                 # gallery 16 x 16
+    (4, 8, 8, 1024, 1024, 1, True),                    # gallery 8 x 8
+    (8, 8, 8, 64, 64, 1, True),
+    (16, 2, 2, 64, 128, 1, False),
+    (256, 64, 64, 64, 64, 2, False),                   # C2 downsample: four parity launches of 4, 2, 2, 1 taps
+    (8, 32, 32, 64, 64, 2, True),
+    (8, 16, 16, 128, 128, 2, True),                    # 8 x 8 dy: pixels-as-M engine
 ]
 
 
 def _dgrad_id(c):
-    N, H, W, Ci, Co, s, acc, halo = c
-    r = launch_route(W // s, H // s, N, Co, Ci, 1, halo and s == 1)
+    N, H, W, Ci, Co, s, acc = c
+    r = launch_route(W // s, H // s, N, Co, Ci, 1, s == 1)
     return ("s2parity-" if s == 2 else "") + f"{r}-B{N}-{H}x{W}-{Ci}from{Co}" + ("-accumulate" if acc else "")
 
 
 @pytest.mark.parametrize("kind", KINDS)
 @pytest.mark.parametrize("case", DGRAD, ids=[_dgrad_id(c) for c in DGRAD])
-def test_conv3x3_dgrad(case, kind, monkeypatch):
-    N, H, W, Ci, Co, s, acc, halo = case
-    if not halo:
-        monkeypatch.setenv("FDX_TCT_HALO", "0")
+def test_conv3x3_dgrad(case, kind):
+    N, H, W, Ci, Co, s, acc = case
     g = gen(2)
     dy = draw((N, H // s, W // s, Co), kind, g)
     w = draw((3, 3, Ci, Co), kind, g, 1 / math.sqrt(9 * Co))

@@ -220,13 +220,16 @@ def test_groupnorm_elementwise_c2_batch():
 
 
 FUSED_SHAPES = [  # (N, H, W, Cin, Cout): Cin 64 ... 512 not a multiple of 256 (the default), and one forced case
-    (2, 16, 16, 64, 64), (2, 32, 32, 192, 128), (2, 16, 16, 320, 64), (3, 16, 16, 448, 64), (2, 16, 8, 256, 64)]
+    (2, 16, 16, 64, 64), (2, 32, 32, 192, 128), (2, 16, 16, 320, 64), (3, 16, 16, 448, 64), (2, 16, 8, 256, 64),
+    (2, 32, 32, 128, 256), (1, 64, 64, 192, 64)]
 
 
+@pytest.mark.parametrize("fused", [True, False], ids=["fused", "two-pass"])
 @pytest.mark.parametrize("N,H,W,C,Co", FUSED_SHAPES)
-def test_groupnorm_conv_dgrad_fused_elementwise(N, H, W, C, Co):
+def test_groupnorm_conv_dgrad_fused_elementwise(N, H, W, C, Co, fused):
     """conv_dgrad_groupnorm_bwd(fused=True): dz = dgrad * silu'(z) in the data gradient's epilogue (a bf16
-    intermediate), then one pass over x and dz; plain with column sums, accumulating and with an addend."""
+    intermediate), then one pass over x and dz; fused=False: the data gradient da as the bf16 intermediate, then
+    the two-pass GroupNorm backward.  Plain with column sums, accumulating and with an addend."""
     G, eps, shape = 8, 1e-4, (N, H, W, C)
     x0, gamma, beta, _ = gn_inputs(shape, G, 11)
     _, x = into_slot(x0)
@@ -251,10 +254,10 @@ def test_groupnorm_conv_dgrad_fused_elementwise(N, H, W, C, Co):
             add = torch.randn(shape, device=dev).bfloat16()
             extra = add.to(F64)
         ops.conv_dgrad_groupnorm_bwd(dy, w, x, G, st, gamma, beta, eps, dg, db, dx, accumulate=mode == "accumulate",
-                                     csum_img=ci, csum_tot=ct, fused=True, addend=add)
+                                     csum_img=ci, csum_tot=ct, fused=fused, addend=add)
         tot = dxv + extra
         report("conv_dgrad_groupnorm_bwd dx", R.assert_elementwise(
-            dx, tot, R.bf16_bound(tot, dxd + R.U32 * tot.abs()), f"fused {mode} dx"))
+            dx, tot, R.bf16_bound(tot, dxd + R.U32 * tot.abs()), f"fused={fused} {mode} dx"))
         assert_neighbours_intact(dxbuf, C)
         for name, got, start in (("dgamma", dg, dg0), ("dbeta", db, db0)):
             v, d = ref[name]

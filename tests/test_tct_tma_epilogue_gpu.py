@@ -3,8 +3,8 @@ image} box per 32-pixel chunk, through a ring of 128-byte-swizzled shared-memory
 The output and the side input are channel slots of wider buffers here (pixel stride above the channel count, a
 non-zero channel offset), so the tensor maps must clip each box to the slot: the channels beside it are random
 sentinels that must come back bit-identical.  Cases: the resident-weight halo launch (K = 64), the plain halo launch
-(K = 128), the per-tap launches (1x1, and 3x3 with FDX_TCT_HALO=0), the fused GroupNorm backward on the halo and
-per-tap paths, an in-place accumulate (side input and output the same view), 64 to 448 columns, and tile counts
+(K = 128), the per-tap 1x1 launches, the fused GroupNorm backward, an in-place accumulate (side input and output
+the same view), 64 to 448 columns, and tile counts
 from one tile to several per CTA, so that each warpgroup's buffer ring wraps across tiles.  Outputs inside the slot
 start as NaN (except where they are the accumulate source), every launch must have run fdx_tct_kernel, and
 results are checked against fp32 torch at the tolerances of test_tct_resident_gpu.py."""
@@ -102,18 +102,17 @@ def test_forward_residual_slot(geom, cout, cin):
 
 
 @pytest.mark.parametrize("geom", sorted(GEOMETRY))
-def test_forward_per_tap_channel_offset_8(geom, monkeypatch):
+def test_1x1_forward_channel_offset_8(geom):
     """per-tap stages; the slots start 16 bytes into the pixel, off the 128-byte line the swizzle works in"""
-    monkeypatch.setenv("FDX_TCT_HALO", "0")
     torch.manual_seed(22)
     B, H, W = GEOMETRY[geom](1)
     x = torch.randn(B, H, W, 64, device=dev).bfloat16()
-    w = (torch.randn(3, 3, 64, 64, device=dev) / 24).bfloat16()
+    w = (torch.randn(64, 64, device=dev) / 8).bfloat16()
     bias = torch.randn(64, device=dev) * 0.3
     res = Slot(B, H, W, 64, 8, 56)
     out = Slot(B, H, W, 64, 8, 8, fill=float("nan"))
-    ops.conv3x3_fwd(x, w, bias, res=res.view, out=out.view)
-    check(out.view, conv_ref(x, w, bias) + res.view.float(), 5e-3, out)
+    ops.conv1x1_fwd(x, w, bias, res=res.view, out=out.view)
+    check(out.view, conv_ref(x, w.view(1, 1, 64, 64), bias) + res.view.float(), 5e-3, out)
 
 
 @pytest.mark.parametrize("cin", [64, 192, 320, 448])
@@ -129,12 +128,9 @@ def test_dgrad_accumulate_in_place_slot(geom, cin):
     check(dx.view, prior + dgrad_ref(dy, w), 5e-3, dx)
 
 
-@pytest.mark.parametrize("halo", [True, False])
 @pytest.mark.parametrize("cin", [64, 320])
 @pytest.mark.parametrize("geom", sorted(GEOMETRY))
-def test_dgrad_fused_groupnorm_backward_slots(geom, cin, halo, monkeypatch):
-    if not halo:
-        monkeypatch.setenv("FDX_TCT_HALO", "0")
+def test_dgrad_fused_groupnorm_backward_slots(geom, cin):
     torch.manual_seed(24)
     B, H, W = GEOMETRY[geom](cin // 64)
     dy = torch.randn(B, H, W, 64, device=dev).bfloat16()

@@ -37,7 +37,5 @@ def test_full_transformer_block_at_1024_channels_constructs():
     assert lay["middle_attention_0/Attention/Attention2/to_k/kernel"] == (768, 8, 128)
 
 
-def test_stored_head_widths(monkeypatch):
+def test_stored_head_widths():
     assert [_attn_width(d) for d in (8, 16, 32, 48, 64, 65, 80, 96, 128)] == [32, 32, 32, 64, 64, 128, 128, 128, 128]
-    monkeypatch.setenv("FDX_ATTN_PAD64", "1")
-    assert [_attn_width(d) for d in (16, 32, 64, 96, 128)] == [64, 64, 64, 128, 128]
