@@ -364,6 +364,22 @@ struct WgAcc {
   }
 };
 
+// ----- ldmatrix / stmatrix --------------------------------------------------------------
+// Four 8 x 8 b16 matrices; lane l gives the shared address of row l % 8 of matrix l / 8.  With .trans, register i
+// of lane l holds (or receives) elements (2 (l % 4), l / 4) and (2 (l % 4) + 1, l / 4) of matrix i as stored, so a
+// row-major [pixel][channel] tile maps onto the (channel row, pixel pair) layout of a wgmma accumulator fragment.
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]),
+               "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+
 // ----- misc ------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

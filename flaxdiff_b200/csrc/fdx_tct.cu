@@ -26,31 +26,32 @@
 namespace {
 
 constexpr int kThreads = 3 * 128;            // two consumer warpgroups + the producer warpgroup
-constexpr int kLdT = 64 + 4;                 // row of the transposed exchange tile [32 px][64 channel rows]
 constexpr int kWBytes = 64 * 128;            // weight tile: 64 channels x 64 k bf16
 constexpr int kPixBytes = 2 * 128 * 128;     // two boxes of 128 pixels x 64 channels bf16
 constexpr int kHaloBytes = 18 * 16 * 128;    // 16 x 18 pixel box
-constexpr int kXchgBytes = 32 * kLdT * 4;    // one warpgroup's exchange tile
 constexpr int kChunkBytes = 32 * 128;        // one epilogue chunk: 32 pixels x 64 channels bf16 (one TMA box)
-constexpr int kCBufs = 3;                    // chunk buffers per consumer warpgroup
-constexpr int kEpiBytes = 2 * kCBufs * kChunkBytes;
-static_assert((2 * 4 + 1 + 2 * kCBufs) * 8 <= 256, "tct: barrier area");
+// Chunk buffers per consumer warpgroup: the side input of a tile's first num_cbufs chunks is requested before
+// its main loop and each later chunk's num_cbufs - 1 chunks ahead, so more buffers hide more of the HBM latency.
+// The halo rings leave room for five; the five-stage per-tap ring for three.
+__host__ __device__ constexpr int num_cbufs(bool halo) { return halo ? 5 : 3; }
+__host__ __device__ constexpr int epi_bytes(bool halo) { return 2 * num_cbufs(halo) * kChunkBytes; }
+static_assert((2 * 5 + 1 + 2 * 3) * 8 <= 256 && (2 * 3 + 1 + 2 * 5) * 8 <= 256, "tct: barrier area");
 
 // RES (halo at K = 64 only): the nine weight tiles stay resident after the ring, so a stage is the pixel box alone
 __host__ __device__ constexpr int stage_bytes(bool halo, bool res) {
   return halo ? (res ? 0 : 3 * kWBytes) + kHaloBytes : kWBytes + kPixBytes;
 }
-// per-tap: a fifth 40 KB stage does not fit beside the chunk buffers
-__host__ __device__ constexpr int num_stages(bool halo) { return halo ? 3 : 4; }
+// halo: a fourth 60 KB (or, with RES, 36 KB) stage does not fit beside the chunk buffers
+__host__ __device__ constexpr int num_stages(bool halo) { return halo ? 3 : 5; }
 __host__ __device__ constexpr int wres_bytes(bool res) { return res ? 9 * kWBytes : 0; }
 __host__ __device__ constexpr int ring_bytes(bool halo, bool res) {
   return num_stages(halo) * stage_bytes(halo, res) + wres_bytes(res);
 }
-// ring (+ resident weights), chunk buffers, barriers, exchange tiles; 1024 = alignment slack of the dynamic base
+// ring (+ resident weights), chunk buffers, barriers; 1024 = alignment slack of the dynamic base
 __host__ __device__ constexpr int smem_bytes(bool halo, bool res) {
-  return ring_bytes(halo, res) + kEpiBytes + 1024 + 256 + 2 * kXchgBytes;
+  return ring_bytes(halo, res) + epi_bytes(halo) + 1024 + 256;
 }
-// halo and RES: 180 + 24 + 18.25 = 222.25 KB; per-tap: 160 + 24 + 18.25 = 202.25 KB
+// halo and RES: 180 + 40 + 1.25 = 221.25 KB; per-tap: 200 + 24 + 1.25 = 225.25 KB
 static_assert(smem_bytes(true, false) <= 227 * 1024 && smem_bytes(true, true) <= 227 * 1024 &&
               smem_bytes(false, false) <= 227 * 1024, "tct: shared memory");
 static_assert((num_stages(true) * stage_bytes(true, true)) % 1024 == 0, "tct: resident weights need 1024-byte alignment");
@@ -101,11 +102,12 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
   constexpr int kStageBytes = stage_bytes(HALO, RES);
   constexpr int S = num_stages(HALO);
   constexpr int kRingBytes = ring_bytes(HALO, RES);                // the ring, then the resident weights
+  constexpr int kCBufs = num_cbufs(HALO);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* wres = smem + S * kStageBytes;                          // RES: tap t at t * kWBytes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes + kEpiBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRingBytes + epi_bytes(HALO));
   uint64_t* full = bars;
   uint64_t* empty = bars + S;
   uint64_t* wfull = bars + 2 * S;                                  // RES: the resident weights have landed
@@ -169,31 +171,29 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
   } else {
     consumer_regs();
     // ============ consumers: warpgroup wg owns the CTA's local tiles wg, wg + 2, ... =========================
-    // The f32 values of a 32-pixel chunk are transposed through the warpgroup's shared-memory tile
-    // [32 px][64 channel rows] and leave as 16-byte channel pieces: warp q owns channels 16 q .. 16 q + 15,
-    // lane -> (pixel l % 16 + 16 k, piece l / 16).  A lane always owns the same 8 channels, so bias, timestep
-    // row and the fused GroupNorm sums are per-lane registers, reduced once per tile.
+    // The epilogue works in the accumulator's own layout: lane l of warp q holds channel rows 16 q + l / 4 and
+    // 16 q + l / 4 + 8 of the tile's 64, and pixel pairs 8 j + 2 (l % 4).  A lane always owns the same two
+    // channels, so bias, timestep row and the fused GroupNorm sums are per-lane registers, reduced once per tile.
     const int q = warp & 3;
     const int wg = warp >> 2;
     const int t128 = threadIdx.x & 127;
     const bool wg_leader = t128 == 0;
-    const int xbar = 1 + wg;                             // named barrier of this warpgroup's exchange tile
+    const int xbar = 1 + wg;                             // named barrier of this warpgroup's chunk buffers
     // MMA hand-off: a warpgroup waits on barrier 3 + wg before its main loop and, after issuing it, arrives on
     // the other's, so the two main loops never interleave on the tensor cores.  It is also what makes the ring's
     // parity waits sound: a warpgroup starts on its tile's stages only after the other has waited on all earlier
     // ones, so no full[] barrier is ever waited on more than one phase ahead (a parity wait one phase early
     // would pass at once, on a stage not yet loaded).
     const int my_turn = 3 + wg, their_turn = 4 - wg;
-    float* xsT = reinterpret_cast<float*>(smem + kRingBytes + kEpiBytes + 256) + wg * (32 * kLdT);
-    const int piece = lane >> 4, prow = lane & 15;
-    const int srow = q * 16 + piece * 8;                 // exchange-tile row (channel) of this lane's first channel
+    const int crow = q * 16 + (lane >> 2);               // this lane's first channel row; the second is crow + 8
     float acc[128];
     // Side input and output move by TMA through the warpgroup's kCBufs chunk buffers.  Chunk c of a tile is
     // pixel rows 2 c, 2 c + 1 of its 16 x 16 block, 64 channels: one {64, 16, 2, 1} box, 128-byte swizzled, so
-    // the 16-byte pieces a quarter-warp reads (8 pixels, one channel piece) fall in 8 different bank groups.
-    // The warpgroup's n-th chunk (8 per tile) uses buffer n % kCBufs and barrier phase n / kCBufs.  The side
-    // input arrives in the buffer, each thread overwrites the pieces it read with its output, and one store
-    // sends the buffer back.  The leader thread issues all of it: bulk async-groups are per thread, so only the
+    // the eight 16-byte rows of one 8 x 8 ldmatrix / stmatrix matrix (8 pixels, one channel piece) fall in 8
+    // different bank groups.  The warpgroup's n-th chunk (8 per tile) uses buffer n % kCBufs and barrier phase
+    // n / kCBufs.  The side input arrives in the buffer, each warp reads its 16 channels of it into accumulator
+    // layout (ldmatrix.trans), overwrites them with its output (stmatrix.trans), and one store sends the buffer
+    // back.  The leader thread issues all of it: bulk async-groups are per thread, so only the
     // thread that committed a buffer's store can tell when its buffer may be refilled.  Side input and output
     // are touched once and carry the evict-first L2 policy, so they do not push out the pixel boxes that
     // neighbouring tiles still read.
@@ -225,23 +225,23 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
 #pragma unroll
         for (int c = 0; c < kCBufs; ++c) load_chunk(tc, c, n0 + c);
       }
-      const int ch = tc.cb * 64 + srow;                    // read phase: this lane's first channel
-      float add[8];
+      const int ch = tc.cb * 64 + crow;                    // this lane's channels: ch and ch + 8
+      float add[2];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        add[j] = 0.f;
+      for (int h = 0; h < 2; ++h) {
+        add[h] = 0.f;
         if constexpr (!GNB) {   // GNB launches have neither (fdx_tct_launch): the zeros then hold no registers
-          if (p.bias) add[j] += __ldg(p.bias + ch + j);
-          if (p.rowvec) add[j] += __ldg(p.rowvec + (long long)nb * p.Ncols + ch + j);
+          if (p.bias) add[h] += __ldg(p.bias + ch + 8 * h);
+          if (p.rowvec) add[h] += __ldg(p.rowvec + (long long)nb * p.Ncols + ch + 8 * h);
         }
       }
-      float ga[8], gb[8];
+      float ga[2], gb[2];
       if constexpr (GNB) {
-        const float4* a4 = reinterpret_cast<const float4*>(p.gn_ab + (long long)nb * 2 * p.Ncols + ch);
-        const float4* b4 = reinterpret_cast<const float4*>(p.gn_ab + ((long long)nb * 2 + 1) * p.Ncols + ch);
-        const float4 a0 = __ldg(a4), a1 = __ldg(a4 + 1), b0 = __ldg(b4), b1 = __ldg(b4 + 1);
-        ga[0] = a0.x; ga[1] = a0.y; ga[2] = a0.z; ga[3] = a0.w; ga[4] = a1.x; ga[5] = a1.y; ga[6] = a1.z; ga[7] = a1.w;
-        gb[0] = b0.x; gb[1] = b0.y; gb[2] = b0.z; gb[3] = b0.w; gb[4] = b1.x; gb[5] = b1.y; gb[6] = b1.z; gb[7] = b1.w;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          ga[h] = __ldg(p.gn_ab + (long long)nb * 2 * p.Ncols + ch + 8 * h);
+          gb[h] = __ldg(p.gn_ab + ((long long)nb * 2 + 1) * p.Ncols + ch + 8 * h);
+        }
       }
       // ---- main loop: the ring holds the CTA's tiles in order; this tile's stages start at i * nst ----
       int stage = (i * nst) % S;
@@ -282,100 +282,86 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
       // the tile's coordinates again: kept in registers across the main loop, they make the GroupNorm-backward
       // variants spill
       const TileCoord ec = tile_coord(p, tile);
-      float s0[8], s1[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { s0[j] = 0.f; s1[j] = 0.f; }
+      float s0[2] = {0.f, 0.f}, s1[2] = {0.f, 0.f};
+      // ldmatrix / stmatrix address of this lane: row l % 8 of matrix l / 8 = (8-pixel group 2 hp + l / 16,
+      // channel half (l / 8) % 2), i.e. box row 8 (l / 16) + l % 8 of the half chunk hp and the 16-byte unit of
+      // channels 16 q + 8 ((l / 8) % 2) .. + 7, under the 128-byte swizzle (unit u -> u ^ (row % 8))
+      const uint32_t lane_off =
+          ((lane >> 4) * 8 + (lane & 7)) * 128 + (((2 * q + ((lane >> 3) & 1)) ^ (lane & 7)) << 4);
       // Unrolled: the chunk index is a compile-time register index, and the 16 accumulator registers of a
       // chunk die once it is written out.
 #pragma unroll
       for (int ci = 0; ci < 8; ++ci) {
         const int n = n0 + ci;
-        uint8_t* cb = cbuf + (n % kCBufs) * kChunkBytes;
-        // ---- write phase: accumulator fragments of columns 32 ci .. 32 ci + 31 -> xsT[px][channel row] ----
-        named_bar_sync(xbar, 128);                       // the previous chunk's reads and buffer writes are done
-        if (wg_leader) {
-          if (ci > 0) store_chunk(ec, ci - 1, n - 1);
-          bulk_wait_group_read<kCBufs - 1>();            // this chunk's buffer has been read by its last store
+        const uint32_t cb = smem_u32(cbuf + (n % kCBufs) * kChunkBytes);
+        if (ci > 0) {
+          named_bar_sync(xbar, 128);                     // every warp has written and fenced chunk ci - 1
+          if (wg_leader) store_chunk(ec, ci - 1, n - 1);
         }
-        {
-          const int w = t128 >> 5, l = t128 & 31;
+        if (p.has_res) mbar_wait(&wg_cfull[n % kCBufs], (n / kCBufs) & 1);
+        // columns 32 ci .. 32 ci + 31 = pixel rows 2 ci, 2 ci + 1; half hp = 8-pixel groups 2 hp, 2 hp + 1
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int r = w * 16 + (l >> 2), n = jj * 8 + 2 * (l & 3);
-            const float* d = &acc[(ci * 4 + jj) * 4];
-            xsT[n * kLdT + r] = d[0];
-            xsT[(n + 1) * kLdT + r] = d[1];
-            xsT[n * kLdT + r + 8] = d[2];
-            xsT[(n + 1) * kLdT + r + 8] = d[3];
-          }
-        }
-        named_bar_sync(xbar, 128);
-        if (p.has_res) {
-          // refill the buffer the previous chunk's store (issued above) is reading: the side input of chunk
-          // ci + kCBufs - 1, two chunks before it is needed
-          if (wg_leader && ci > 0 && ci + kCBufs - 1 < 8) {
-            bulk_wait_group_read<0>();
-            load_chunk(ec, ci + kCBufs - 1, n + kCBufs - 1);
-          }
-          mbar_wait(&wg_cfull[n % kCBufs], (n / kCBufs) & 1);
-        }
-        // ---- read phase: 16-byte channel pieces; columns 32 ci .. 32 ci + 31 = pixel rows 2 ci, 2 ci + 1 ----
+        for (int hp = 0; hp < 2; ++hp) {
+          const uint32_t addr = cb + hp * 16 * 128 + lane_off;
+          uint32_t r[4];
+          if (p.has_res) ldmatrix_x4_trans(addr, r);
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const int j = prow + 16 * k;                     // pixel (column) within the chunk = box row
-          const float4 a = *reinterpret_cast<const float4*>(xsT + j * kLdT + srow);
-          const float4 b = *reinterpret_cast<const float4*>(xsT + j * kLdT + srow + 4);
-          float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+          for (int m = 0; m < 4; ++m) {
+            const int h = m & 1;                           // channel row crow + 8 h
+            const float* d = &acc[(ci * 4 + 2 * hp + (m >> 1)) * 4 + 2 * h];
+            float f[2] = {d[0] * p.alpha + add[h], d[1] * p.alpha + add[h]};
+            float xv[2];
+            if (p.has_res) {
+              const float2 x2 = unpack_bf16x2(r[m]);
+              xv[0] = x2.x; xv[1] = x2.y;
+              if constexpr (GNB) {
 #pragma unroll
-          for (int e = 0; e < 8; ++e) f[e] = f[e] * p.alpha + add[e];
-          // this lane's 16-byte piece of box row j under the 128-byte swizzle (16-byte unit u -> u ^ (row % 8))
-          uint4* piece_p = reinterpret_cast<uint4*>(cb + j * 128 + (((srow >> 3) ^ (j & 7)) << 4));
-          float xv[8];
-          if (p.has_res) {
-            const uint4 r = *piece_p;
-            const float2 r0 = unpack_bf16x2(r.x), r1 = unpack_bf16x2(r.y), r2 = unpack_bf16x2(r.z),
-                         r3 = unpack_bf16x2(r.w);
-            xv[0] = r0.x; xv[1] = r0.y; xv[2] = r1.x; xv[3] = r1.y;
-            xv[4] = r2.x; xv[5] = r2.y; xv[6] = r3.x; xv[7] = r3.y;
-            if constexpr (GNB) {
+                for (int e = 0; e < 2; ++e) f[e] = epi_silu_grad_times(f[e], fmaf(xv[e], ga[h], gb[h]));
+              } else {
 #pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = epi_silu_grad_times(f[e], fmaf(xv[e], ga[e], gb[e]));
-            } else {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] += xv[e];
+                for (int e = 0; e < 2; ++e) f[e] += xv[e];
+              }
+            }
+            r[m] = pack_bf16x2(f[0], f[1]);
+            if (p.cs_ws) {
+              const float2 hv = unpack_bf16x2(r[m]);
+              // second factor: the GroupNorm input x (GNB) or the stored value itself (forward column statistics)
+              s0[h] += hv.x; s1[h] = fmaf(hv.x, GNB ? xv[0] : hv.x, s1[h]);
+              s0[h] += hv.y; s1[h] = fmaf(hv.y, GNB ? xv[1] : hv.y, s1[h]);
             }
           }
-          uint4 o;
-          o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]);
-          o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
-          *piece_p = o;
-          if (p.cs_ws) {
-            const float2 h0 = unpack_bf16x2(o.x), h1 = unpack_bf16x2(o.y), h2 = unpack_bf16x2(o.z),
-                         h3 = unpack_bf16x2(o.w);
-            const float hv[8] = {h0.x, h0.y, h1.x, h1.y, h2.x, h2.y, h3.x, h3.y};
-            // second factor: the GroupNorm input x (GNB) or the stored value itself (forward column statistics)
-#pragma unroll
-            for (int e = 0; e < 8; ++e) { s0[e] += hv[e]; s1[e] = fmaf(hv[e], GNB ? xv[e] : hv[e], s1[e]); }
-          }
+          stmatrix_x4_trans(addr, r);                      // the rows ldmatrix read: each warp owns its channels
         }
         fence_proxy_async_smem();                        // the buffer's new contents, visible to the TMA store
+        if (wg_leader) {
+          if (p.has_res) {
+            // refill the buffer of chunk ci - 1, whose store was issued at the top of this chunk: the side input
+            // of chunk ci + kCBufs - 1, kCBufs - 1 chunks before it is needed
+            if (ci > 0 && ci + kCBufs - 1 < 8) {
+              bulk_wait_group_read<0>();
+              load_chunk(ec, ci + kCBufs - 1, n + kCBufs - 1);
+            }
+          } else {
+            bulk_wait_group_read<kCBufs - 2>();          // chunk n + 1's buffer has been read by its last store
+          }
+        }
       }
       named_bar_sync(xbar, 128);
       if (wg_leader) store_chunk(ec, 7, n0 + 7);
       if (p.cs_ws) {
-        // the 16 lanes with the same piece (l / 16) hold the same 8 channels: combine them
+        // the four lanes of a quad hold the same two channels: combine them
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-          for (int o = 1; o < 16; o <<= 1) {
-            s0[e] += __shfl_xor_sync(0xffffffffu, s0[e], o);
-            s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], o);
+          for (int o = 1; o < 4; o <<= 1) {
+            s0[h] += __shfl_xor_sync(0xffffffffu, s0[h], o);
+            s1[h] += __shfl_xor_sync(0xffffffffu, s1[h], o);
           }
         }
-        if (prow == 0) {
-          float* w = p.cs_ws + (((long long)(tile % p.cs_slots) * p.nimg + ec.nb) * 2) * p.cs_ld + ec.cb * 64 + srow;
+        if ((lane & 3) == 0) {
+          float* w = p.cs_ws + (((long long)(tile % p.cs_slots) * p.nimg + ec.nb) * 2) * p.cs_ld + ec.cb * 64 + crow;
 #pragma unroll
-          for (int e = 0; e < 8; ++e) { atomicAdd(w + e, s0[e]); atomicAdd(w + p.cs_ld + e, s1[e]); }
+          for (int h = 0; h < 2; ++h) { atomicAdd(w + 8 * h, s0[h]); atomicAdd(w + p.cs_ld + 8 * h, s1[h]); }
         }
       }
     }
