@@ -50,6 +50,33 @@ def _attn_width(d: int) -> int:
     return 32 if d <= 32 else 64
 
 
+def _dense_wgrad(g: torch.Tensor, x2: torch.Tensor, dy2: torch.Tensor, head_axis: Optional[int] = None,
+                 dp: int = 0):
+    """g += x2^T dy2: the f32 kernel gradient of a dense layer y2 = x2 W (x2 [rows, K], dy2 [rows, N] bf16,
+    row-strided).  An attention kernel whose head axis `head_axis` of g is stored `dp` wide (Unet._pad_heads)
+    has its padded gradient formed in a scratch buffer, and the true head columns are added into g."""
+    K, N = x2.shape[1], dy2.shape[1]
+    padded = head_axis is not None and g.shape[head_axis] != dp
+    dst = torch.zeros((K, N), dtype=F32, device=g.device) if padded else g.view(K, N)
+    ops.gemm(GEMM_MNMN, x2, dy2, dst, K, N, x2.shape[0], x2.stride(0), dy2.stride(0), N, atomic=True,
+             reduce_batch=True)
+    if padded:
+        shape = list(g.shape)
+        shape[head_axis] = dp
+        g.add_(dst.view(shape).narrow(head_axis, 0, g.shape[head_axis]))
+
+
+def _dense_dgrad(dy2: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None,
+                 res: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out = dy2 w^T (+ res): the input gradient of a dense layer with bf16 kernel w [K, N] (dy2 [rows, N];
+    out / res [rows, K]; all row-strided)."""
+    K, N = w.shape
+    if out is None:
+        out = torch.empty((dy2.shape[0], K), dtype=BF16, device=dy2.device)
+    ops.gemm(GEMM_KK, dy2, w, out, dy2.shape[0], K, N, dy2.stride(0), N, out.stride(0),
+             res=res, r_ld=(res.stride(0) if res is not None else 0))
+    return out
+
 
 class _SideStream:
     """Weight-gradient kernels have no consumer before the optimizer step, so the backward pass issues them
@@ -466,11 +493,7 @@ class Unet:
                 cur = dst
             elif kind == "attn":
                 dst = out_node(idx, h, w, cin)
-                if cout.get("only_pure_attention", True) and not cout.get("use_projection", False):
-                    rec = self._attn_fwd(name, cur, dst, cout["heads"], W, W16, ctx16)
-                else:
-                    rec = self._tblock_fwd(name, cur, dst, cout, W, W16, ctx16)
-                tape.append(rec)
+                tape.append(self._tblock_fwd(name, cur, dst, cout, W, W16, ctx16))
                 cur = dst
             elif kind == "down":
                 h, w = h // 2, w // 2
@@ -540,50 +563,14 @@ class Unet:
         pads = [0, 0] * (w.dim() - 1 - axis) + [0, dp - d]
         return torch.nn.functional.pad(w, pads)
 
-    def _attn_fwd(self, name, xin: Node, dst: Node, heads, W, W16, ctx16=None):
-        """TransformerBlock(only_pure_attention) (models/attention.py:321-380): xn = RMSNorm(x);
-        out = xn + to_out(softmax(q k^T / sqrt(d)) v), keys / values from `textcontext` (cross-attention,
-        77 x 768) or from xn itself.  q / k / v / out projections are tensor-core GEMMs; the attention core is ONE
-        fused kernel (fdx_attention_fwd: logits and probabilities stay in registers / shared memory).  Heads
-        narrower than 32 are zero-padded to 32, and heads of 65 - 127 channels to 128 (the kernel stores heads
-        32, 64 or 128 wide)."""
-        x = xin.t
-        Bn, hh, ww, C = x.shape
-        L = hh * ww
-        d = C // heads
-        dp = _attn_width(d)
-        if d > 128:
-            raise FdxError(f"attention: head width {d} > 128 is not supported")
-        HD = heads * dp
-        base = f"{name}/Attention/Attention2"
-        dev = x.device
-        xn = ops.rmsnorm_fwd(x, W[f"{name}/RMSNorm_0/scale"], ATTN_EPS)
-        x2 = xn.view(Bn * L, C)
-        if ctx16 is None:
-            ctx, Lk, Cc = xn.view(Bn, L, C), L, C
-        else:
-            ctx, Lk, Cc = ctx16, ctx16.shape[1], ctx16.shape[2]
-        wq = self._pad_heads(W16[f"{base}/to_q/kernel"], 2, d, dp).reshape(C, HD)
-        wk = self._pad_heads(W16[f"{base}/to_k/kernel"], 2, d, dp).reshape(Cc, HD)
-        wv = self._pad_heads(W16[f"{base}/to_v/kernel"], 2, d, dp).reshape(Cc, HD)
-        wo = self._pad_heads(W16[f"{base}/to_out_0/kernel"], 1, d, dp).reshape(HD, C)
-        q = ops.linear_fwd(x2, wq).view(Bn, L, HD)
-        k = torch.empty((Bn, Lk, HD), dtype=BF16, device=dev)
-        v = torch.empty((Bn, Lk, HD), dtype=BF16, device=dev)
-        ops.linear_fwd(ctx.reshape(Bn * Lk, Cc), wk, out=k.view(Bn * Lk, HD))
-        ops.linear_fwd(ctx.reshape(Bn * Lk, Cc), wv, out=v.view(Bn * Lk, HD))
-        o, lse = ops.attention_fwd(q, k, v, heads, dp, d ** -0.5)
-        out2 = dst.t
-        ops.gemm(GEMM_KMN, o, wo, out2, Bn * L, C, HD, HD, C, out2.stride(2), res=xn, r_ld=C)
-        return ("attn", name, xin, dst, heads, xn, q, k, v, lse, o, ctx if ctx16 is not None else None,
-                (wq, wk, wv, wo), Lk)
-
-
-    # ------------------------------------------------------------------ full transformer block (f3)
+    # ------------------------------------------------------------------ transformer block
     def _mha_fwd(self, base, xq: torch.Tensor, ctx: torch.Tensor, heads: int, W16, res: torch.Tensor,
                  out: torch.Tensor):
         """NormalAttention (models/attention.py:117-177) on 2-D token matrices: out = res + to_out(attn(
-        to_q(xq), to_k(ctx), to_v(ctx))).  xq [B, L, C], ctx [B, Lk, Cc] bf16; res / out [B*L, C]."""
+        to_q(xq), to_k(ctx), to_v(ctx))).  xq [B, L, C], ctx [B, Lk, Cc] bf16; res / out [B*L, C], row-strided.
+        The projections are tensor-core GEMMs; the attention core is ONE fused kernel (fdx_attention_fwd: logits
+        and probabilities stay in registers / shared memory).  Heads narrower than 32 are zero-padded to 32, and
+        heads of 65 - 127 channels to 128 (the kernel stores heads 32, 64 or 128 wide)."""
         Bn, L, C = xq.shape
         Lk, Cc = ctx.shape[1], ctx.shape[2]
         d = C // heads
@@ -602,54 +589,35 @@ class Unet:
         ops.gemm(GEMM_KMN, o, wo, out, Bn * L, C, HD, HD, C, out.stride(0), res=res, r_ld=res.stride(0))
         return (base, xq, ctx, heads, q, k, v, o, lse, (wq, wk, wv, wo))
 
-    def _mha_bwd(self, saved, dout: torch.Tensor, Gd):
-        """-> (d xq [B*L, C], d ctx [B*Lk, Cc]) bf16 given dout = d(out) [B*L, C] (the residual path is the
-        caller's); accumulates the four projection-kernel gradients."""
+    def _mha_bwd(self, saved, dout: torch.Tensor, Gd, res: Optional[torch.Tensor] = None,
+                 kv: Optional[str] = "split"):
+        """-> (d xq [B*L, C], d ctx [B*Lk, Cc] or None) bf16 given dout = d(out) [B*L, C] (row-strided), with
+        `res` (the residual path's gradient) added into d xq when given; accumulates the four projection-kernel
+        gradients.  fdx_attention_bwd recomputes the logits on chip from the saved log-sum-exp.  `kv` routes the
+        key / value paths: "split" returns them as d ctx, "fold" accumulates them into d xq (ctx is xq), None
+        skips them (ctx is a constant such as the text context)."""
         base, xq, ctx, heads, q, k, v, o, lse, (wq, wk, wv, wo) = saved
         Bn, L, C = xq.shape
         Lk, Cc = ctx.shape[1], ctx.shape[2]
         d = C // heads
         dp = _attn_width(d)
-        HD = heads * dp
         M, Mk = Bn * L, Bn * Lk
-        dev = xq.device
-
-        def wgrad(pname, src2, dy2, rows, kin, shape_view, sl):
-            g = Gd[pname]
-            if dp == d:
-                ops.gemm(GEMM_MNMN, src2, dy2, g.view(-1, dy2.shape[1]) if shape_view is None else g.view(shape_view),
-                         kin, dy2.shape[1], rows, src2.stride(0), dy2.stride(0), dy2.shape[1], atomic=True,
-                         reduce_batch=True)
-            else:
-                tmp = torch.zeros((kin, dy2.shape[1]), dtype=F32, device=dev)
-                ops.gemm(GEMM_MNMN, src2, dy2, tmp, kin, dy2.shape[1], rows, src2.stride(0), dy2.stride(0),
-                         dy2.shape[1], atomic=True, reduce_batch=True)
-                g.add_(tmp.view(sl[0])[sl[1]])
-
-        o2 = o.view(M, HD)
-        g_o = Gd[f"{base}/to_out_0/kernel"]
-        if dp == d:
-            ops.gemm(GEMM_MNMN, o2, dout, g_o.view(HD, C), HD, C, M, HD, dout.stride(0), C, atomic=True,
-                     reduce_batch=True)
-        else:
-            tmp = torch.zeros((HD, C), dtype=F32, device=dev)
-            ops.gemm(GEMM_MNMN, o2, dout, tmp, HD, C, M, HD, dout.stride(0), C, atomic=True, reduce_batch=True)
-            g_o.add_(tmp.view(heads, dp, C)[:, :d, :])
-        do = torch.empty((Bn, L, HD), dtype=BF16, device=dev)
-        ops.gemm(GEMM_KK, dout, wo, do, M, HD, C, dout.stride(0), C, HD)
+        _dense_wgrad(Gd[f"{base}/to_out_0/kernel"], o.view(M, -1), dout, 1, dp)
+        do = _dense_dgrad(dout, wo).view(q.shape)
         dq, dk, dv = ops.attention_bwd(q, k, v, o, lse, do, heads, dp, d ** -0.5)
-        dq2, dk2, dv2 = dq.view(M, HD), dk.view(Mk, HD), dv.view(Mk, HD)
-        xq2, ctx2 = xq.reshape(M, C), ctx.reshape(Mk, Cc)
-        pad_view = ((C, heads, dp), (slice(None), slice(None), slice(0, d)))
-        wgrad(f"{base}/to_q/kernel", xq2, dq2, M, C, (C, HD), pad_view)
-        pad_view_c = ((Cc, heads, dp), (slice(None), slice(None), slice(0, d)))
-        wgrad(f"{base}/to_k/kernel", ctx2, dk2, Mk, Cc, (Cc, HD), pad_view_c)
-        wgrad(f"{base}/to_v/kernel", ctx2, dv2, Mk, Cc, (Cc, HD), pad_view_c)
-        dxq = torch.empty((M, C), dtype=BF16, device=dev)
-        ops.gemm(GEMM_KK, dq2, wq, dxq, M, C, HD, HD, HD, C)
-        dctx = torch.empty((Mk, Cc), dtype=BF16, device=dev)
-        ops.gemm(GEMM_KK, dk2, wk, dctx, Mk, Cc, HD, HD, HD, Cc)
-        ops.gemm(GEMM_KK, dv2, wv, dctx, Mk, Cc, HD, HD, HD, Cc, res=dctx, r_ld=Cc)
+        dq2, dk2, dv2 = dq.view(M, -1), dk.view(Mk, -1), dv.view(Mk, -1)
+        ctx2 = ctx.reshape(Mk, Cc)
+        _dense_wgrad(Gd[f"{base}/to_q/kernel"], xq.reshape(M, C), dq2, 2, dp)
+        _dense_wgrad(Gd[f"{base}/to_k/kernel"], ctx2, dk2, 2, dp)
+        _dense_wgrad(Gd[f"{base}/to_v/kernel"], ctx2, dv2, 2, dp)
+        dxq = _dense_dgrad(dq2, wq, res=res)
+        dctx = None
+        if kv == "fold":
+            _dense_dgrad(dk2, wk, out=dxq, res=dxq)
+            _dense_dgrad(dv2, wv, out=dxq, res=dxq)
+        elif kv == "split":
+            dctx = _dense_dgrad(dk2, wk)
+            _dense_dgrad(dv2, wv, out=dctx, res=dctx)
         return dxq, dctx
 
     @staticmethod
@@ -659,14 +627,15 @@ class Unet:
         ops.act_add(v(a), v(b), v(out))
 
     def _tblock_fwd(self, name, xin: Node, dst: Node, acfg: dict, W, W16, ctx16=None):
-        """TransformerBlock with only_pure_attention=False and / or use_projection=True
-        (models/attention.py:289-303, 321-380):
-            xn = RMSNorm_0(x); px = project_in(xn)
+        """TransformerBlock (models/attention.py:289-303, 321-380); keys / values of Attention2 come from
+        `textcontext` (cross-attention, e.g. 77 x 768) or, when it is None, from px:
+            xn = RMSNorm_0(x); px = project_in(xn)               [use_projection, else px = xn]
             h = px + Attention1(norm1(px))                       [use_self_and_cross]
             h = h + Attention2(norm2(h), textcontext or px)
             h = h + net_2(GEGLU(net_0.proj(norm3(h))))
-            out = xn + project_out(h)
-        or, with only_pure_attention, out = xn + project_out(Attention2(project_in(xn), context))."""
+            out = xn + project_out(h)                            [use_projection, else out = xn + h]
+        or, with only_pure_attention, h = Attention2(px, textcontext or px).  Without projections the pure block's
+        output GEMM writes out = xn + Attention2(xn, ...) straight into the destination, xn as its residual."""
         x = xin.t
         Bn, hh, ww, C = x.shape
         L, M = hh * ww, Bn * hh * ww
@@ -680,17 +649,17 @@ class Unet:
         xn2 = xn.view(M, C)
         px = ops.linear_fwd(xn2, W16[f"{name}/project_in/kernel"]) if proj else xn2
         ctx = px.view(Bn, L, C) if ctx16 is None else ctx16
-        out2 = dst.t.view(M, C) if dst.t.is_contiguous() else None
-        sv = {"xn": xn, "px": px, "ctx_is_px": ctx16 is None, "ctx": ctx}
-        zeros = None
+        sv = {"xn": xn, "ctx_is_px": ctx16 is None}
 
         def rms(t2, pname):
             return ops.rmsnorm_fwd(t2.view(Bn, hh, ww, C), W[pname], ATTN_EPS).view(M, C)
 
         if pure:
-            zeros = torch.zeros((M, C), dtype=BF16, device=dev)
-            h = torch.empty((M, C), dtype=BF16, device=dev)
-            sv["a2"] = self._mha_fwd(f"{pre}/Attention2", px.view(Bn, L, C), ctx, heads, W16, zeros, h)
+            if proj:
+                res, h = torch.zeros((M, C), dtype=BF16, device=dev), torch.empty((M, C), dtype=BF16, device=dev)
+            else:       # a channel slot viewed as [M, C] has row stride = pixel stride
+                res, h = xn2, dst.t.view(M, C)
+            sv["a2"] = self._mha_fwd(f"{pre}/Attention2", px.view(Bn, L, C), ctx, heads, W16, res, h)
         else:
             h = px
             if both:
@@ -713,7 +682,7 @@ class Unet:
         if proj:
             ops.gemm(GEMM_KMN, h, W16[f"{name}/project_out/kernel"], dst.t, M, C, C, C, C, dst.t.stride(2),
                      res=xn, r_ld=C)
-        else:
+        elif not pure:
             ops.act_add(xn, h.view(Bn, hh, ww, C), dst.t)
         return ("tblock", name, xin, dst, acfg, sv)
 
@@ -721,75 +690,64 @@ class Unet:
         _, name, xin, dst, acfg, sv = rec
         x = xin.t
         Bn, hh, ww, C = x.shape
-        L, M = hh * ww, Bn * hh * ww
+        M = Bn * hh * ww
         pure = acfg.get("only_pure_attention", True)
         proj = acfg.get("use_projection", False)
         both = acfg.get("use_self_and_cross", True)
         pre = f"{name}/Attention"
-        dev = x.device
         dout = grad_of(dst)                                   # [B,h,w,C], possibly a slot view
-        dout2 = dout.reshape(M, C) if dout.is_contiguous() else dout.contiguous().view(M, C)
-        xn, px = sv["xn"], sv["px"]
-
-        def lin_wgrad(pname, src2, dy2):
-            kin, n = src2.shape[1], dy2.shape[1]
-            ops.gemm(GEMM_MNMN, src2, dy2, Gd[pname], kin, n, src2.shape[0], src2.stride(0), dy2.stride(0), n,
-                     atomic=True, reduce_batch=True)
-
-        def lin_dgrad(dy2, w_kn, out=None, res=None):
-            kin, n = w_kn.shape
-            out = out if out is not None else torch.empty((dy2.shape[0], kin), dtype=BF16, device=dev)
-            ops.gemm(GEMM_KK, dy2, w_kn, out, dy2.shape[0], kin, n, dy2.stride(0), n, kin,
-                     res=res, r_ld=(res.stride(0) if res is not None else 0))
-            return out
+        xn = sv["xn"]
+        kv2 = "split" if sv["ctx_is_px"] else None            # Attention2's d(context) is only needed when it is px
 
         def rms_bwd_into(x2, dy2, pname, dx2):
             """dx2 += d/dx RMSNorm(x2) given dy2 (accumulates in place)."""
             v4 = lambda t: t.view(Bn, hh, ww, C)
             ops.rmsnorm_bwd(v4(x2), v4(dy2), W[pname], ATTN_EPS, v4(dx2), Gd[pname], True)
 
-        # out = xn + project_out(h)
-        if proj:
-            lin_wgrad(f"{name}/project_out/kernel", sv["h_last"], dout2)
-            dh = lin_dgrad(dout2, W16[f"{name}/project_out/kernel"])
+        if pure and not proj:
+            # out = xn + Attention2(xn, ctx): d xn = dout (added in the dq GEMM's epilogue) + dq Wq^T
+            # (+ dk Wk^T + dv Wv^T for self-attention); dout is read in place as a row-strided [M, C] view
+            dout2 = dout.view(M, C)
+            dxn, _ = self._mha_bwd(sv["a2"], dout2, Gd, res=dout2, kv="fold" if sv["ctx_is_px"] else None)
         else:
-            dh = dout2.clone()
-        dctx_px = None
-        if pure:
-            dpx, dctx = self._mha_bwd(sv["a2"], dh, Gd)
-            if sv["ctx_is_px"]:
-                dctx_px = dctx
-        else:
-            # h3 = h2 + net_2(g)
-            g, u, n3, h2 = sv["g"], sv["u"], sv["n3"], sv["h2"]
-            lin_wgrad(f"{pre}/ff/net_2/kernel", g, dh)
-            ops.colsum_rows(dh, Gd[f"{pre}/ff/net_2/bias"])
-            dg = lin_dgrad(dh, W16[f"{pre}/ff/net_2/kernel"])
-            du = ops.geglu_bwd(u, dg)
-            lin_wgrad(f"{pre}/ff/net_0/proj/kernel", n3, du)
-            ops.colsum_rows(du, Gd[f"{pre}/ff/net_0/proj/bias"])
-            dn3 = lin_dgrad(du, W16[f"{pre}/ff/net_0/proj/kernel"])
-            rms_bwd_into(h2, dn3, f"{pre}/norm3/scale", dh)            # dh = d h2
-            # h2 = h1 + Attention2(norm2(h1), ctx)
-            dn2, dctx = self._mha_bwd(sv["a2"], dh, Gd)
-            if sv["ctx_is_px"]:
-                dctx_px = dctx
-            rms_bwd_into(sv["h1"], dn2, f"{pre}/norm2/scale", dh)      # dh = d h1
-            if both:
-                # h1 = h0 + Attention1(norm1(h0)) with keys / values from the same normed tensor
-                dn1, dkv1 = self._mha_bwd(sv["a1"], dh, Gd)
-                self._add2d(dn1, dkv1, dn1)
-                rms_bwd_into(sv["h0"], dn1, f"{pre}/norm1/scale", dh)  # dh = d h0 = d px
-            dpx = dh
-        if dctx_px is not None:                                        # context = px (textcontext is None)
-            self._add2d(dpx, dctx_px, dpx)
-        # px = project_in(xn);  d xn = dout (residual) + d px . W_in^T
-        dxn = torch.empty((M, C), dtype=BF16, device=dev)
-        if proj:
-            lin_wgrad(f"{name}/project_in/kernel", xn.view(M, C), dpx)
-            lin_dgrad(dpx, W16[f"{name}/project_in/kernel"], out=dxn, res=dout2)
-        else:
-            self._add2d(dpx, dout2, dxn)
+            dout2 = dout.reshape(M, C) if dout.is_contiguous() else dout.contiguous().view(M, C)
+            # out = xn + project_out(h)
+            if proj:
+                _dense_wgrad(Gd[f"{name}/project_out/kernel"], sv["h_last"], dout2)
+                dh = _dense_dgrad(dout2, W16[f"{name}/project_out/kernel"])
+            else:
+                dh = dout2.clone()
+            if pure:
+                dpx, dctx_px = self._mha_bwd(sv["a2"], dh, Gd, kv=kv2)
+            else:
+                # h3 = h2 + net_2(g)
+                g, u, n3, h2 = sv["g"], sv["u"], sv["n3"], sv["h2"]
+                _dense_wgrad(Gd[f"{pre}/ff/net_2/kernel"], g, dh)
+                ops.colsum_rows(dh, Gd[f"{pre}/ff/net_2/bias"])
+                dg = _dense_dgrad(dh, W16[f"{pre}/ff/net_2/kernel"])
+                du = ops.geglu_bwd(u, dg)
+                _dense_wgrad(Gd[f"{pre}/ff/net_0/proj/kernel"], n3, du)
+                ops.colsum_rows(du, Gd[f"{pre}/ff/net_0/proj/bias"])
+                dn3 = _dense_dgrad(du, W16[f"{pre}/ff/net_0/proj/kernel"])
+                rms_bwd_into(h2, dn3, f"{pre}/norm3/scale", dh)            # dh = d h2
+                # h2 = h1 + Attention2(norm2(h1), ctx)
+                dn2, dctx_px = self._mha_bwd(sv["a2"], dh, Gd, kv=kv2)
+                rms_bwd_into(sv["h1"], dn2, f"{pre}/norm2/scale", dh)      # dh = d h1
+                if both:
+                    # h1 = h0 + Attention1(norm1(h0)) with keys / values from the same normed tensor
+                    dn1, dkv1 = self._mha_bwd(sv["a1"], dh, Gd)
+                    self._add2d(dn1, dkv1, dn1)
+                    rms_bwd_into(sv["h0"], dn1, f"{pre}/norm1/scale", dh)  # dh = d h0 = d px
+                dpx = dh
+            if dctx_px is not None:                                        # context = px (textcontext is None)
+                self._add2d(dpx, dctx_px, dpx)
+            # px = project_in(xn);  d xn = dout (residual) + d px . W_in^T
+            dxn = torch.empty((M, C), dtype=BF16, device=x.device)
+            if proj:
+                _dense_wgrad(Gd[f"{name}/project_in/kernel"], xn.view(M, C), dpx)
+                _dense_dgrad(dpx, W16[f"{name}/project_in/kernel"], out=dxn, res=dout2)
+            else:
+                self._add2d(dpx, dout2, dxn)
         dx, acc = want(xin)
         ops.rmsnorm_bwd(x, dxn.view(Bn, hh, ww, C), W[f"{name}/RMSNorm_0/scale"], ATTN_EPS, dx,
                         Gd[f"{name}/RMSNorm_0/scale"], acc)
@@ -863,8 +821,6 @@ class Unet:
                 xin = rec[2]
                 if id(xin) in children:
                     mark_children_written(xin, children[id(xin)])
-            elif kind == "attn":
-                self._attn_bwd(rec, W, W16, Gd, want, grad_of)
             elif kind == "tblock":
                 self._tblock_bwd(rec, W, W16, Gd, want, grad_of)
             elif kind == "conv":
@@ -931,8 +887,7 @@ class Unet:
             ops.conv3x3_wgrad(a2, dout, Gd[f"{name}/conv2/conv/kernel"])
             ops.colsum(dout, False, out=Gd[f"{name}/conv2/conv/bias"])
             if cin != cout:      # the 1x1 residual conv sees the same dout
-                ops.gemm(GEMM_MNMN, x, dout, Gd[kres + "kernel"], cin, cout, M, x.stride(2), dout.stride(2), cout,
-                         atomic=True, reduce_batch=True)
+                _dense_wgrad(Gd[kres + "kernel"], x.view(M, cin), dout.view(M, cout))
                 Gd[kres + "bias"].copy_(Gd[f"{name}/conv2/conv/bias"])
         side.run(conv2_param_grads)
         # conv2 data gradient -> norm2 + silu backward (first pass fused into the dgrad epilogue).
@@ -949,8 +904,7 @@ class Unet:
             # timestep projection (its bias gradient = conv1's), then the conv1 weight gradient
             Gd[f"{name}/temb_projection/bias"].copy_(Gd[f"{name}/conv1/conv/bias"])
             drow16 = ops.cast_f32_bf16(drow)
-            ops.gemm(GEMM_MNMN, emb16, drow16, Gd[f"{name}/temb_projection/kernel"], E, cout, Bn, E, cout, cout,
-                     atomic=True, reduce_batch=True)
+            _dense_wgrad(Gd[f"{name}/temb_projection/kernel"], emb16, drow16)
             ops.gemm(GEMM_KK, drow16, W16[f"{name}/temb_projection/kernel"], demb, Bn, E, cout, cout, cout, E,
                      atomic=True)
             side.keep.append(drow16)
@@ -974,58 +928,3 @@ class Unet:
         else:
             ops.conv_dgrad_groupnorm_bwd(*gn1, False, addend=dout)
         del dh
-
-    def _attn_bwd(self, rec, W, W16, Gd, want, grad_of):
-        """Backward of _attn_fwd: projection GEMMs around fdx_attention_bwd (dQ / dK / dV with the logits
-        recomputed on chip from the saved log-sum-exp)."""
-        _, name, xin, dst, heads, xn, q, k, v, lse, o, ctx, (wq, wk, wv, wo), Lk = rec
-        x = xin.t
-        Bn, hh, ww, C = x.shape
-        L = hh * ww
-        d = C // heads
-        dp = _attn_width(d)
-        HD = heads * dp
-        cross = ctx is not None
-        kv_src = ctx if cross else xn.view(Bn, L, C)
-        Cc = kv_src.shape[2]
-        base = f"{name}/Attention/Attention2"
-        dout = grad_of(dst)
-        M = Bn * L
-        dev = x.device
-
-        def grad_target(pname, shape_p):
-            g = Gd[pname]
-            if dp == d:
-                return g.view(shape_p), None
-            return torch.zeros(shape_p, dtype=F32, device=dev), g
-
-        def finish(tmp, g, axis_view, sl):
-            if g is not None:
-                g.add_(tmp.view(axis_view)[sl])
-
-        o2 = o.view(M, HD)
-        t_o, g_o = grad_target(f"{base}/to_out_0/kernel", (HD, C))
-        ops.gemm(GEMM_MNMN, o2, dout, t_o, HD, C, M, HD, dout.stride(2), C, atomic=True, reduce_batch=True)
-        finish(t_o, g_o, (heads, dp, C), (slice(None), slice(0, d), slice(None)))
-        do = torch.empty((Bn, L, HD), dtype=BF16, device=dev)
-        ops.gemm(GEMM_KK, dout, wo, do, M, HD, C, dout.stride(2), C, HD)
-        dq, dk, dv = ops.attention_bwd(q, k, v, o, lse, do, heads, dp, d ** -0.5)
-        dq2, dk2, dv2 = dq.view(M, HD), dk.view(Bn * Lk, HD), dv.view(Bn * Lk, HD)
-        x2 = xn.view(M, C)
-        t_q, g_q = grad_target(f"{base}/to_q/kernel", (C, HD))
-        ops.gemm(GEMM_MNMN, x2, dq2, t_q, C, HD, M, C, HD, HD, atomic=True, reduce_batch=True)
-        finish(t_q, g_q, (C, heads, dp), (slice(None), slice(None), slice(0, d)))
-        src2 = kv_src.reshape(Bn * Lk, Cc)
-        for nm, dy_ in (("to_k", dk2), ("to_v", dv2)):
-            t_w, g_w = grad_target(f"{base}/{nm}/kernel", (Cc, HD))
-            ops.gemm(GEMM_MNMN, src2, dy_, t_w, Cc, HD, Bn * Lk, Cc, HD, HD, atomic=True, reduce_batch=True)
-            finish(t_w, g_w, (Cc, heads, dp), (slice(None), slice(None), slice(0, d)))
-        # d(xn) = dout (residual) + dq Wq^T (+ dk Wk^T + dv Wv^T for self-attention)
-        dxn = torch.empty((Bn, hh, ww, C), dtype=BF16, device=dev)
-        dxn2 = dxn.view(M, C)
-        ops.gemm(GEMM_KK, dq2, wq, dxn2, M, C, HD, HD, HD, C, res=dout, r_ld=dout.stride(2))
-        if not cross:
-            for dy_, w_ in ((dk2, wk), (dv2, wv)):
-                ops.gemm(GEMM_KK, dy_, w_, dxn2, M, C, HD, HD, HD, C, res=dxn2, r_ld=C)
-        dx, acc = want(xin)
-        ops.rmsnorm_bwd(x, dxn, W[f"{name}/RMSNorm_0/scale"], ATTN_EPS, dx, Gd[f"{name}/RMSNorm_0/scale"], acc)
