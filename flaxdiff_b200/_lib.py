@@ -83,6 +83,18 @@ class fdx_attn_desc(ctypes.Structure):
 
 GEMM_KK, GEMM_KMN, GEMM_MNMN = 0, 1, 2
 OPT_ADAM, OPT_LAMB = 0, 1
+ACT_QUICK_GELU, ACT_GELU = 0, 1          # fdx_bias_act
+
+
+def _declare(lib) -> None:
+    """Argument types of the entry points whose integer arguments are wider than C int or are pointers passed
+    as Python ints (ctypes would otherwise truncate them)."""
+    vp, i, ll, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
+    lib.fdx_attention_fwd_masked.argtypes = [ctypes.POINTER(fdx_attn_desc), i, vp, vp]
+    lib.fdx_token_embed.argtypes = [vp, i, i, vp, i, vp, i, vp, vp]
+    lib.fdx_layernorm_fwd.argtypes = [vp, ll, i, vp, vp, f, vp, vp]
+    lib.fdx_bias_act.argtypes = [vp, ll, i, vp, i, vp, vp]
+
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -102,6 +114,7 @@ def load() -> ctypes.CDLL:
             "or `make -C flaxdiff_b200/csrc`. flaxdiff_b200 has no CPU fallback.")
     lib = ctypes.CDLL(_LIB_PATH)
     lib.fdx_last_error.restype = ctypes.c_char_p
+    _declare(lib)
     if os.environ.get("FDX_TRACE"):
         lib = _TracingLib(lib)
     _lib = lib

@@ -49,6 +49,9 @@ struct AttnDev {
   __nv_bfloat16* dq; long long dq_ld, dq_bs;
   __nv_bfloat16* dk; long long dk_ld, dk_bs;
   __nv_bfloat16* dv; long long dv_ld, dv_bs;
+  // masked forward (fdx_attention_fwd_masked)
+  const int32_t* key_mask;  // [B][Lk] 0 / 1, or NULL
+  int causal;
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -72,13 +75,30 @@ __device__ __forceinline__ void store_p_chunk(uint32_t sP, int r, int c0, const 
                  : "memory");
 }
 
+// bit i set: query `qrow` may attend key key0 + i (inside the tensor, key_mask[b][key] set, and key <= qrow when
+// causal).  One coalesced key-mask load per lane, then a ballot: every lane of the warp gets the whole word.
+__device__ __forceinline__ uint32_t allowed_bits(const AttnDev& p, int b, int key0, int qrow, int lane) {
+  const int key = key0 + lane;
+  bool ok = key < p.Lk;
+  if (ok && p.key_mask) ok = p.key_mask[(long long)b * p.Lk + key] != 0;
+  uint32_t w = __ballot_sync(0xffffffffu, ok);
+  if (p.causal) {
+    const int lim = qrow - key0;                   // highest allowed bit
+    w &= lim >= 31 ? 0xffffffffu : (lim < 0 ? 0u : (2u << lim) - 1u);
+  }
+  return w;
+}
+
 // ======================================================================================================
 // forward
 // ======================================================================================================
 // SHORT = the keys fit one 128-key block (77 text tokens): a single K/V stage.  Otherwise a ring of NKV stages
 // keeps the next key blocks in flight while the warpgroup works through the serial chain
 // S_j -> softmax_j -> PV_j.
-template <int DH, bool SHORT>
+// MASKED = fdx_attention_fwd_masked: the bounds test on the last key block becomes the per-row allowed-key word of
+// allowed_bits on every block; a row with no allowed key so far keeps m = -inf with corr = 1 and ends with l = 0,
+// which writes zeros.
+template <int DH, bool SHORT, bool MASKED = false>
 __global__ void __launch_bounds__(kThreads, 1)
 fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                     const __grid_constant__ CUtensorMap mapV, const AttnDev p) {
@@ -97,7 +117,10 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int q0 = qt * 128;
-  const int nblk = (p.Lk + 127) / 128;
+  int nblk = (p.Lk + 127) / 128;
+  if constexpr (MASKED) {
+    if (p.causal && nblk > qt + 1) nblk = qt + 1;           // later key blocks lie wholly after the tile's queries
+  }
   const int c0 = (head * DH) / 64 * 64;                     // first channel of the 64-wide TMA box
   const uint32_t koff = (uint32_t)((head * DH) % 64) * 2;   // byte offset of this head inside the swizzle row
 
@@ -153,7 +176,12 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
       for (int c = 0; c < 128; c += 32) {
         float v[32];
         S.row32(xs, 1, c, v);
-        if (partial) {
+        if constexpr (MASKED) {
+          const uint32_t ok = allowed_bits(p, b, kbase + c, q0 + row, lane);
+#pragma unroll
+          for (int i = 0; i < 32; ++i)
+            if ((ok >> i) & 1u) mx = fmaxf(mx, v[i]);
+        } else if (partial) {
 #pragma unroll
           for (int i = 0; i < 32; ++i)
             if (kbase + c + i < p.Lk) mx = fmaxf(mx, v[i]);
@@ -168,7 +196,10 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
         }
       }
       const float m_new = fmaxf(m, mx * p.scale_log2);
-      const float corr = ex2(m - m_new);           // first block: exp2(-inf) = 0
+      float corr = ex2(m - m_new);                 // first block: exp2(-inf) = 0
+      if constexpr (MASKED) {
+        if (m_new == -INFINITY) corr = 1.f;        // no allowed key yet: acc and l stay 0
+      }
       // pass B: probabilities -> bf16 -> the swizzled A tile of the PV MMA
       float rs = 0.f;
 #pragma unroll 1
@@ -176,6 +207,8 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
         float v[32];
         uint32_t w[16];
         S.row32(xs, 1, c, v);
+        uint32_t ok = 0;
+        if constexpr (MASKED) ok = allowed_bits(p, b, kbase + c, q0 + row, lane);
         float rs4[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {
@@ -183,7 +216,11 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             pe[u] = ex2(fmaf(v[i + u], p.scale_log2, -m_new));
-            if (partial && !(kbase + c + i + u < p.Lk)) pe[u] = 0.f;
+            if constexpr (MASKED) {
+              if (!((ok >> (i + u)) & 1u)) pe[u] = 0.f;
+            } else if (partial && !(kbase + c + i + u < p.Lk)) {
+              pe[u] = 0.f;
+            }
             rs4[u] += pe[u];
           }
           w[i >> 1] = pack_bf16x2(pe[0], pe[1]);
@@ -217,7 +254,10 @@ fdx_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_const
       }
     }
     if (q0 + row < p.L) {
-      const float inv = 1.f / l;
+      float inv = 1.f / l;
+      if constexpr (MASKED) {
+        if (l == 0.f) inv = 0.f;                   // no allowed key: zeros
+      }
       __nv_bfloat16* op = p.o + (long long)b * p.o_bs + (long long)(q0 + row) * p.o_ld + head * DH;
 #pragma unroll
       for (int c = 0; c < DH; c += 8) {
@@ -878,25 +918,34 @@ int check_io(const void* ptr, long long ld, long long bs, const char* name, cons
   return FDX_OK;
 }
 
+// argument checks, TMA maps and kernel parameters of both forward entry points
+int fwd_prepare(const fdx_attn_desc* a, const char* who, CUtensorMap* mQ, CUtensorMap* mK, CUtensorMap* mV,
+                AttnDev* d) {
+  int s = check_desc(a, who);
+  if (s != FDX_OK) return s;
+  FDX_REQUIRE(a->o, "%s: null output", who);
+  if ((s = check_io(a->o, a->o_ld, a->o_bs, "o", "o_ld", "o_bs", who)) != FDX_OK) return s;
+  const int hd = a->heads * a->dh;
+  if ((s = make_map(mQ, a->q, hd, a->L, a->B, a->q_ld, a->q_bs)) != FDX_OK) return s;
+  if ((s = make_map(mK, a->k, hd, a->Lk, a->B, a->k_ld, a->k_bs)) != FDX_OK) return s;
+  if ((s = make_map(mV, a->v, hd, a->Lk, a->B, a->v_ld, a->v_bs)) != FDX_OK) return s;
+  *d = AttnDev{};
+  d->B = a->B; d->heads = a->heads; d->L = a->L; d->Lk = a->Lk; d->dh = a->dh;
+  d->scale = a->scale; d->scale_log2 = a->scale * kLog2e;
+  d->o = (__nv_bfloat16*)a->o; d->o_ld = a->o_ld; d->o_bs = a->o_bs;
+  d->lse = a->lse;
+  return FDX_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
 int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
-  int s = check_desc(a, "attention_fwd");
-  if (s != FDX_OK) return s;
-  FDX_REQUIRE(a->o, "attention_fwd: null output");
-  if ((s = check_io(a->o, a->o_ld, a->o_bs, "o", "o_ld", "o_bs", "attention_fwd")) != FDX_OK) return s;
-  const int hd = a->heads * a->dh;
   CUtensorMap mQ, mK, mV;
-  if ((s = make_map(&mQ, a->q, hd, a->L, a->B, a->q_ld, a->q_bs)) != FDX_OK) return s;
-  if ((s = make_map(&mK, a->k, hd, a->Lk, a->B, a->k_ld, a->k_bs)) != FDX_OK) return s;
-  if ((s = make_map(&mV, a->v, hd, a->Lk, a->B, a->v_ld, a->v_bs)) != FDX_OK) return s;
-  AttnDev d{};
-  d.B = a->B; d.heads = a->heads; d.L = a->L; d.Lk = a->Lk; d.dh = a->dh;
-  d.scale = a->scale; d.scale_log2 = a->scale * kLog2e;
-  d.o = (__nv_bfloat16*)a->o; d.o_ld = a->o_ld; d.o_bs = a->o_bs;
-  d.lse = a->lse;
+  AttnDev d;
+  int s = fwd_prepare(a, "attention_fwd", &mQ, &mK, &mV, &d);
+  if (s != FDX_OK) return s;
   const bool short_keys = a->Lk <= 128;
   if (a->dh == 128) {
     const int smem128 = (2 + 2 * (short_keys ? 1 : 2)) * kWTile + 1024 + 64;
@@ -941,6 +990,43 @@ int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
     else FDX_ATTN_FWD_LAUNCH(32, false, 3)
   }
 #undef FDX_ATTN_FWD_LAUNCH
+  fdx_note_kernel(FDX_KERNEL_ATTN_FWD);
+  FDX_LAUNCH_CHECK();
+  return FDX_OK;
+}
+
+int fdx_attention_fwd_masked(const fdx_attn_desc* a, int causal, const int32_t* key_mask, void* stream) {
+  if (a && a->dh == 128) {
+    fdx_set_error("attention_fwd_masked: head width 128 is not supported (32 or 64)");
+    return FDX_ERR_UNSUPPORTED;
+  }
+  CUtensorMap mQ, mK, mV;
+  AttnDev d;
+  int s = fwd_prepare(a, "attention_fwd_masked", &mQ, &mK, &mV, &d);
+  if (s != FDX_OK) return s;
+  d.key_mask = key_mask;
+  d.causal = causal ? 1 : 0;
+  const bool short_keys = a->Lk <= 128;
+  const int smem = (1 + 2 * (short_keys ? 1 : kKV) + 2) * kTile + kAccXchgBytes + 1024 + 256;
+  dim3 grid((a->L + 127) / 128, a->heads, a->B);
+  static bool attr[4] = {false, false, false, false};
+#define FDX_ATTN_FWD_MASKED_LAUNCH(DHV, SH, IDX)                                                                  \
+  {                                                                                                               \
+    if (!attr[IDX]) {                                                                                             \
+      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_fwd_kernel<DHV, SH, true>,                                           \
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize, smem));                          \
+      attr[IDX] = true;                                                                                           \
+    }                                                                                                             \
+    fdx_attn_fwd_kernel<DHV, SH, true><<<grid, kThreads, smem, (cudaStream_t)stream>>>(mQ, mK, mV, d);            \
+  }
+  if (a->dh == 64) {
+    if (short_keys) FDX_ATTN_FWD_MASKED_LAUNCH(64, true, 0)
+    else FDX_ATTN_FWD_MASKED_LAUNCH(64, false, 1)
+  } else {
+    if (short_keys) FDX_ATTN_FWD_MASKED_LAUNCH(32, true, 2)
+    else FDX_ATTN_FWD_MASKED_LAUNCH(32, false, 3)
+  }
+#undef FDX_ATTN_FWD_MASKED_LAUNCH
   fdx_note_kernel(FDX_KERNEL_ATTN_FWD);
   FDX_LAUNCH_CHECK();
   return FDX_OK;

@@ -66,24 +66,31 @@ class CLIPTextEncoder(ConditioningEncoder):
     `transformers` (SURVEY $8 f3): tokenizer(padding="max_length", max_length=model_max_length, truncation=True)
     -> CLIPTextModel -> last_hidden_state (B, 77, 768), frozen, evaluated under no_grad.  The text tower is
     conditioning PRE-processing, not the hot path: it runs as stock PyTorch modules; its output feeds the UNet's
-    cross-attention as a bf16 CUDA tensor.  `model` / `tokenizer` may be injected (tests, custom towers);
-    `from_modelname` needs the weights in the local Hugging Face cache (there is no network here)."""
+    cross-attention as a bf16 CUDA tensor.  backend="fdx" runs the same weights as the engine's text tower
+    (models/clip_text.py), which the trainer then evaluates inside its training step.  `model` / `tokenizer` may be
+    injected (tests, custom towers); `from_modelname` needs the weights in the local Hugging Face cache."""
     key = "text"
 
     def __init__(self, model, tokenizer, modelname: str = "openai/clip-vit-large-patch14", backend: str = "torch",
                  device=None, dtype: torch.dtype = torch.bfloat16):
         self.model, self.tokenizer, self.modelname, self.backend = model, tokenizer, modelname, backend
         self.device, self.dtype = device, dtype
+        self.tower = None
         if hasattr(model, "eval"):
             model.eval()
-        if device is not None and hasattr(model, "to"):
+        if backend == "fdx":
+            # the engine's tower: the weights are packed onto the GPU once, the transformers model stays on the host
+            from ..models.clip_text import CLIPTextTower
+            self.tower = CLIPTextTower.from_transformers(model, device, seq_len=tokenizer.model_max_length)
+        elif device is not None and hasattr(model, "to"):
             model.to(device)
 
     @staticmethod
     def from_modelname(modelname: str = "openai/clip-vit-large-patch14", backend: str = "torch", device=None):
         from .._lib import FdxError
-        if backend not in ("torch", "pt"):
-            raise FdxError(f"CLIPTextEncoder backend {backend!r}: only the torch backend exists here (JAX is not installed)")
+        if backend not in ("torch", "pt", "fdx"):
+            raise FdxError(f"CLIPTextEncoder backend {backend!r}: only the torch backend and the engine's 'fdx' "
+                           "tower exist here (JAX is not installed)")
         try:
             from transformers import AutoTokenizer, CLIPTextModel
             model = CLIPTextModel.from_pretrained(modelname, local_files_only=True)
@@ -91,7 +98,7 @@ class CLIPTextEncoder(ConditioningEncoder):
         except Exception as e:  # noqa: BLE001
             raise FdxError(f"CLIPTextEncoder: cannot load {modelname!r} from the local Hugging Face cache "
                            f"({type(e).__name__}); pass model= / tokenizer= or use RandomEmbeddingEncoder") from e
-        return CLIPTextEncoder(model, tokenizer, modelname, "torch", device)
+        return CLIPTextEncoder(model, tokenizer, modelname, "fdx" if backend == "fdx" else "torch", device)
 
     def tokenize(self, data):
         return self.tokenizer(list(data), padding="max_length", max_length=self.tokenizer.model_max_length,
@@ -99,6 +106,8 @@ class CLIPTextEncoder(ConditioningEncoder):
 
     def encode_from_tokens(self, tokens) -> torch.Tensor:
         ids, mask = tokens["input_ids"], tokens["attention_mask"]
+        if self.tower is not None:
+            return self.tower.encode(ids, mask)         # bf16 on the GPU
         if self.device is not None:
             ids, mask = ids.to(self.device), mask.to(self.device)
         with torch.no_grad():

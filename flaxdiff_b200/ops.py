@@ -778,6 +778,58 @@ def attention_bwd(q, k, v, o, lse, d_o, heads: int, dh: int, scale: float):
     return dq, dk, dv
 
 
+def attention_fwd_masked(q, k, v, heads: int, dh: int, scale: float, causal: bool,
+                         key_mask: Optional[torch.Tensor] = None, out=None) -> torch.Tensor:
+    """fdx_attention_fwd_masked: key j is allowed for query i iff (not causal or j <= i) and key_mask[b][j];
+    key_mask int32 [B, Lk] or None.  A row with no allowed key is zeros.  -> o bf16 [B, L, heads*dh]."""
+    B, L, HD = q.shape
+    if key_mask is not None:
+        assert key_mask.dtype == torch.int32 and key_mask.is_contiguous() and key_mask.shape == (B, k.shape[1])
+    o = out if out is not None else torch.empty((B, L, HD), dtype=torch.bfloat16, device=q.device)
+    a = _attn_desc(q, k, v, o, None, heads, dh, scale)
+    check(load().fdx_attention_fwd_masked(ctypes.byref(a), 1 if causal else 0, ptr(key_mask), stream_ptr()),
+          "attention_fwd_masked")
+    return o
+
+
+# --------------------------------------------------------------------------- CLIP text tower
+def token_embed(ids: torch.Tensor, tok: torch.Tensor, pos: torch.Tensor, out=None) -> torch.Tensor:
+    """bf16(tok[ids] + pos[t]) -> [B, T, D]; ids int32 [B, T]; an id outside [0, vocab) gives a NaN row."""
+    B, T = ids.shape
+    vocab, D = tok.shape
+    assert ids.dtype == torch.int32 and ids.is_contiguous() and tok.dtype == pos.dtype == torch.float32
+    assert tok.is_contiguous() and pos.is_contiguous() and pos.shape[1] == D and pos.shape[0] >= T
+    if out is None:
+        out = torch.empty((B, T, D), dtype=torch.bfloat16, device=ids.device)
+    assert out.is_contiguous() and out.shape == (B, T, D)
+    check(load().fdx_token_embed(ptr(ids), B, T, ptr(tok), vocab, ptr(pos), D, ptr(out), stream_ptr()),
+          "token_embed")
+    return out
+
+
+def layernorm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, out=None) -> torch.Tensor:
+    """nn.LayerNorm over the last axis of a contiguous bf16 tensor; gamma / beta f32."""
+    C = x.shape[-1]
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and gamma.dtype == beta.dtype == torch.float32
+    if out is None:
+        out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
+    assert out.is_contiguous() and out.shape == x.shape
+    check(load().fdx_layernorm_fwd(ptr(x), x.numel() // C, C, ptr(gamma), ptr(beta), eps, ptr(out), stream_ptr()),
+          "layernorm_fwd")
+    return out
+
+
+def bias_act(x: torch.Tensor, bias: Optional[torch.Tensor], act_kind: int, out=None) -> torch.Tensor:
+    """act(x + bias) over the last axis (_lib.ACT_QUICK_GELU / ACT_GELU); out may be x."""
+    C = x.shape[-1]
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and (bias is None or bias.dtype == torch.float32)
+    if out is None:
+        out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
+    assert out.is_contiguous() and out.shape == x.shape
+    check(load().fdx_bias_act(ptr(x), x.numel() // C, C, ptr(bias), act_kind, ptr(out), stream_ptr()), "bias_act")
+    return out
+
+
 # --------------------------------------------------------------------------- temb / softmax
 def time_embed_fwd(t, freqs, W1, b1, W2, b2):
     B, D = t.shape[0], W1.shape[0]

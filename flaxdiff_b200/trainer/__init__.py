@@ -463,6 +463,8 @@ class GeneralDiffusionTrainer:
         self.latest_step = 0
         self._graph = None
         self._static = None
+        self._null_tokens = None
+        self._step_ctx = None
         self._dyn = torch.zeros(3, dtype=torch.float32, device=self.device)
         # gradient buffer = the parameter layout + a 64-float tail; tail[0] carries the loss through the
         # exchange (general_diffusion_trainer.py:334 pmean(loss))
@@ -509,9 +511,40 @@ class GeneralDiffusionTrainer:
         return state, best
 
     # ------------------------------------------------------------------ the step
-    def _fwd_bwd(self, images, noise, noise_level, ctx=None):
-        """noise-add -> UNet fwd -> loss -> UNet bwd [-> bucketed gradient exchange]; returns the loss tensor
-        (f32[1]); gradients land in self._grads."""
+    def _text_tower(self):
+        """The engine's CLIP text tower when the first condition encodes with CLIPTextEncoder(backend="fdx"), else
+        None: the step then carries the tokens and encodes them itself."""
+        conds = self.input_config.conditions
+        return getattr(conds[0].encoder, "tower", None) if conds else None
+
+    def _device_tokens(self, batch):
+        """-> (ids, attention_mask) int32 [B, T] on the device; the tokenizer runs on the host."""
+        cond = self.input_config.conditions[0]
+        data = batch[cond.conditioning_data_key or cond.encoder.key]
+        return self._to_device_tokens(data if cond.pretokenized else cond.encoder.tokenize(data))
+
+    def _to_device_tokens(self, tokens):
+        return tuple(torch.as_tensor(tokens[k]).to(self.device, torch.int32, non_blocking=True).contiguous()
+                     for k in ("input_ids", "attention_mask"))
+
+    def _encode_tokens(self, ids, amask, umask):
+        """Null mixing + the text tower inside the step: the masked samples get the null prompt's tokens before the
+        tower.  Every kernel of the tower computes each sequence on its own, so this equals substituting
+        get_unconditional() into their embeddings, and no (B, T, D) tensor is touched outside the tower."""
+        if self._null_tokens is None:                   # the prompt get_unconditional() encodes
+            cond = self.input_config.conditions[0]
+            null = cond.unconditional_input if cond.unconditional_input is not None else ""
+            self._null_tokens = self._to_device_tokens(cond.encoder.tokenize([null]))
+        null_ids, null_mask = self._null_tokens
+        sel = umask.view(-1, 1)
+        return self._text_tower().encode(torch.where(sel, null_ids, ids), torch.where(sel, null_mask, amask))
+
+    def _fwd_bwd(self, images, noise, noise_level, ctx=None, tokens=None):
+        """[text tower ->] noise-add -> UNet fwd -> loss -> UNet bwd [-> bucketed gradient exchange]; returns the
+        loss tensor (f32[1]); gradients land in self._grads.  tokens = (ids, attention_mask, unconditional mask)
+        for an fdx text encoder; the context it produced stays in self._step_ctx."""
+        if tokens is not None:
+            ctx = self._step_ctx = self._encode_tokens(*tokens)
         sched, tr, st = self.noise_schedule, self.model_output_transform, self.state
         B = images.shape[0]
         rates = sched.get_rates(noise_level, shape=(-1,))
@@ -555,13 +588,16 @@ class GeneralDiffusionTrainer:
             images = data.to(dev, non_blocking=True).contiguous()      # HOST -> DEVICE boundary
             B = images.shape[0]
             local, uncond_key = local.get_random_key()
-            ctx = None
+            ctx = tokens = None
             if self.input_config.conditions:
                 # per-sample unconditional mask (bernoulli p = unconditional_prob) and null-embedding mixing
                 # (general_diffusion_trainer.py:266-275; inputs/__init__.py:123-146)
                 mask = utils.device_bernoulli(uncond_key, self.unconditional_prob, (B,), dev)
-                ctx = self.input_config.process_conditioning(batch, uncond_mask=mask)[0]
-                ctx = ctx.to(device=dev, dtype=torch.float32).contiguous()
+                if self._text_tower() is not None:
+                    tokens = self._device_tokens(batch) + (mask,)      # encoded and mixed inside the step
+                else:
+                    ctx = self.input_config.process_conditioning(batch, uncond_mask=mask)[0]
+                    ctx = ctx.to(device=dev, dtype=torch.float32).contiguous()
             noise_level, local = self.noise_schedule.generate_timesteps(B, local)
             local, noise_key = local.get_random_key()
             noise = utils.device_normal(noise_key, tuple(images.shape), dev)
@@ -569,9 +605,9 @@ class GeneralDiffusionTrainer:
                 self.state = train_state               # the step reads parameters through self.state
                 self._graph = None
             if self.use_cuda_graph:
-                loss = self._graphed_fwd_bwd(images, noise, noise_level, ctx)
+                loss = self._graphed_fwd_bwd(images, noise, noise_level, ctx, tokens)
             else:
-                loss = self._fwd_bwd(images, noise, noise_level, ctx)
+                loss = self._fwd_bwd(images, noise, noise_level, ctx, tokens)
                 if self._overlap:
                     loss = loss.clone()             # a view of the exchange buffer's tail otherwise
             gscale = 1.0
@@ -588,11 +624,11 @@ class GeneralDiffusionTrainer:
 
         return train_step
 
-    def _graphed_fwd_bwd(self, images, noise, noise_level, ctx=None):
+    def _graphed_fwd_bwd(self, images, noise, noise_level, ctx=None, tokens=None):
         if self._graph is None or self._static[0].shape != images.shape or self._static[0].dtype != images.dtype:
-            self._static = [images.clone(), noise.clone(), noise_level.clone()]
-            if ctx is not None:
-                self._static.append(ctx.clone())
+            self._static = [images.clone(), noise.clone(), noise_level.clone(),
+                            None if ctx is None else ctx.clone(),
+                            None if tokens is None else tuple(t.clone() for t in tokens)]
             self.state.params.shadow()              # bf16 weights current before warm-up and capture
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
@@ -610,6 +646,9 @@ class GeneralDiffusionTrainer:
         self._static[2].copy_(noise_level)
         if ctx is not None:
             self._static[3].copy_(ctx)
+        if tokens is not None:
+            for dst, src in zip(self._static[4], tokens):
+                dst.copy_(src)
         if not self.state.params.shadow_is_fresh():
             self.state.params.shadow()              # parameters changed outside the fused optimiser (load, ...)
         self._graph.replay()

@@ -361,6 +361,27 @@ typedef struct fdx_attn_desc {
 } fdx_attn_desc;
 int fdx_attention_fwd(const fdx_attn_desc* a, void* stream);
 int fdx_attention_bwd(const fdx_attn_desc* a, void* stream);
+/* Forward with a key mask, as CLIPTextTransformer's self-attention (transformers' create_causal_mask over
+ * `attention_mask`): key j is allowed for query i iff (!causal || j <= i) && key_mask[b][j] != 0.  key_mask is
+ * int32 [B][Lk] of 0 / 1, or NULL (every key allowed).  A query row with no allowed key writes zeros (and
+ * lse = -inf); the CLIP tokenizer never produces one.  dh 32 or 64; dh 128 gives FDX_ERR_UNSUPPORTED. */
+int fdx_attention_fwd_masked(const fdx_attn_desc* a, int causal, const int32_t* key_mask, void* stream);
+
+/* ---- CLIP text tower (fdx_clip.cu): FlaxCLIPTextModel of the text-conditioned trainer ------------------------
+ * (flaxdiff/inputs/encoders.py, trainer/general_diffusion_trainer.py:266-275).  Rows are contiguous bf16.
+ *   fdx_token_embed   : out[b][t][:] = bf16(tok[ids[b][t]] + pos[t]); ids int32 [B][T], tok f32 [vocab][D],
+ *                       pos f32 [>= T][D]; an id outside [0, vocab) gives a NaN row (jnp.take's fill mode) and
+ *                       reads nothing.  D a multiple of 8.
+ *   fdx_layernorm_fwd : nn.LayerNorm(eps): y = (x - mean) / sqrt(var + eps) * gamma + beta, f32 statistics from
+ *                       a two-pass mean / variance.  C a multiple of 8, <= 1280.
+ *   fdx_bias_act      : y = act(x + bias) (bias f32 [C] or NULL; x == y allowed).  C a multiple of 8. */
+#define FDX_ACT_QUICK_GELU 0 /* z * sigmoid(1.702 z) */
+#define FDX_ACT_GELU 1       /* exact erf gelu */
+int fdx_token_embed(const int32_t* ids, int B, int T, const float* tok, int vocab, const float* pos, int D,
+                    void* out_bf16, void* stream);
+int fdx_layernorm_fwd(const void* x_bf16, long long rows, int C, const float* gamma, const float* beta, float eps,
+                      void* y_bf16, void* stream);
+int fdx_bias_act(const void* x_bf16, long long rows, int C, const float* bias, int act, void* y_bf16, void* stream);
 
 #ifdef __cplusplus
 }
