@@ -168,7 +168,13 @@ int fdx_conv3x3_dgrad(const fdx_act* dy, const void* w_hwio, const fdx_act* dx, 
 
 int fdx_conv3x3_dgrad_gn(const fdx_act* dy, const void* w_hwio, const fdx_act* dz, const fdx_act* x,
                          const float* ab, float* ws_slots, int slots, void* stream) {
+  return fdx_conv3x3_dgrad_gn_act(dy, w_hwio, dz, x, ab, ws_slots, slots, 1, stream);
+}
+
+int fdx_conv3x3_dgrad_gn_act(const fdx_act* dy, const void* w_hwio, const fdx_act* dz, const fdx_act* x,
+                             const float* ab, float* ws_slots, int slots, int act, void* stream) {
   int s;
+  FDX_REQUIRE(act == 1 || act == 2, "conv3x3_dgrad_gn: act=%d (1 = silu, 2 = mish)", act);
   if ((s = check_act(dy, "conv3x3_dgrad_gn dy")) != FDX_OK) return s;
   if ((s = check_act(dz, "conv3x3_dgrad_gn dz")) != FDX_OK) return s;
   if ((s = check_act(x, "conv3x3_dgrad_gn x")) != FDX_OK) return s;
@@ -210,7 +216,14 @@ int fdx_conv3x3_dgrad_gn(const fdx_act* dy, const void* w_hwio, const fdx_act* d
   L.gn_ab = ab;
   L.gn_ws = ws_slots;
   L.gn_slots = slots;
-  return fdx_tc_launch(L, (cudaStream_t)stream);
+  if (act == 1) return fdx_tc_launch(L, (cudaStream_t)stream);
+  // mish: the transposed engine's epilogue only (the pixels-as-M engine has no mish variant)
+  L.gn_mish = 1;
+  s = fdx_tct_launch(L, (cudaStream_t)stream);
+  if (s == FDX_ERR_UNSUPPORTED)
+    fdx_set_error("conv3x3_dgrad_gn: mish is fused on the transposed engine only (Cin = 64 .. 512 not a multiple "
+                  "of 256, images 16-aligned); use fdx_conv3x3_dgrad + fdx_groupnorm_bwd with act = 2");
+  return s;
 }
 
 int fdx_conv3x3_wgrad(const fdx_act* x, const fdx_act* dy, float* dw_hwio, int stride,

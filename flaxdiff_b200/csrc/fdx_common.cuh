@@ -403,6 +403,25 @@ __device__ __forceinline__ float sigmoid_fast(float z) {
 }
 __device__ __forceinline__ float silu_f(float z) { return z * sigmoid_fast(z); }
 
+// mish(z) = z * tanh(softplus(z)) (jax.nn.mish).  With w = e^z and n = w (w + 2): tanh(softplus(z)) = t = n / (n + 2),
+// so one ex2 and one rcp (MUFU).  e^z takes min(z, 20): w^2 would overflow from z ~ 44, and from z = 20 on t rounds
+// to 1 in f32 anyway.  For z below ~ -87 w flushes to 0 and mish(z) = z * 0 = -0.
+__device__ __forceinline__ float mish_f(float z) {
+  const float w = __expf(fminf(z, 20.f));
+  const float n = w * (w + 2.f);
+  return z * __fdividef(n, n + 2.f);
+}
+// mish'(z) = t + z sigmoid(z) (1 - t^2).  With r = 1 / (n + 2): t = n r and sigmoid(z) (1 - t^2) = 4 w (w + 1) r^2, so
+// mish'(z) = r (n + 4 z w (w + 1) r), free of the cancellation in 1 - t^2.  The clamped z is used throughout: at
+// z >= 20 the second term is < 1e-15 and mish' = 1.
+__device__ __forceinline__ float mish_grad(float z) {
+  const float zc = fminf(z, 20.f);
+  const float w = __expf(zc);
+  const float n = w * (w + 2.f);
+  const float r = __fdividef(1.f, n + 2.f);
+  return r * fmaf(4.f * zc * fmaf(w, w, w), r, n);
+}
+
 // ---- f32 pairs ---------------------------------------------------------------------------------------
 // The streaming GroupNorm kernels work on channel pairs; sm_90 has no packed f32x2 instructions, so each
 // pair operation is two scalar f32 operations.

@@ -1,4 +1,4 @@
-// fdx_norm.cu -- GroupNorm(+SiLU) and RMSNorm, forward and backward, NHWC bf16.
+// fdx_norm.cu -- GroupNorm(+SiLU or mish) and RMSNorm, forward and backward, NHWC bf16.
 //
 // Replaces the XLA lowering of
 //   nn.GroupNorm(8, eps) + swish      flaxdiff/models/common.py:273-281,286-288,310-312
@@ -74,8 +74,12 @@ gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int 
   }
 }
 
-// y = silu?(a x + b) per channel pair: h = x*(a/2) + b/2, silu(z) = h*(1 + tanh(h))
-template <bool SILU>
+// Activation codes (the C ABI's `act`).  The kernels take it as a template argument, so an instantiation carries
+// only its own activation's arithmetic.
+enum { GN_NONE = 0, GN_SILU = 1, GN_MISH = 2 };
+
+// y = act(a x + b) per channel pair.  SiLU: h = x*(a/2) + b/2, silu(z) = h*(1 + tanh(h)); none and mish: h = z.
+template <int ACT>
 __global__ void __launch_bounds__(kNT)
 gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int C, int G,
                 const float* __restrict__ stats, const float* __restrict__ gamma,
@@ -119,7 +123,7 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int 
   const float mean = sum0 / cnt;
   const float var = fmaxf(0.f, sum1 / cnt - mean * mean);
   const float rstd = rsqrtf(var + eps);
-  const float sc = SILU ? 0.5f : 1.f;
+  const float sc = ACT == GN_SILU ? 0.5f : 1.f;
   f32x2_t a[4], b[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -147,7 +151,9 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int 
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const f32x2_t h = f2_fma(f2_from_bf16x2(w[j]), a[j], b[j]);
-          o[j] = f2_to_bf16x2(SILU ? f2_fma(h, f2_tanh(h), h) : h);
+          o[j] = f2_to_bf16x2(ACT == GN_SILU   ? f2_fma(h, f2_tanh(h), h)
+                              : ACT == GN_MISH ? f2_pack(mish_f(h.x), mish_f(h.y))
+                                               : h);
         }
         *reinterpret_cast<uint4*>(yb + (long long)p * yps) = make_uint4(o[0], o[1], o[2], o[3]);
       }
@@ -155,8 +161,8 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int 
   }
 }
 
-// ---- GroupNorm(+SiLU) backward ---------------------------------------------------------------
-// With a_c = rstd*gamma_c, b_c = beta_c - mean*a_c:  z = a_c*x + b_c,  dz = dy * silu'(z).
+// ---- GroupNorm(+activation) backward -----------------------------------------------------------
+// With a_c = rstd*gamma_c, b_c = beta_c - mean*a_c:  z = a_c*x + b_c,  dz = dy * act'(z).
 // Pass 1 needs only two per-(image, channel) sums, S0 = sum dz and S1 = sum dz*x, because
 //   dbeta_c  = sum_n S0                       dgamma_c = sum_n rstd*(S1 - mean*S0)
 //   red[n][g] = ( sum_{c in g} gamma_c*S0 ,   sum_{c in g} gamma_c*rstd*(S1 - mean*S0) )
@@ -166,15 +172,21 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps, int HW, int 
 // The two streaming passes of the backward work on channel pairs (f32x2_t, fdx_common.cuh) with reduced
 // algebra, because they are instruction-issue sensitive.  Per channel PAIR: h = x*(a/2) + b/2, t = tanh(h),
 //   sigmoid(z) = (1+t)/2,  silu'(z) = sigmoid(z) * (1 + h*(1-t)),  dz = dy * silu'(z)
-// = 6 pair ops + 2 MUFU.  Every thread owns 8 channels (16-byte vectors) of kBU pixels per iteration.
+// = 6 pair ops + 2 MUFU.  Mish: z = 2 h (exact), dz = dy * mish'(z) (fdx_common.cuh), 4 MUFU per pair.
+// Every thread owns 8 channels (16-byte vectors) of kBU pixels per iteration.
 constexpr int kBU = 3;   // pixels in flight per thread
 
 struct GnPair4 { f32x2_t v[4]; };
 
 // dz (x 2 when TWICE) for one channel pair
-template <bool SILU, bool TWICE>
+template <int ACT, bool TWICE>
 __device__ __forceinline__ f32x2_t gn_dz_pair(f32x2_t x, f32x2_t dy, f32x2_t ah, f32x2_t bh) {
-  if (!SILU) return TWICE ? f2_add(dy, dy) : dy;
+  if (ACT == GN_NONE) return TWICE ? f2_add(dy, dy) : dy;
+  if (ACT == GN_MISH) {
+    const f32x2_t h = f2_fma(x, ah, bh);
+    const f32x2_t d = f2_mul(dy, f2_pack(mish_grad(h.x + h.x), mish_grad(h.y + h.y)));
+    return TWICE ? f2_add(d, d) : d;
+  }
   const f32x2_t one = f2_pack(1.f, 1.f);
   const f32x2_t h = f2_fma(x, ah, bh);
   const f32x2_t t = f2_tanh(h);
@@ -186,7 +198,7 @@ __device__ __forceinline__ f32x2_t gn_dz_pair(f32x2_t x, f32x2_t dy, f32x2_t ah,
 // Pass 1.  red, dgamma and dbeta are linear in the per-(image, channel) sums, so every CTA adds its partial's
 // contribution straight into red[n][g][2] (zeroed by the caller), dgamma[c] and dbeta[c]; the first CTA of each
 // image also zeroes the column-sum outputs the second pass accumulates into.
-template <bool SILU>
+template <int ACT>
 __global__ void __launch_bounds__(kNT, 3)
 gn_bwd_stats_kernel(const __nv_bfloat16* __restrict__ x, long long xps,
                     const __nv_bfloat16* __restrict__ dy, long long dps, int HW, int C, int G,
@@ -242,7 +254,7 @@ gn_bwd_stats_kernel(const __nv_bfloat16* __restrict__ x, long long xps,
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const f32x2_t xv = f2_from_bf16x2(xw[j]);
-          const f32x2_t dz = gn_dz_pair<SILU, false>(xv, f2_from_bf16x2(dw[j]), ah.v[j], bh.v[j]);
+          const f32x2_t dz = gn_dz_pair<ACT, false>(xv, f2_from_bf16x2(dw[j]), ah.v[j], bh.v[j]);
           s0.v[j] = f2_add(s0.v[j], dz);
           s1.v[j] = f2_fma(dz, xv, s1.v[j]);
         }
@@ -324,7 +336,7 @@ gn_stats_from_cols_kernel(const float* __restrict__ cols, int slots, int N, int 
 
 // pass 2: dx (+= if accumulate); optionally the column sums of dx (csum_img[n][c], csum_tot[c]).
 //   dx = dz*a - x*c2 + c3 = (2 dz)*(a/2) + (c3 - x*c2)
-template <bool SILU, bool ACC, bool CS>
+template <int ACT, bool ACC, bool CS>
 __global__ void __launch_bounds__(kNT, ACC ? 2 : 3)
 gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps,
                     const __nv_bfloat16* __restrict__ dy, long long dps, int HW, int C, int G,
@@ -387,7 +399,7 @@ gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps,
     for (int j = 0; j < 4; ++j) {
       const float a0 = rstd * gamma[cv * 8 + 2 * j], a1 = rstd * gamma[cv * 8 + 2 * j + 1];
       ah.v[j] = f2_pack(0.5f * a0, 0.5f * a1);
-      bh.v[j] = SILU ? f2_pack(0.5f * (beta[cv * 8 + 2 * j] - mean * a0),
+      bh.v[j] = ACT != GN_NONE ? f2_pack(0.5f * (beta[cv * 8 + 2 * j] - mean * a0),
                                0.5f * (beta[cv * 8 + 2 * j + 1] - mean * a1))
                      : f2_pack(0.f, 0.f);
       cs.v[j] = f2_pack(0.f, 0.f);
@@ -422,7 +434,7 @@ gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xps,
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const f32x2_t xv = f2_from_bf16x2(xw[j]);
-            const f32x2_t dz2 = gn_dz_pair<SILU, true>(xv, f2_from_bf16x2(dw[j]), ah.v[j], bh.v[j]);
+            const f32x2_t dz2 = gn_dz_pair<ACT, true>(xv, f2_from_bf16x2(dw[j]), ah.v[j], bh.v[j]);
             f32x2_t v = f2_fma(dz2, ah.v[j], f2_fma(xv, nc2, c3p));
             if (CS) cs.v[j] = f2_add(cs.v[j], v);
             if (ACC) v = f2_add(v, f2_from_bf16x2(ow[j]));
@@ -587,7 +599,7 @@ dim3 gn_grid(const fdx_act* x, int unroll, int resident) {
 
 // second pass of the GroupNorm backward: template dispatch on (activation, accumulate, column sums)
 void launch_bwd_apply(const fdx_act* x, const fdx_act* dy, int groups, const float* stats, const float* red,
-                      const float* gamma, const float* beta, float eps, int silu, const fdx_act* dx,
+                      const float* gamma, const float* beta, float eps, int act, const fdx_act* dx,
                       const fdx_act* acc, float* csum_img, cudaStream_t st, float* csum_tot = nullptr,
                       const float* slot_ws = nullptr, int slots = 0, float* dgamma = nullptr, float* dbeta = nullptr) {
   const int accumulate = acc != nullptr;
@@ -605,18 +617,41 @@ void launch_bwd_apply(const fdx_act* x, const fdx_act* dy, int groups, const flo
                                                          (const __nv_bfloat16*)(acc ? acc->ptr : nullptr),          \
                                                          (long long)(acc ? acc->pix_stride : 0), csum_tot, slot_ws, \
                                                          slots, dgamma, dbeta)
-  const int key = (silu ? 4 : 0) | (accumulate ? 2 : 0) | (csum_img ? 1 : 0);
+  const int key = act * 4 | (accumulate ? 2 : 0) | (csum_img ? 1 : 0);
   switch (key) {
-    case 0: FDX_GN_APPLY(false, false, false); break;
-    case 1: FDX_GN_APPLY(false, false, true); break;
-    case 2: FDX_GN_APPLY(false, true, false); break;
-    case 3: FDX_GN_APPLY(false, true, true); break;
-    case 4: FDX_GN_APPLY(true, false, false); break;
-    case 5: FDX_GN_APPLY(true, false, true); break;
-    case 6: FDX_GN_APPLY(true, true, false); break;
-    default: FDX_GN_APPLY(true, true, true); break;
+    case 0: FDX_GN_APPLY(GN_NONE, false, false); break;
+    case 1: FDX_GN_APPLY(GN_NONE, false, true); break;
+    case 2: FDX_GN_APPLY(GN_NONE, true, false); break;
+    case 3: FDX_GN_APPLY(GN_NONE, true, true); break;
+    case 4: FDX_GN_APPLY(GN_SILU, false, false); break;
+    case 5: FDX_GN_APPLY(GN_SILU, false, true); break;
+    case 6: FDX_GN_APPLY(GN_SILU, true, false); break;
+    case 7: FDX_GN_APPLY(GN_SILU, true, true); break;
+    case 8: FDX_GN_APPLY(GN_MISH, false, false); break;
+    case 9: FDX_GN_APPLY(GN_MISH, false, true); break;
+    case 10: FDX_GN_APPLY(GN_MISH, true, false); break;
+    default: FDX_GN_APPLY(GN_MISH, true, true); break;
   }
 #undef FDX_GN_APPLY
+}
+
+bool act_ok(int act) { return act == GN_NONE || act == GN_SILU || act == GN_MISH; }
+
+// the GroupNorm apply, statistics from `stats` or (cols != nullptr) from the producers' column sums
+void launch_apply(int act, const fdx_act* x, int groups, const float* stats, const float* gamma, const float* beta,
+                  float eps, const fdx_act* y, const float* cols, int slots, int ld, int c0, float* stats_out,
+                  cudaStream_t st) {
+#define FDX_GN_FWD(A)                                                                                     \
+  gn_apply_kernel<A><<<gn_grid(x, kU, 5), kNT, 0, st>>>((const __nv_bfloat16*)x->ptr, x->pix_stride,       \
+                                                        x->h * x->w, x->c, groups, stats, gamma, beta, eps, \
+                                                        (__nv_bfloat16*)y->ptr, y->pix_stride, cols, slots, ld, c0, \
+                                                        stats_out)
+  switch (act) {
+    case GN_NONE: FDX_GN_FWD(GN_NONE); break;
+    case GN_SILU: FDX_GN_FWD(GN_SILU); break;
+    default: FDX_GN_FWD(GN_MISH); break;
+  }
+#undef FDX_GN_FWD
 }
 
 }  // namespace
@@ -646,50 +681,39 @@ int fdx_groupnorm_stats_from_cols(const float* cols, int slots, int N, int ld, i
 }
 
 int fdx_groupnorm_apply_cols(const fdx_act* x, int groups, const float* cols, int slots, int ld, int c0,
-                             const float* gamma, const float* beta, float eps, int silu, const fdx_act* y,
+                             const float* gamma, const float* beta, float eps, int act, const fdx_act* y,
                              float* stats_out, void* stream) {
   int s = gn_check(x, groups, "groupnorm_apply_cols");
   if (s != FDX_OK) return s;
+  FDX_REQUIRE(act_ok(act), "groupnorm_apply_cols: act=%d (0 = none, 1 = silu, 2 = mish)", act);
   FDX_REQUIRE(y && y->ptr && y->n == x->n && y->h == x->h && y->w == x->w && y->c == x->c,
               "groupnorm_apply_cols: output shape mismatch");
   FDX_REQUIRE(cols && stats_out && slots > 0 && c0 >= 0 && c0 + x->c <= ld && groups <= 64,
               "groupnorm_apply_cols: bad column-sum workspace");
-  if (silu)
-    gn_apply_kernel<true><<<gn_grid(x, kU, 5), kNT, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)x->ptr, x->pix_stride, x->h * x->w, x->c, groups, nullptr, gamma, beta, eps,
-        (__nv_bfloat16*)y->ptr, y->pix_stride, cols, slots, ld, c0, stats_out);
-  else
-    gn_apply_kernel<false><<<gn_grid(x, kU, 5), kNT, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)x->ptr, x->pix_stride, x->h * x->w, x->c, groups, nullptr, gamma, beta, eps,
-        (__nv_bfloat16*)y->ptr, y->pix_stride, cols, slots, ld, c0, stats_out);
+  launch_apply(act, x, groups, nullptr, gamma, beta, eps, y, cols, slots, ld, c0, stats_out, (cudaStream_t)stream);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
 }
 
 int fdx_groupnorm_apply(const fdx_act* x, int groups, const float* stats, const float* gamma,
-                        const float* beta, float eps, int silu, const fdx_act* y, void* stream) {
+                        const float* beta, float eps, int act, const fdx_act* y, void* stream) {
   int s = gn_check(x, groups, "groupnorm_apply");
   if (s != FDX_OK) return s;
+  FDX_REQUIRE(act_ok(act), "groupnorm_apply: act=%d (0 = none, 1 = silu, 2 = mish)", act);
   FDX_REQUIRE(y && y->ptr && y->n == x->n && y->h == x->h && y->w == x->w && y->c == x->c,
               "groupnorm_apply: output shape mismatch");
-  if (silu)
-    gn_apply_kernel<true><<<gn_grid(x, kU, 5), kNT, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)x->ptr, x->pix_stride, x->h * x->w, x->c, groups, stats, gamma, beta, eps,
-        (__nv_bfloat16*)y->ptr, y->pix_stride, nullptr, 0, 0, 0, nullptr);
-  else
-    gn_apply_kernel<false><<<gn_grid(x, kU, 5), kNT, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)x->ptr, x->pix_stride, x->h * x->w, x->c, groups, stats, gamma, beta, eps,
-        (__nv_bfloat16*)y->ptr, y->pix_stride, nullptr, 0, 0, 0, nullptr);
+  launch_apply(act, x, groups, stats, gamma, beta, eps, y, nullptr, 0, 0, 0, nullptr, (cudaStream_t)stream);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
 }
 
 static int groupnorm_bwd_impl(const fdx_act* x, const fdx_act* dy, int groups, const float* stats,
-                              const float* gamma, const float* beta, float eps, int silu, float* ws,
+                              const float* gamma, const float* beta, float eps, int act, float* ws,
                               float* dgamma, float* dbeta, const fdx_act* dx, const fdx_act* acc,
                               float* csum_img, float* csum_tot, void* stream) {
   int s = gn_check(x, groups, "groupnorm_bwd");
   if (s != FDX_OK) return s;
+  FDX_REQUIRE(act_ok(act), "groupnorm_bwd: act=%d (0 = none, 1 = silu, 2 = mish)", act);
   FDX_REQUIRE(dy && dy->ptr && dx && dx->ptr && ws && dgamma && dbeta, "groupnorm_bwd: null tensor");
   FDX_REQUIRE(dy->c == x->c && dx->c == x->c && dy->n == x->n && dx->n == x->n &&
                   dy->h == x->h && dy->w == x->w && dx->h == x->h && dx->w == x->w,
@@ -700,36 +724,38 @@ static int groupnorm_bwd_impl(const fdx_act* x, const fdx_act* dy, int groups, c
   float* red = ws;                          // [N][G][2]
   FDX_CUDA(cudaMemsetAsync(red, 0, sizeof(float) * 2 * N * groups, st));
   const size_t shm = sizeof(float) * (2 * (size_t)(kNT / (C / 8)) * C + 2 * C);
-  if (silu)
-    gn_bwd_stats_kernel<true><<<gn_grid(x, kBU, 3), kNT, shm, st>>>(
-        (const __nv_bfloat16*)x->ptr, x->pix_stride, (const __nv_bfloat16*)dy->ptr, dy->pix_stride, HW, C,
-        groups, stats, gamma, beta, eps, red, dgamma, dbeta, csum_img, csum_tot);
-  else
-    gn_bwd_stats_kernel<false><<<gn_grid(x, kBU, 3), kNT, shm, st>>>(
-        (const __nv_bfloat16*)x->ptr, x->pix_stride, (const __nv_bfloat16*)dy->ptr, dy->pix_stride, HW, C,
-        groups, stats, gamma, beta, eps, red, dgamma, dbeta, csum_img, csum_tot);
+#define FDX_GN_STATS(A)                                                                                    \
+  gn_bwd_stats_kernel<A><<<gn_grid(x, kBU, 3), kNT, shm, st>>>(                                            \
+      (const __nv_bfloat16*)x->ptr, x->pix_stride, (const __nv_bfloat16*)dy->ptr, dy->pix_stride, HW, C, groups, \
+      stats, gamma, beta, eps, red, dgamma, dbeta, csum_img, csum_tot)
+  switch (act) {
+    case GN_NONE: FDX_GN_STATS(GN_NONE); break;
+    case GN_SILU: FDX_GN_STATS(GN_SILU); break;
+    default: FDX_GN_STATS(GN_MISH); break;
+  }
+#undef FDX_GN_STATS
   FDX_LAUNCH_CHECK();
-  launch_bwd_apply(x, dy, groups, stats, red, gamma, beta, eps, silu, dx, acc, csum_img, st, csum_tot);
+  launch_bwd_apply(x, dy, groups, stats, red, gamma, beta, eps, act, dx, acc, csum_img, st, csum_tot);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
 }
 
 int fdx_groupnorm_bwd(const fdx_act* x, const fdx_act* dy, int groups, const float* stats,
-                      const float* gamma, const float* beta, float eps, int silu, float* ws,
+                      const float* gamma, const float* beta, float eps, int act, float* ws,
                       float* dgamma, float* dbeta, const fdx_act* dx, int accumulate,
                       float* csum_img, float* csum_tot, void* stream) {
-  return groupnorm_bwd_impl(x, dy, groups, stats, gamma, beta, eps, silu, ws, dgamma, dbeta, dx,
+  return groupnorm_bwd_impl(x, dy, groups, stats, gamma, beta, eps, act, ws, dgamma, dbeta, dx,
                             accumulate ? dx : nullptr, csum_img, csum_tot, stream);
 }
 
 int fdx_groupnorm_bwd_add(const fdx_act* x, const fdx_act* dy, int groups, const float* stats,
-                          const float* gamma, const float* beta, float eps, int silu, float* ws,
+                          const float* gamma, const float* beta, float eps, int act, float* ws,
                           float* dgamma, float* dbeta, const fdx_act* dx, const fdx_act* addend,
                           float* csum_img, float* csum_tot, void* stream) {
   FDX_REQUIRE(addend && addend->ptr, "groupnorm_bwd_add: null addend");
   FDX_REQUIRE(addend->c == x->c && addend->n == x->n && addend->h == x->h && addend->w == x->w,
               "groupnorm_bwd_add: addend shape mismatch");
-  return groupnorm_bwd_impl(x, dy, groups, stats, gamma, beta, eps, silu, ws, dgamma, dbeta, dx, addend, csum_img,
+  return groupnorm_bwd_impl(x, dy, groups, stats, gamma, beta, eps, act, ws, dgamma, dbeta, dx, addend, csum_img,
                             csum_tot, stream);
 }
 
@@ -759,10 +785,10 @@ static int groupnorm_bwd_dz_impl(const fdx_act* x, const fdx_act* dz, int groups
   cudaStream_t st = (cudaStream_t)stream;
   const int N = x->n, C = x->c;
   // one launch: the apply kernel's prologue collapses the slots and derives the per-group constants; dz already
-  // carries silu'(z), so it is the activation-free apply (beta is not read)
+  // carries the activation's derivative, so it is the activation-free apply (beta is not read)
   if (csum_img) FDX_CUDA(cudaMemsetAsync(csum_img, 0, sizeof(float) * N * C, st));
   if (csum_tot) FDX_CUDA(cudaMemsetAsync(csum_tot, 0, sizeof(float) * C, st));
-  launch_bwd_apply(x, dz, groups, stats, nullptr, gamma, gamma, eps, 0, dx, acc, csum_img, st, csum_tot, ws_slots,
+  launch_bwd_apply(x, dz, groups, stats, nullptr, gamma, gamma, eps, GN_NONE, dx, acc, csum_img, st, csum_tot, ws_slots,
                    slots, dgamma, dbeta);
   FDX_LAUNCH_CHECK();
   return FDX_OK;

@@ -62,6 +62,7 @@ struct TcLaunch {
   const float* gn_ab;
   float* gn_ws;
   int gn_slots;
+  int gn_mish;            // with gn_ab: dz = dy * mish'(z) instead of silu'(z); transposed engine only
   // gn_ws without gn_ab (TC_KMN only): per-(image, output channel) sum / sum of squares of the stored
   // values, gn_ws = [gn_slots][N][2][ws_ld] already offset to this launch's first channel.
   int ws_ld;

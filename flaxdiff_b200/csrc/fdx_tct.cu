@@ -88,17 +88,19 @@ __device__ __forceinline__ TileCoord tile_coord(const TctDev& p, int tile) {
 // GNB = true (HALO data gradient only): the first pass of the GroupNorm(+SiLU) backward in the epilogue - with x = the
 // GroupNorm input (side input `res`) and z = a_c x + b_c the kernel stores dz = dy * silu'(z) instead of dy and
 // accumulates S0 = sum dz, S1 = sum dz * x per (image, channel) into the column-sum workspace, exactly as the
-// pixels-as-M engine's EPI_GN_BWD (fdx_epilogue.cuh).
+// pixels-as-M engine's EPI_GN_BWD (fdx_epilogue.cuh).  MISH = true (GNB only): dz = dy * mish'(z) instead, for UNets
+// built with the mish activation; the pixels-as-M engine has no such variant.
 // RES = true (HALO with one K chunk, K = 64): all nine 8 KB weight tiles of the CTA's column block are loaded
 // once per CTA, on their own mbarrier, into 72 KB after the ring; a stage then carries only the 36 KB pixel box.
 // Otherwise every tile re-fetched the same 72 KB of weights, 40 % of its 180 KB of L2 -> shared-memory traffic.
 // The MMAs and their order (kx, ky, k16) are those of the plain HALO path, so the outputs are bit-identical.
-template <bool A_MN, bool HALO, bool GNB, bool RES>
+template <bool A_MN, bool HALO, bool GNB, bool RES, bool MISH>
 __global__ void __launch_bounds__(kThreads, 1)
 fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapX,
                const __grid_constant__ CUtensorMap mapR, const __grid_constant__ CUtensorMap mapO,
                const __grid_constant__ TctDev p) {
   static_assert(HALO || !RES, "tct: resident weights need the halo stage");
+  static_assert(GNB || !MISH, "tct: mish is an activation of the fused GroupNorm backward");
   constexpr int kStageBytes = stage_bytes(HALO, RES);
   constexpr int S = num_stages(HALO);
   constexpr int kRingBytes = ring_bytes(HALO, RES);                // the ring, then the resident weights
@@ -316,7 +318,10 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
               xv[0] = x2.x; xv[1] = x2.y;
               if constexpr (GNB) {
 #pragma unroll
-                for (int e = 0; e < 2; ++e) f[e] = epi_silu_grad_times(f[e], fmaf(xv[e], ga[h], gb[h]));
+                for (int e = 0; e < 2; ++e) {
+                  const float z = fmaf(xv[e], ga[h], gb[h]);
+                  f[e] = MISH ? f[e] * mish_grad(z) : epi_silu_grad_times(f[e], z);
+                }
               } else {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) f[e] += xv[e];
@@ -372,12 +377,12 @@ fdx_tct_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__
 // weights, pixels (the A operand), side input (unset without one) and output
 struct TctMaps { CUtensorMap w, x, r, o; };
 
-template <bool A_MN, bool HALO, bool GNB, bool RES>
+template <bool A_MN, bool HALO, bool GNB, bool RES, bool MISH>
 int launch_tct_grid(const TctMaps& m, const TctDev& d, cudaStream_t stream) {
   constexpr int smem = smem_bytes(HALO, RES);
   static bool attr_set = false;
   if (!attr_set) {
-    FDX_CUDA(cudaFuncSetAttribute(fdx_tct_kernel<A_MN, HALO, GNB, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    FDX_CUDA(cudaFuncSetAttribute(fdx_tct_kernel<A_MN, HALO, GNB, RES, MISH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   smem));
     attr_set = true;
   }
@@ -387,7 +392,7 @@ int launch_tct_grid(const TctMaps& m, const TctDev& d, cudaStream_t stream) {
   // multiple of cblks, so the clamp below keeps that.
   if (RES) grid = (grid >= d.cblks ? grid / d.cblks : 1) * d.cblks;
   if (d.ntiles < grid) grid = d.ntiles;
-  fdx_tct_kernel<A_MN, HALO, GNB, RES><<<grid, kThreads, smem, stream>>>(m.w, m.x, m.r, m.o, d);
+  fdx_tct_kernel<A_MN, HALO, GNB, RES, MISH><<<grid, kThreads, smem, stream>>>(m.w, m.x, m.r, m.o, d);
   fdx_note_kernel(FDX_KERNEL_TCT);
   FDX_LAUNCH_CHECK();
   return FDX_OK;
@@ -396,14 +401,14 @@ int launch_tct_grid(const TctMaps& m, const TctDev& d, cudaStream_t stream) {
 // Halo launches with one K chunk keep their weights resident (RES); at K >= 128 the nine taps (147 KB and more)
 // do not fit beside the ring.  RES needs a grid of whole column-block groups; where that would leave SMs idle
 // (cblks = 5 on 132 SMs: 130 CTAs) the plain halo launch is the faster one, by about 1 % on an H100 SXM.
-template <bool A_MN, bool HALO, bool GNB = false>
+template <bool A_MN, bool HALO, bool GNB = false, bool MISH = false>
 int launch_tct(const TctMaps& m, const TctDev& d, cudaStream_t stream) {
   if constexpr (HALO) {
     const int sms = fdx_num_sms();
     if (d.kchunks == 1 && std::min(d.ntiles, sms / d.cblks * d.cblks) == std::min(d.ntiles, sms))
-      return launch_tct_grid<A_MN, true, GNB, true>(m, d, stream);
+      return launch_tct_grid<A_MN, true, GNB, true, MISH>(m, d, stream);
   }
-  return launch_tct_grid<A_MN, HALO, GNB, false>(m, d, stream);
+  return launch_tct_grid<A_MN, HALO, GNB, false, MISH>(m, d, stream);
 }
 
 // TMA needs a 16-byte-aligned base and strides that are multiples of 16 bytes
@@ -474,6 +479,7 @@ int fdx_tct_launch(const TcLaunch& L, cudaStream_t stream) {
   if (s != FDX_OK) return s;
   if (L.res && (s = make_chunk_map(&m.r, L.res, L, L.rs_x, L.rs_y, L.rs_n)) != FDX_OK) return s;
   if (L.mode == TC_KMN) return halo ? launch_tct<true, true>(m, d, stream) : launch_tct<true, false>(m, d, stream);
-  if (L.gn_ab) return launch_tct<false, true, true>(m, d, stream);   // fused GroupNorm backward
+  if (L.gn_ab)   // fused GroupNorm backward
+    return L.gn_mish ? launch_tct<false, true, true, true>(m, d, stream) : launch_tct<false, true, true>(m, d, stream);
   return halo ? launch_tct<false, true>(m, d, stream) : launch_tct<false, false>(m, d, stream);
 }

@@ -135,15 +135,15 @@ class Node:
         self.cs_ok = True
         return (root.cs, self.coff)
 
-    def norm_apply(self, groups: int, gamma, beta, eps: float, silu: bool):
-        """(GroupNorm(+SiLU) of this tensor, its statistics): ONE launch when every producer's epilogue left its
+    def norm_apply(self, groups: int, gamma, beta, eps: float, act_fn: int):
+        """(act_fn(GroupNorm) of this tensor, its statistics): ONE launch when every producer's epilogue left its
         column sums (fdx_groupnorm_apply_cols), else a pass of fdx_groupnorm_stats + apply."""
         done = all(k.cs_ok for k in self.kids) if self.kids else self.cs_ok
         root = self.parent if self.parent is not None else self
         if done and root.cs is not None:
-            return ops.groupnorm_apply_cols(self.t, groups, root.cs, self.coff, gamma, beta, eps, silu)
+            return ops.groupnorm_apply_cols(self.t, groups, root.cs, self.coff, gamma, beta, eps, act_fn)
         st = ops.groupnorm_stats(self.t, groups)
-        return ops.groupnorm_apply(self.t, groups, st, gamma, beta, eps, silu), st
+        return ops.groupnorm_apply(self.t, groups, st, gamma, beta, eps, act_fn), st
 
     def grad_buf(self) -> torch.Tensor:
         if self.g is None:
@@ -174,10 +174,17 @@ class Unet:
         self.context_dim = context_dim
         if norm_groups <= 0:
             raise FdxError("Unet: norm_groups=0 (RMSNorm blocks) is not on the supported hot path")
-        # the kernels implement exactly one activation and one compute type: anything else must fail loudly
+        # the kernels implement two activations (swish = silu, and mish) and one compute type: anything else must fail
+        # loudly.  The activation runs after norm1 / norm2 of every ResidualBlock and after conv_out_norm
+        # (common.py:286-288, 310-312; simple_unet.py:209-210); it is resolved here to the kernels' code.
         act_name = activation if isinstance(activation, str) else getattr(activation, "__name__", repr(activation))
-        if act_name not in ("swish", "silu"):
-            raise FdxError(f"Unet: activation {act_name!r} is not supported (the fused kernels implement swish / silu)")
+        if act_name in ("swish", "silu"):
+            self._act = ops.ACT_SILU
+        elif act_name == "mish":
+            self._act = ops.ACT_MISH
+        else:
+            raise FdxError(f"Unet: activation {act_name!r} is not supported (the fused kernels implement swish / silu "
+                           "and mish)")
         if dtype is not None and dtype != torch.bfloat16:
             raise FdxError(f"Unet: dtype={dtype} is not supported: the engine computes in bf16 with f32 accumulation "
                            "(pass dtype=None or torch.bfloat16)")
@@ -519,7 +526,7 @@ class Unet:
                 tape.append(("conv", name, cur, dst))
                 cur = dst
             elif kind == "out":
-                a, st = cur.norm_apply(G, W[self._nout + "/scale"], W[self._nout + "/bias"], OUT_EPS, True)
+                a, st = cur.norm_apply(G, W[self._nout + "/scale"], W[self._nout + "/bias"], OUT_EPS, self._act)
                 Fo = ops.conv_out_fwd(a, W[name + "/conv/kernel"], W[name + "/conv/bias"])
                 tape.append(("out", name, cur, st, a))
                 cur = None
@@ -531,7 +538,7 @@ class Unet:
     def _res_fwd(self, name, xin: Node, dst: Node, emb16, W, W16, G, eps):
         x = xin.t
         cin, cout = x.shape[-1], dst.t.shape[-1]
-        a1, st1 = xin.norm_apply(G, W[f"{name}/{self._n1}/scale"], W[f"{name}/{self._n1}/bias"], eps, True)
+        a1, st1 = xin.norm_apply(G, W[f"{name}/{self._n1}/scale"], W[f"{name}/{self._n1}/bias"], eps, self._act)
         pre = self._rows.pop(name, None)
         if pre is not None:                       # computed on the side stream at the start of the forward
             row, ev = pre
@@ -543,7 +550,7 @@ class Unet:
         hnode = Node(torch.empty((x.shape[0], x.shape[1], x.shape[2], cout), dtype=BF16, device=x.device))
         hmid = ops.conv3x3_fwd(a1, W16[f"{name}/conv1/conv/kernel"], W[f"{name}/conv1/conv/bias"], rowvec=row,
                                out=hnode.t, colstats=hnode.colstats())
-        a2, st2 = hnode.norm_apply(G, W[f"{name}/{self._n2}/scale"], W[f"{name}/{self._n2}/bias"], eps, True)
+        a2, st2 = hnode.norm_apply(G, W[f"{name}/{self._n2}/scale"], W[f"{name}/{self._n2}/bias"], eps, self._act)
         if cin != cout:
             Bn, hh, ww, _ = x.shape
             r = torch.empty((Bn, hh, ww, cout), dtype=BF16, device=x.device)
@@ -815,7 +822,7 @@ class Unet:
                          col)
                 dx, acc = want(xin)
                 ops.groupnorm_bwd(xin.t, da, G, st, W[self._nout + "/scale"], W[self._nout + "/bias"], OUT_EPS,
-                                  True, Gd[self._nout + "/scale"], Gd[self._nout + "/bias"], dx, acc)
+                                  self._act, Gd[self._nout + "/scale"], Gd[self._nout + "/bias"], dx, acc)
             elif kind == "res":
                 self._res_bwd(rec, W, W16, Gd, G, emb16, demb, want, grad_of, side)
                 xin = rec[2]
@@ -890,7 +897,7 @@ class Unet:
                 _dense_wgrad(Gd[kres + "kernel"], x.view(M, cin), dout.view(M, cout))
                 Gd[kres + "bias"].copy_(Gd[f"{name}/conv2/conv/bias"])
         side.run(conv2_param_grads)
-        # conv2 data gradient -> norm2 + silu backward (first pass fused into the dgrad epilogue).
+        # conv2 data gradient -> norm2 + activation backward (first pass fused into the dgrad epilogue).
         # The same pass also emits the per-image / total column sums of dh: the timestep
         # row-vector gradient and the conv1 (= temb_projection) bias gradient
         dh = torch.empty_like(hmid)
@@ -898,7 +905,7 @@ class Unet:
         ops.conv_dgrad_groupnorm_bwd(dout, W16[f"{name}/conv2/conv/kernel"], hmid, G, st2,
                                      W[f"{name}/{self._n2}/scale"], W[f"{name}/{self._n2}/bias"], RES_EPS,
                                      Gd[f"{name}/{self._n2}/scale"], Gd[f"{name}/{self._n2}/bias"], dh, False,
-                                     csum_img=drow, csum_tot=Gd[f"{name}/conv1/conv/bias"])
+                                     csum_img=drow, csum_tot=Gd[f"{name}/conv1/conv/bias"], act_fn=self._act)
 
         def conv1_param_grads():
             # timestep projection (its bias gradient = conv1's), then the conv1 weight gradient
@@ -910,7 +917,7 @@ class Unet:
             side.keep.append(drow16)
             ops.conv3x3_wgrad(a1, dh, Gd[f"{name}/conv1/conv/kernel"])
         side.run(conv1_param_grads, dh, drow)
-        # conv1 data gradient -> norm1 + silu backward -> dx, joined with the skip gradient (out = h + residual,
+        # conv1 data gradient -> norm1 + activation backward -> dx, joined with the skip gradient (out = h + residual,
         # common.py:334-336) WITHOUT a separate read-modify-write pass over dx:
         #   1x1 residual conv : its data gradient is written (or accumulated) into dx FIRST - a plain store when dx is
         #                       fresh - and the GroupNorm backward adds on top (reads dx at HBM speed instead of
@@ -921,10 +928,10 @@ class Unet:
                W[f"{name}/{self._n1}/bias"], RES_EPS, Gd[f"{name}/{self._n1}/scale"], Gd[f"{name}/{self._n1}/bias"], dx)
         if cin != cout:
             ops.conv1x1_dgrad(dout, W16[kres + "kernel"], dx, accumulate=acc)
-            ops.conv_dgrad_groupnorm_bwd(*gn1, True)
+            ops.conv_dgrad_groupnorm_bwd(*gn1, True, act_fn=self._act)
         elif acc:
-            ops.conv_dgrad_groupnorm_bwd(*gn1, True)
+            ops.conv_dgrad_groupnorm_bwd(*gn1, True, act_fn=self._act)
             ops.act_add(dx, dout, dx)
         else:
-            ops.conv_dgrad_groupnorm_bwd(*gn1, False, addend=dout)
+            ops.conv_dgrad_groupnorm_bwd(*gn1, False, addend=dout, act_fn=self._act)
         del dh

@@ -148,6 +148,18 @@ def linear_fwd(x2d: torch.Tensor, w_kn: torch.Tensor, out: Optional[torch.Tensor
 
 
 # --------------------------------------------------------------------------- norms
+# Activation codes of the GroupNorm entry points' `act` argument.  The wrappers take the code or a bool, so that
+# the positional True / False of existing callers keep meaning silu / none.
+ACT_NONE, ACT_SILU, ACT_MISH = 0, 1, 2
+
+
+def _act_code(a) -> int:
+    code = int(a)
+    if code not in (ACT_NONE, ACT_SILU, ACT_MISH):
+        raise ValueError(f"activation code {a!r}: expected 0 (none), 1 (silu) or 2 (mish)")
+    return code
+
+
 def groupnorm_stats(x: torch.Tensor, groups: int) -> torch.Tensor:
     stats = torch.empty((x.shape[0], groups, 2), dtype=torch.float32, device=x.device)
     check(load().fdx_groupnorm_stats(ctypes.byref(act(x, "x")), ctypes.c_int(groups), ptr(stats),
@@ -155,17 +167,18 @@ def groupnorm_stats(x: torch.Tensor, groups: int) -> torch.Tensor:
     return stats
 
 
-def groupnorm_apply(x, groups, stats, gamma, beta, eps: float, silu: bool, out=None) -> torch.Tensor:
+def groupnorm_apply(x, groups, stats, gamma, beta, eps: float, act_fn, out=None) -> torch.Tensor:
+    """y = act_fn(GroupNorm(x)); act_fn = ACT_NONE / ACT_SILU / ACT_MISH (or False / True)."""
     if out is None:
         out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
     check(load().fdx_groupnorm_apply(ctypes.byref(act(x, "x")), ctypes.c_int(groups), ptr(stats),
                                      ptr(gamma), ptr(beta), ctypes.c_float(eps),
-                                     ctypes.c_int(1 if silu else 0), ctypes.byref(act(out, "out")),
+                                     ctypes.c_int(_act_code(act_fn)), ctypes.byref(act(out, "out")),
                                      stream_ptr()), "groupnorm_apply")
     return out
 
 
-def groupnorm_apply_cols(x, groups, cs: "ColStats", c0: int, gamma, beta, eps: float, silu: bool, out=None):
+def groupnorm_apply_cols(x, groups, cs: "ColStats", c0: int, gamma, beta, eps: float, act_fn, out=None):
     """groupnorm_apply with the statistics read from the producers' epilogue column sums (no stats_from_cols
     launch) -> (y, stats[N][groups][2] for the backward)."""
     if out is None:
@@ -173,28 +186,29 @@ def groupnorm_apply_cols(x, groups, cs: "ColStats", c0: int, gamma, beta, eps: f
     stats = torch.empty((cs.n, groups, 2), dtype=torch.float32, device=x.device)
     check(load().fdx_groupnorm_apply_cols(ctypes.byref(act(x, "x")), ctypes.c_int(groups), ptr(cs.ws),
                                           ctypes.c_int(cs.slots), ctypes.c_int(cs.channels), ctypes.c_int(c0),
-                                          ptr(gamma), ptr(beta), ctypes.c_float(eps), ctypes.c_int(1 if silu else 0),
+                                          ptr(gamma), ptr(beta), ctypes.c_float(eps), ctypes.c_int(_act_code(act_fn)),
                                           ctypes.byref(act(out, "out")), ptr(stats), stream_ptr()),
           "groupnorm_apply_cols")
     return out, stats
 
 
-def groupnorm_bwd(x, dy, groups, stats, gamma, beta, eps, silu, dgamma, dbeta, dx,
+def groupnorm_bwd(x, dy, groups, stats, gamma, beta, eps, act_fn, dgamma, dbeta, dx,
                   accumulate: bool = False, csum_img=None, csum_tot=None, addend=None) -> torch.Tensor:
-    """dx (+)= d/dx GroupNorm(+SiLU); `addend`: dx = d/dx + addend (another tensor of the same shape)."""
+    """dx (+)= d/dx act_fn(GroupNorm(x)); `addend`: dx = d/dx + addend (another tensor of the same shape)."""
+    code = _act_code(act_fn)
     red = torch.empty(2 * x.shape[0] * groups, dtype=torch.float32, device=x.device)
     if addend is not None:
         assert not accumulate
         check(load().fdx_groupnorm_bwd_add(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")),
                                            ctypes.c_int(groups), ptr(stats), ptr(gamma), ptr(beta),
-                                           ctypes.c_float(eps), ctypes.c_int(1 if silu else 0), ptr(red),
+                                           ctypes.c_float(eps), ctypes.c_int(code), ptr(red),
                                            ptr(dgamma), ptr(dbeta), ctypes.byref(act(dx, "dx")),
                                            ctypes.byref(act(addend, "addend")), ptr(csum_img), ptr(csum_tot),
                                            stream_ptr()), "groupnorm_bwd_add")
         return dx
     check(load().fdx_groupnorm_bwd(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")),
                                    ctypes.c_int(groups), ptr(stats), ptr(gamma), ptr(beta),
-                                   ctypes.c_float(eps), ctypes.c_int(1 if silu else 0), ptr(red),
+                                   ctypes.c_float(eps), ctypes.c_int(code), ptr(red),
                                    ptr(dgamma), ptr(dbeta), ctypes.byref(act(dx, "dx")),
                                    ctypes.c_int(1 if accumulate else 0), ptr(csum_img), ptr(csum_tot),
                                    stream_ptr()),
@@ -204,6 +218,9 @@ def groupnorm_bwd(x, dy, groups, stats, gamma, beta, eps, silu, dgamma, dbeta, d
 
 GN_FUSE_SLOTS = 8
 GN_FUSE_MIN_PIXELS = 128    # fdx_conv3x3_dgrad_gn needs one image per 128-pixel tile
+# Mish fuses by default only on images of at most 16 x 16 pixels: at 32^2 and 64^2 its epilogue (an exponential and a
+# reciprocal per element) made the fused backward 2-5 % slower than the two passes on an H100 SXM (DESIGN 3.2).
+GN_FUSE_MISH_MAX_PIXELS = 256
 
 
 def groupnorm_coeffs(stats, gamma, beta, hw: int, eps: float) -> torch.Tensor:
@@ -218,14 +235,15 @@ def groupnorm_coeffs(stats, gamma, beta, hw: int, eps: float) -> torch.Tensor:
 
 
 def conv3x3_dgrad_gn(dy: torch.Tensor, w_hwio: torch.Tensor, dz: torch.Tensor, x: torch.Tensor,
-                     ab: torch.Tensor, slots: int = GN_FUSE_SLOTS) -> torch.Tensor:
-    """Stride-1 data gradient with the first pass of GroupNorm(+SiLU) backward fused into its epilogue:
-    writes dz = dgrad * silu'(a x + b) and returns the per-slot sums workspace for groupnorm_bwd_dz."""
+                     ab: torch.Tensor, slots: int = GN_FUSE_SLOTS, act_fn=ACT_SILU) -> torch.Tensor:
+    """Stride-1 data gradient with the first pass of GroupNorm(+activation) backward fused into its epilogue:
+    writes dz = dgrad * act'(a x + b) and returns the per-slot sums workspace for groupnorm_bwd_dz.  act_fn =
+    ACT_SILU or ACT_MISH; mish runs on the transposed engine only (_gn_fuse_default) and raises elsewhere."""
     n, c = dz.shape[0], dz.shape[-1]
     ws = torch.empty((slots, n, 2, c), dtype=torch.float32, device=dz.device)
-    check(load().fdx_conv3x3_dgrad_gn(ctypes.byref(act(dy, "dy")), ptr(w_hwio), ctypes.byref(act(dz, "dz")),
-                                      ctypes.byref(act(x, "x")), ptr(ab), ptr(ws), ctypes.c_int(slots),
-                                      stream_ptr()), "conv3x3_dgrad_gn")
+    check(load().fdx_conv3x3_dgrad_gn_act(ctypes.byref(act(dy, "dy")), ptr(w_hwio), ctypes.byref(act(dz, "dz")),
+                                          ctypes.byref(act(x, "x")), ptr(ab), ptr(ws), ctypes.c_int(slots),
+                                          ctypes.c_int(_act_code(act_fn)), stream_ptr()), "conv3x3_dgrad_gn")
     return ws
 
 
@@ -259,22 +277,28 @@ def _gn_fuse_default(x: torch.Tensor, dy: torch.Tensor) -> bool:
 
 def conv_dgrad_groupnorm_bwd(dy, w_hwio, x, groups, stats, gamma, beta, eps, dgamma, dbeta, dx,
                              accumulate: bool = False, csum_img=None, csum_tot=None,
-                             fused: Optional[bool] = None, addend=None) -> torch.Tensor:
-    """d/dx of conv3x3(silu(groupnorm(x))) given dy = d/d(conv output): the data gradient with the first pass
-    of the GroupNorm backward in its epilogue (dz = dy * silu'(z), sum dz, sum dz*x) where that convolution runs
+                             fused: Optional[bool] = None, addend=None, act_fn=ACT_SILU) -> torch.Tensor:
+    """d/dx of conv3x3(act_fn(groupnorm(x))) given dy = d/d(conv output): the data gradient with the first pass
+    of the GroupNorm backward in its epilogue (dz = dy * act'(z), sum dz, sum dz*x) where that convolution runs
     on the transposed engine, then ONE pass over x and dz; elsewhere data gradient + the two-pass GroupNorm
-    backward.  `fused=True` fuses wherever an image has >= 128 pixels (also on the pixels-as-M engine),
-    `fused=False` never."""
+    backward.  SiLU: `fused=True` fuses wherever an image has >= 128 pixels (also on the pixels-as-M engine),
+    `fused=False` never.  Mish has a fused epilogue on the transposed engine only: by default it fuses where
+    _gn_fuse_default holds on images of at most GN_FUSE_MISH_MAX_PIXELS, `fused=True` wherever _gn_fuse_default
+    holds; every other shape takes the two passes."""
+    code = _act_code(act_fn)
     da = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
-    if fused is None:
+    if code == ACT_MISH:
+        small = x.shape[1] * x.shape[2] <= GN_FUSE_MISH_MAX_PIXELS
+        fused = fused is not False and _gn_fuse_default(x, dy) and (fused is True or small)
+    elif fused is None:
         fused = _gn_fuse_default(x, dy)
     if fused and x.shape[1] * x.shape[2] >= GN_FUSE_MIN_PIXELS:
         ab = groupnorm_coeffs(stats, gamma, beta, x.shape[1] * x.shape[2], eps)
-        ws = conv3x3_dgrad_gn(dy, w_hwio, da, x, ab)
+        ws = conv3x3_dgrad_gn(dy, w_hwio, da, x, ab, act_fn=code)
         return groupnorm_bwd_dz(x, da, groups, stats, gamma, eps, ws, dgamma, dbeta, dx, accumulate,
                                 csum_img=csum_img, csum_tot=csum_tot, addend=addend)
     conv3x3_dgrad(dy, w_hwio, da)
-    return groupnorm_bwd(x, da, groups, stats, gamma, beta, eps, True, dgamma, dbeta, dx, accumulate,
+    return groupnorm_bwd(x, da, groups, stats, gamma, beta, eps, code, dgamma, dbeta, dx, accumulate,
                          csum_img=csum_img, csum_tot=csum_tot, addend=addend)
 
 

@@ -265,15 +265,6 @@ def denormalize_images(images: torch.Tensor, target_type=torch.uint8, source_ran
     return images
 
 
-DTYPE_MAP = {
-    'bfloat16': torch.bfloat16, 'float32': torch.float32,
-    'jax.numpy.float32': torch.float32, 'jax.numpy.bfloat16': torch.bfloat16,
-    'None': None, None: None,
-}
-PRECISION_MAP = {k: k for k in ('high', 'HIGH', 'default', 'DEFAULT', 'highest', 'HIGHEST', 'None', None)}
-ACTIVATION_MAP = {'swish': 'swish', 'silu': 'swish', 'jax._src.nn.functions.silu': 'swish'}
-
-
 # ---------------------------------------------------------------------------------------------------------
 # configuration / checkpoint helpers of flaxdiff/utils.py:40-90, 239-263 (host side, no device work)
 # ---------------------------------------------------------------------------------------------------------
@@ -282,8 +273,10 @@ DTYPE_MAP = {"bfloat16": torch.bfloat16, "float32": torch.float32, "float16": to
 # accumulation), so they all map to None ("backend default")
 PRECISION_MAP = {"high": None, "HIGH": None, "default": None, "DEFAULT": None, "highest": None, "HIGHEST": None,
                  "None": None, None: None}
-# the reference maps names to jax.nn functions; the Unet here takes the NAME (only swish / silu is implemented)
-ACTIVATION_MAP = {"swish": "swish", "silu": "swish", "relu": "relu", "gelu": "gelu", "mish": "mish"}
+# the reference maps names to jax.nn functions; the Unet here takes the NAME (swish / silu and mish are implemented;
+# relu and gelu pass through so that the Unet refuses them by name)
+ACTIVATION_MAP = {"swish": "swish", "silu": "swish", "jax._src.nn.functions.silu": "swish", "mish": "mish",
+                  "relu": "relu", "gelu": "gelu"}
 
 
 def map_nested_config(config: dict) -> dict:

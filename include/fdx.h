@@ -129,41 +129,49 @@ int fdx_upconv3x3_wgrad(const fdx_act* x, const fdx_act* dy, float* dweff_ws, fl
 /* ---- normalisation (HBM-bound; warp-shuffle + shared/global atomics reductions) ---- */
 /* nn.GroupNorm(groups, eps) statistics (models/common.py:273-281): stats[n][g] = (sum, sumsq), f32. */
 int fdx_groupnorm_stats(const fdx_act* x, int groups, float* stats, void* stream);
-/* y = silu?((x-mean)*rstd*gamma+beta) (models/common.py:286-288,310-312; simple_unet.py:209-210). */
+/* y = act((x-mean)*rstd*gamma+beta) (models/common.py:286-288,310-312; simple_unet.py:209-210).
+ * act selects the activation, as in every GroupNorm entry point below: 0 = none, 1 = silu (swish),
+ * 2 = mish (z * tanh(softplus(z)), jax.nn.mish); any other value is FDX_ERR_INVALID_ARG. */
 int fdx_groupnorm_apply(const fdx_act* x, int groups, const float* stats, const float* gamma,
-                        const float* beta, float eps, int silu, const fdx_act* y, void* stream);
+                        const float* beta, float eps, int act, const fdx_act* y, void* stream);
 /* fdx_groupnorm_apply with the statistics taken straight from the producers' epilogue column sums
  * (cols = [slots][N][2][ld] as written by fdx_conv3x3_fwd_stats / fdx_upconv3x3_fwd_stats, channels c0 .. c0+C of
  * the buffer): no fdx_groupnorm_stats_from_cols launch; stats_out[N][groups][2] receives the statistics for the
  * backward. */
 int fdx_groupnorm_apply_cols(const fdx_act* x, int groups, const float* cols, int slots, int ld, int c0,
-                             const float* gamma, const float* beta, float eps, int silu, const fdx_act* y,
+                             const float* gamma, const float* beta, float eps, int act, const fdx_act* y,
                              float* stats_out, void* stream);
 /* Backward of the pair above.  ws: f32 scratch of 2*N*groups floats.  dgamma/dbeta ACCUMULATED.
  * csum_img [n][c] / csum_tot [c] (NULL allowed; csum_tot needs csum_img): column sums over pixels of the
  * dx this call produces, written (not accumulated) - the timestep row-vector and conv-bias gradients. */
 int fdx_groupnorm_bwd(const fdx_act* x, const fdx_act* dy, int groups, const float* stats,
-                      const float* gamma, const float* beta, float eps, int silu, float* ws,
+                      const float* gamma, const float* beta, float eps, int act, float* ws,
                       float* dgamma, float* dbeta, const fdx_act* dx, int accumulate,
                       float* csum_img, float* csum_tot, void* stream);
 /* Same, with the result ADDED to another tensor: dx = d/dx + addend (addend may be dx itself = accumulate).  The
  * ResidualBlock's skip gradient (common.py:334-336: out + residual) joins here instead of in a separate pass. */
 int fdx_groupnorm_bwd_add(const fdx_act* x, const fdx_act* dy, int groups, const float* stats,
-                          const float* gamma, const float* beta, float eps, int silu, float* ws,
+                          const float* gamma, const float* beta, float eps, int act, float* ws,
                           float* dgamma, float* dbeta, const fdx_act* dx, const fdx_act* addend,
                           float* csum_img, float* csum_tot, void* stream);
 /* Fused variant of the backward above: the data-gradient convolution that PRODUCES dy applies
- * silu'(z) in its epilogue and accumulates the first-pass sums, so x and dy are read once less.
+ * act'(z) in its epilogue and accumulates the first-pass sums, so x and dy are read once less.
  *   fdx_groupnorm_coeffs : ab[n][0][c] = rstd*gamma_c, ab[n][1][c] = beta_c - mean*rstd*gamma_c
  *   fdx_conv3x3_dgrad_gn : stride-1 3x3 data gradient (as fdx_conv3x3_dgrad) writing
  *                          dz = dgrad * silu'(a x + b) and ws_slots[slot][n][{0,1}][c] += (sum dz, sum dz*x);
  *                          zeroes ws_slots (slots*N*2*C floats) itself; FDX_ERR_UNSUPPORTED when an image
  *                          has fewer than 128 pixels (caller then uses the two-pass path)
+ *   fdx_conv3x3_dgrad_gn_act : the same with act'(z), act = 1 (silu; = fdx_conv3x3_dgrad_gn) or 2 (mish).
+ *                          Mish runs on the transposed engine only: FDX_ERR_UNSUPPORTED where it does not take
+ *                          the layer (Cin not in 64 .. 512, or a multiple of 256; H or W not a multiple of 16),
+ *                          and the caller uses fdx_conv3x3_dgrad + fdx_groupnorm_bwd(act = 2)
  *   fdx_groupnorm_bwd_dz : second pass from dz; ws is unused (NULL allowed). */
 int fdx_groupnorm_coeffs(const float* stats, const float* gamma, const float* beta, int N, int HW, int C,
                          int groups, float eps, float* ab, void* stream);
 int fdx_conv3x3_dgrad_gn(const fdx_act* dy, const void* w_hwio, const fdx_act* dz, const fdx_act* x,
                          const float* ab, float* ws_slots, int slots, void* stream);
+int fdx_conv3x3_dgrad_gn_act(const fdx_act* dy, const void* w_hwio, const fdx_act* dz, const fdx_act* x,
+                             const float* ab, float* ws_slots, int slots, int act, void* stream);
 int fdx_groupnorm_bwd_dz(const fdx_act* x, const fdx_act* dz, int groups, const float* stats,
                          const float* gamma, float eps, const float* ws_slots, int slots, float* ws,
                          float* dgamma, float* dbeta, const fdx_act* dx, int accumulate, float* csum_img,
