@@ -94,6 +94,10 @@ def _declare(lib) -> None:
     lib.fdx_token_embed.argtypes = [vp, i, i, vp, i, vp, i, vp, vp]
     lib.fdx_layernorm_fwd.argtypes = [vp, ll, i, vp, vp, f, vp, vp]
     lib.fdx_bias_act.argtypes = [vp, ll, i, vp, i, vp, vp]
+    lib.fdx_clip_image_prep.argtypes = [vp, i, i, i, vp, i, i, vp, i, i, i, vp, vp, vp]
+    lib.fdx_clip_vision_embed.argtypes = [vp, i, i, i, vp, vp, vp, vp, f, vp, vp]
+    lib.fdx_clip_pool.argtypes = [vp, i, i, i, vp, vp, vp, f, vp, vp]
+    lib.fdx_clip_similarity.argtypes = [vp, vp, i, i, vp, vp, vp]
 
 
 _lib: Optional[ctypes.CDLL] = None

@@ -72,50 +72,14 @@ class CLIPTextTower:
 
     # ------------------------------------------------------------------ weights
     def _pack(self, sd: Dict[str, torch.Tensor]) -> None:
-        def get(name, shape):
-            if name not in sd:
-                raise FdxError(f"CLIPTextTower: state dict has no {name!r}")
-            t = sd[name].detach().to("cpu", torch.float32)
-            if tuple(t.shape) != tuple(shape):
-                raise FdxError(f"CLIPTextTower: {name} has shape {tuple(t.shape)}, expected {tuple(shape)}")
-            return t
-
-        D, I = self.D, self.inner
+        get = state_getter(sd, "CLIPTextTower")
+        D = self.D
         entries = [("tok", get("embeddings.token_embedding.weight", (self.vocab, D)), torch.float32),
                    ("pos", get("embeddings.position_embedding.weight", (self.max_pos, D)), torch.float32)]
-        for i in range(self.layers):
-            p = f"encoder.layers.{i}."
-            wq, wk, wv = (get(p + f"self_attn.{n}_proj.weight", (D, D)) for n in "qkv")
-            bq, bk, bv = (get(p + f"self_attn.{n}_proj.bias", (D,)) for n in "qkv")
-            entries += [
-                (f"{i}.ln1_g", get(p + "layer_norm1.weight", (D,)), torch.float32),
-                (f"{i}.ln1_b", get(p + "layer_norm1.bias", (D,)), torch.float32),
-                (f"{i}.wqkv", torch.cat([wq.t(), wk.t(), wv.t()], dim=1), torch.bfloat16),
-                (f"{i}.bqkv", torch.cat([bq, bk, bv]), torch.float32),
-                (f"{i}.wo", get(p + "self_attn.out_proj.weight", (D, D)).t(), torch.bfloat16),
-                (f"{i}.bo", get(p + "self_attn.out_proj.bias", (D,)), torch.float32),
-                (f"{i}.ln2_g", get(p + "layer_norm2.weight", (D,)), torch.float32),
-                (f"{i}.ln2_b", get(p + "layer_norm2.bias", (D,)), torch.float32),
-                (f"{i}.w1", get(p + "mlp.fc1.weight", (I, D)).t(), torch.bfloat16),
-                (f"{i}.b1", get(p + "mlp.fc1.bias", (I,)), torch.float32),
-                (f"{i}.w2", get(p + "mlp.fc2.weight", (D, I)).t(), torch.bfloat16),
-                (f"{i}.b2", get(p + "mlp.fc2.bias", (D,)), torch.float32)]
+        entries += layer_entries(get, self.layers, D, self.inner)
         entries += [("lnf_g", get("final_layer_norm.weight", (D,)), torch.float32),
                     ("lnf_b", get("final_layer_norm.bias", (D,)), torch.float32)]
-        offsets, total = [], 0
-        for _, t, dt in entries:
-            offsets.append(total)
-            nbytes = t.numel() * (2 if dt == torch.bfloat16 else 4)
-            total += (nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
-        host = torch.zeros(total, dtype=torch.uint8)
-        for (_, t, dt), off in zip(entries, offsets):
-            b = t.to(dt).contiguous().view(torch.uint8).reshape(-1)
-            host[off:off + b.numel()] = b
-        self.buffer = host.to(self.device)
-        self.w = {}
-        for (name, t, dt), off in zip(entries, offsets):
-            n = t.numel() * (2 if dt == torch.bfloat16 else 4)
-            self.w[name] = self.buffer[off:off + n].view(dt).view(tuple(t.shape))
+        self.buffer, self.w = pack(entries, self.device)
 
     # ------------------------------------------------------------------ forward
     def encode(self, ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
@@ -132,23 +96,94 @@ class CLIPTextTower:
             if tuple(attention_mask.shape) != (B, T):
                 raise FdxError(f"CLIPTextTower: attention_mask {tuple(attention_mask.shape)} does not match ids")
             mask = attention_mask.to(self.device, torch.int32).contiguous()
-        D, w = self.D, self.w
-        h = ops.token_embed(ids, w["tok"], w["pos"])
-        h2 = h.view(B * T, D)
-        x = torch.empty((B * T, D), dtype=torch.bfloat16, device=self.device)
-        qkv = torch.empty((B, T, 3 * D), dtype=torch.bfloat16, device=self.device)
-        o = torch.empty((B, T, D), dtype=torch.bfloat16, device=self.device)
-        u = torch.empty((B * T, self.inner), dtype=torch.bfloat16, device=self.device)
-        for i in range(self.layers):
-            ops.layernorm_fwd(h2, w[f"{i}.ln1_g"], w[f"{i}.ln1_b"], self.eps, out=x)
-            ops.linear_fwd(x, w[f"{i}.wqkv"], out=qkv.view(B * T, 3 * D), bias=w[f"{i}.bqkv"])
-            ops.attention_fwd_masked(qkv[:, :, :D], qkv[:, :, D:2 * D], qkv[:, :, 2 * D:], self.heads, self.dh,
-                                     self.scale, True, mask, out=o)
-            ops.linear_fwd(o.view(B * T, D), w[f"{i}.wo"], out=h2, bias=w[f"{i}.bo"], res=h2)
-            ops.layernorm_fwd(h2, w[f"{i}.ln2_g"], w[f"{i}.ln2_b"], self.eps, out=x)
-            ops.linear_fwd(x, w[f"{i}.w1"], out=u)
-            ops.bias_act(u, w[f"{i}.b1"], self.act, out=u)
-            ops.linear_fwd(u, w[f"{i}.w2"], out=h2, bias=w[f"{i}.b2"], res=h2)
+        h = ops.token_embed(ids, self.w["tok"], self.w["pos"])
+        encoder_layers(h, self.w, self.layers, self.heads, self.inner, self.eps, self.act, causal=True, key_mask=mask)
         if out is None:
-            out = torch.empty((B, T, D), dtype=torch.bfloat16, device=self.device)
-        return ops.layernorm_fwd(h, w["lnf_g"], w["lnf_b"], self.eps, out=out)
+            out = torch.empty((B, T, self.D), dtype=torch.bfloat16, device=self.device)
+        return ops.layernorm_fwd(h, self.w["lnf_g"], self.w["lnf_b"], self.eps, out=out)
+
+
+def state_getter(sd: Dict[str, torch.Tensor], who: str):
+    """get(name, shape) -> the f32 CPU copy of sd[name], or FdxError when it is missing or has another shape."""
+    def get(name, shape):
+        if name not in sd:
+            raise FdxError(f"{who}: state dict has no {name!r}")
+        t = sd[name].detach().to("cpu", torch.float32)
+        if tuple(t.shape) != tuple(shape):
+            raise FdxError(f"{who}: {name} has shape {tuple(t.shape)}, expected {tuple(shape)}")
+        return t
+    return get
+
+
+def layer_entries(get, layers: int, D: int, I: int):
+    """The packed weights of CLIPEncoder's layers (shared by the text and vision towers): linear kernels bf16 in the
+    (in, out) layout, q / k / v fused into one [D, 3D] kernel; LayerNorm parameters and biases f32."""
+    entries = []
+    for i in range(layers):
+        p = f"encoder.layers.{i}."
+        wq, wk, wv = (get(p + f"self_attn.{n}_proj.weight", (D, D)) for n in "qkv")
+        bq, bk, bv = (get(p + f"self_attn.{n}_proj.bias", (D,)) for n in "qkv")
+        entries += [
+            (f"{i}.ln1_g", get(p + "layer_norm1.weight", (D,)), torch.float32),
+            (f"{i}.ln1_b", get(p + "layer_norm1.bias", (D,)), torch.float32),
+            (f"{i}.wqkv", torch.cat([wq.t(), wk.t(), wv.t()], dim=1), torch.bfloat16),
+            (f"{i}.bqkv", torch.cat([bq, bk, bv]), torch.float32),
+            (f"{i}.wo", get(p + "self_attn.out_proj.weight", (D, D)).t(), torch.bfloat16),
+            (f"{i}.bo", get(p + "self_attn.out_proj.bias", (D,)), torch.float32),
+            (f"{i}.ln2_g", get(p + "layer_norm2.weight", (D,)), torch.float32),
+            (f"{i}.ln2_b", get(p + "layer_norm2.bias", (D,)), torch.float32),
+            (f"{i}.w1", get(p + "mlp.fc1.weight", (I, D)).t(), torch.bfloat16),
+            (f"{i}.b1", get(p + "mlp.fc1.bias", (I,)), torch.float32),
+            (f"{i}.w2", get(p + "mlp.fc2.weight", (D, I)).t(), torch.bfloat16),
+            (f"{i}.b2", get(p + "mlp.fc2.bias", (D,)), torch.float32)]
+    return entries
+
+
+def pack(entries, device):
+    """One device buffer holding every (name, tensor, dtype) entry at a 256-byte aligned offset -> (buffer, {name:
+    view})."""
+    offsets, total = [], 0
+    for _, t, dt in entries:
+        offsets.append(total)
+        nbytes = t.numel() * (2 if dt == torch.bfloat16 else 4)
+        total += (nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
+    host = torch.zeros(total, dtype=torch.uint8)
+    for (_, t, dt), off in zip(entries, offsets):
+        b = t.to(dt).contiguous().view(torch.uint8).reshape(-1)
+        host[off:off + b.numel()] = b
+    buffer = host.to(device)
+    w = {}
+    for (name, t, dt), off in zip(entries, offsets):
+        n = t.numel() * (2 if dt == torch.bfloat16 else 4)
+        w[name] = buffer[off:off + n].view(dt).view(tuple(t.shape))
+    return buffer, w
+
+
+def encoder_layers(h: torch.Tensor, w, layers: int, heads: int, inner: int, eps: float, act: int,
+                   causal: bool = False, key_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """CLIPEncoder's pre-LN layers over the bf16 hidden state h [B, T, D], in place.  The text tower's attention is
+    causal under its attention mask (fdx_attention_fwd_masked), the vision tower's attends to every token
+    (fdx_attention_fwd)."""
+    B, T, D = h.shape
+    dh = D // heads
+    scale = 1.0 / math.sqrt(dh)
+    h2 = h.view(B * T, D)
+    x = torch.empty((B * T, D), dtype=torch.bfloat16, device=h.device)
+    qkv = torch.empty((B, T, 3 * D), dtype=torch.bfloat16, device=h.device)
+    o = torch.empty((B, T, D), dtype=torch.bfloat16, device=h.device)
+    u = torch.empty((B * T, inner), dtype=torch.bfloat16, device=h.device)
+    masked = causal or key_mask is not None
+    for i in range(layers):
+        ops.layernorm_fwd(h2, w[f"{i}.ln1_g"], w[f"{i}.ln1_b"], eps, out=x)
+        ops.linear_fwd(x, w[f"{i}.wqkv"], out=qkv.view(B * T, 3 * D), bias=w[f"{i}.bqkv"])
+        q, k, v = qkv[:, :, :D], qkv[:, :, D:2 * D], qkv[:, :, 2 * D:]
+        if masked:
+            ops.attention_fwd_masked(q, k, v, heads, dh, scale, causal, key_mask, out=o)
+        else:
+            ops.attention_fwd(q, k, v, heads, dh, scale, out=o)
+        ops.linear_fwd(o.view(B * T, D), w[f"{i}.wo"], out=h2, bias=w[f"{i}.bo"], res=h2)
+        ops.layernorm_fwd(h2, w[f"{i}.ln2_g"], w[f"{i}.ln2_b"], eps, out=x)
+        ops.linear_fwd(x, w[f"{i}.w1"], out=u)
+        ops.bias_act(u, w[f"{i}.b1"], act, out=u)
+        ops.linear_fwd(u, w[f"{i}.w2"], out=h2, bias=w[f"{i}.b2"], res=h2)
+    return h

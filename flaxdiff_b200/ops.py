@@ -854,6 +854,61 @@ def bias_act(x: torch.Tensor, bias: Optional[torch.Tensor], act_kind: int, out=N
     return out
 
 
+# --------------------------------------------------------------------------- CLIP metrics
+def clip_image_prep(x: torch.Tensor, tables: torch.Tensor, ksize_y: int, ksize_x: int, lut: torch.Tensor, crop: int,
+                    patch: int, ld: int, u8_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """f32 samples [B, H, W, 3] in [-1, 1] -> bf16 patch matrix [B * (crop / patch)^2, ld] (fdx_clip_image_prep);
+    u8_out: uint8 [B, crop, crop, 3] receives the resized, cropped image."""
+    B, H, W, C = x.shape
+    assert C == 3 and x.dtype == torch.float32 and x.is_contiguous()
+    assert tables.dtype == torch.int32 and tables.is_contiguous() and lut.dtype == torch.float32 and lut.numel() == 768
+    if u8_out is not None:
+        assert u8_out.dtype == torch.uint8 and u8_out.is_contiguous() and u8_out.shape == (B, crop, crop, 3)
+    G = crop // patch
+    out = torch.empty((B * G * G, ld), dtype=torch.bfloat16, device=x.device)
+    check(load().fdx_clip_image_prep(ptr(x), B, H, W, ptr(tables), ksize_y, ksize_x, ptr(lut), crop, patch, ld,
+                                     ptr(out), ptr(u8_out), stream_ptr()), "clip_image_prep")
+    return out
+
+
+def clip_vision_embed(patch_f32: torch.Tensor, B: int, cls: torch.Tensor, pos: torch.Tensor, gamma: torch.Tensor,
+                      beta: torch.Tensor, eps: float) -> torch.Tensor:
+    """bf16 [B, G2 + 1, D] = LN([cls; patch embeddings] + pos) from the patch GEMM's f32 [B * G2, D]."""
+    rows, D = patch_f32.shape
+    G2 = rows // B
+    assert patch_f32.dtype == torch.float32 and patch_f32.is_contiguous() and rows == B * G2
+    assert tuple(pos.shape) == (G2 + 1, D) and cls.numel() == D
+    out = torch.empty((B, G2 + 1, D), dtype=torch.bfloat16, device=patch_f32.device)
+    check(load().fdx_clip_vision_embed(ptr(patch_f32), B, G2, D, ptr(cls), ptr(pos), ptr(gamma), ptr(beta), eps,
+                                       ptr(out), stream_ptr()), "clip_vision_embed")
+    return out
+
+
+def clip_pool(x: torch.Tensor, ids: Optional[torch.Tensor] = None, gamma: Optional[torch.Tensor] = None,
+              beta: Optional[torch.Tensor] = None, eps: float = 1e-5) -> torch.Tensor:
+    """bf16 [B, D]: row 0 of each sequence of x [B, T, D] (ids None), or the row at argmax(ids[b]) (int32 [B, T]);
+    LayerNorm(gamma, beta) applied when given."""
+    B, T, D = x.shape
+    assert x.dtype == torch.bfloat16 and x.is_contiguous()
+    if ids is not None:
+        assert ids.dtype == torch.int32 and ids.is_contiguous() and tuple(ids.shape) == (B, T)
+    out = torch.empty((B, D), dtype=torch.bfloat16, device=x.device)
+    check(load().fdx_clip_pool(ptr(x), B, T, D, ptr(ids), ptr(gamma), ptr(beta), eps, ptr(out), stream_ptr()),
+          "clip_pool")
+    return out
+
+
+def clip_similarity(img: torch.Tensor, txt: torch.Tensor):
+    """-> (cos f32 [B], f32 [2] = (mean(1 - cos), mean(100 max(cos, 0)))) of the f32 embeddings [B, P]."""
+    B, P = img.shape
+    assert img.dtype == txt.dtype == torch.float32 and img.is_contiguous() and txt.is_contiguous()
+    assert tuple(txt.shape) == (B, P)
+    cos = torch.empty(B, dtype=torch.float32, device=img.device)
+    out2 = torch.empty(2, dtype=torch.float32, device=img.device)
+    check(load().fdx_clip_similarity(ptr(img), ptr(txt), B, P, ptr(cos), ptr(out2), stream_ptr()), "clip_similarity")
+    return cos, out2
+
+
 # --------------------------------------------------------------------------- temb / softmax
 def time_embed_fwd(t, freqs, W1, b1, W2, b2):
     B, D = t.shape[0], W1.shape[0]

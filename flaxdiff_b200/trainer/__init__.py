@@ -692,6 +692,8 @@ class GeneralDiffusionTrainer:
         samples = None
         try:
             metrics = {m.name: [] for m in self.eval_metrics} if self.eval_metrics else {}
+            # the direction a metric declares (EvaluationMetric.higher_is_better); metric_higher_is_better overrides it
+            declared = {f"val/{m.name}": bool(getattr(m, "higher_is_better", False)) for m in self.eval_metrics or []}
             for _ in range(val_steps_per_epoch):
                 batch = next(val_it) if val_it is not None else None
                 samples = val_step_fn(val_state, batch, diffusion_steps)
@@ -704,7 +706,7 @@ class GeneralDiffusionTrainer:
                 if not v:
                     continue
                 val, fk = float(np.mean(v)), f"val/{k}"
-                hib = self.metric_higher_is_better.get(fk, False)
+                hib = self.metric_higher_is_better.get(fk, declared.get(fk, False))
                 prev = self.best_val_metrics.get(fk)
                 self.best_val_metrics[fk] = val if prev is None else (max(prev, val) if hib else min(prev, val))
         except StopIteration:

@@ -391,6 +391,37 @@ int fdx_layernorm_fwd(const void* x_bf16, long long rows, int C, const float* ga
                       void* y_bf16, void* stream);
 int fdx_bias_act(const void* x_bf16, long long rows, int C, const float* bias, int act, void* y_bf16, void* stream);
 
+/* ---- CLIP validation metrics (fdx_clip.cu): get_clip_metric / get_clip_score_metric -----------------------------
+ * (flaxdiff/metrics/images.py:32-112, training.py:515-525).  The vision tower (transformers modeling_clip.py:640-690)
+ * and the text tower run on fdx_gemm, fdx_layernorm_fwd, fdx_attention_fwd[_masked] and fdx_bias_act; these four
+ * entry points are the rest.
+ *   fdx_clip_image_prep   : images.py:69-70 + AutoProcessor(use_fast=False): x f32 [B][H][W][3] ->
+ *                           u8 = ((x + 1) / 2) * 255 in f32, truncated (clamped to [0, 255], NaN -> 0) -> PIL's 8-bit
+ *                           two-pass bicubic resize of the crop window only -> lut[c][u8] (x / 255 normalised by the
+ *                           processor's mean / std) -> bf16 patches [B*G*G][ld], G = crop / patch, one row per
+ *                           patch in the (c, ky, kx) order of the HF conv weight, zero from 3*patch^2 to ld (a
+ *                           multiple of 8).  tables: int32 [crop][2 + ksize_y] (output rows) then
+ *                           [crop][2 + ksize_x] (output columns), each entry = first source index, tap count, taps
+ *                           with 22 fraction bits (PIL's precompute_coeffs + normalize_coeffs_8bpc; a pass PIL skips
+ *                           is one tap of 1 << 22).  lut: f32 [3][256].  u8_out: uint8 [B][crop][crop][3] or NULL.
+ *   fdx_clip_vision_embed : modeling_clip.py:206-245 + pre_layrnorm: out[b][t] = bf16(LN((t == 0 ? cls :
+ *                           patch_f32[b*G2 + t - 1]) + pos[t])) [B][G2 + 1][D], f32 statistics, one rounding.
+ *                           D a multiple of 8, <= 1280.
+ *   fdx_clip_pool         : out[b] = [LN](x[b][r_b]) bf16 [B][D] from x bf16 [B][T][D]; r_b = 0 when ids is NULL
+ *                           (the CLS row, with gamma / beta = post_layernorm), else the first position of the largest
+ *                           id of sequence b (FlaxCLIP's argmax(input_ids) EOS rule; ids int32 [B][T]).  gamma / beta
+ *                           NULL = no LayerNorm.  D a multiple of 8, <= 1280.
+ *   fdx_clip_similarity   : images.py:44-46, 65, 96: cos[b] = <a / (|a| + 1e-6), t / (|t| + 1e-6)> over img / txt f32 [B][P];
+ *                           out2 = {mean(1 - cos) (clip_similarity), mean(100 max(cos, 0)) (clip_score)}, f32. */
+int fdx_clip_image_prep(const float* x, int B, int H, int W, const int32_t* tables, int ksize_y, int ksize_x,
+                        const float* lut, int crop, int patch, int ld, void* patches_bf16, uint8_t* u8_out,
+                        void* stream);
+int fdx_clip_vision_embed(const float* patch_f32, int B, int G2, int D, const float* cls, const float* pos,
+                          const float* gamma, const float* beta, float eps, void* out_bf16, void* stream);
+int fdx_clip_pool(const void* x_bf16, int B, int T, int D, const int32_t* ids, const float* gamma, const float* beta,
+                  float eps, void* out_bf16, void* stream);
+int fdx_clip_similarity(const float* img, const float* txt, int B, int P, float* cos, float* out2, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
