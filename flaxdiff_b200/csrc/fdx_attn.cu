@@ -19,10 +19,11 @@
 //       fdx_attn_bwd_dkv  per 128-key block, loop over query tiles (transposed tiles, tile row = key):
 //                         dV += P^T dO ;  dK += dS^T Q
 //     with P = exp2(s * scale*log2e - lse*log2e), D = rowsum(dO o O), dS including the 1/sqrt(d) factor.
-// Tensors are bf16 [B][L][heads * dh] (row stride and batch stride given), dh in {32, 64, 128}; keys beyond Lk
-// and query rows beyond L are handled by TMA zero fill + masking, so 77-key cross-attention needs no padded copies.
-// dh = 128 has kernels of its own (fdx_attn_fwd128_kernel, fdx_attn_bwd128_kernel: two consumer warpgroups of 64
-// rows that keep every product in its wgmma fragment, 64-row backward tiles), described above them.
+// Tensors are bf16 [B][L][heads * dh] (row stride and batch stride given), dh in {32, 64, 128, 256}; keys beyond
+// Lk and query rows beyond L are handled by TMA zero fill + masking, so 77-key cross-attention needs no padded
+// copies.  dh = 128 has kernels of its own (fdx_attn_fwd128_kernel, fdx_attn_bwd128_kernel: two consumer
+// warpgroups of 64 rows that keep every product in its wgmma fragment, 64-row backward tiles), and so has dh = 256
+// (fdx_attn_fwd256_kernel, fdx_attn_bwd256_kernel: the same design on 64-key blocks), described above them.
 #include "fdx_common.cuh"
 #include "../../include/fdx.h"
 #include <math.h>
@@ -880,6 +881,382 @@ fdx_attn_bwd128_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_c
   }
 }
 
+// ======================================================================================================
+// head width 256.  The width-128 design with the key / column side cut to 64-row blocks: a 256-channel operand
+// is four 64-channel chunks (four TMA boxes), and a [128 keys][256 ch] K or V tile alone would take 64 KB.
+// Fragment layout, quad reductions and the P / dS tiles as above; every chunk of a 64-row operand is
+// [64 rows][64 ch] = 8 KB, so the MN-major B operands advance 8 KB per 64 channels.
+// ======================================================================================================
+constexpr int kChunk64 = 64 * 128;               // bytes of one [64 rows][64 ch] bf16 swizzled chunk
+constexpr int kOp256 = 4 * kChunk64;             // [64 rows][256 ch]: 32 KB
+
+// forward, 128 queries per CTA: warpgroup wg owns query rows [64 wg, 64 wg + 64); per 64-key block S = Q K_j^T is
+// one m64n64 fragment (32 registers) and O one m64n256 fragment (128 registers); P_j goes through the
+// warpgroup's own [64][64] bf16 tile.  Shared memory: Q 64 KB, 2 x (K, V) 128 KB, P 2 x 8 KB.
+// SHORT (<= 128 keys): both key blocks are loaded once behind one barrier; otherwise the two stages are a ring.
+template <bool SHORT>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+fdx_attn_fwd256_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                       const __grid_constant__ CUtensorMap mapV, const AttnDev p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  constexpr int NKV = 2;
+  uint8_t* sQ = smem;                                 // [4 chunks][128 queries][64 ch]
+  uint8_t* sKV = smem + 4 * kTile;                    // NKV x (K, V), each [4 chunks][64 keys][64 ch]
+  uint8_t* sP = sKV + NKV * 2 * kOp256;               // per warpgroup [64 queries][64 keys]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kChunk64);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;          // [NKV]
+  uint64_t* kv_empty = bars + 3;         // [NKV]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int head = blockIdx.y, b = blockIdx.z;
+  const int q0 = blockIdx.x * 128;
+  const int nblk = (p.Lk + 63) / 64;
+  const int c0 = head * 256;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&mapQ); tma_prefetch_desc(&mapK); tma_prefetch_desc(&mapV);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < NKV; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 2); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  // setmaxnreg sits inside each role's branch: issued before code both roles run, ptxas ignores it (C7507)
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && lane == 0) {
+      mbar_arrive_expect_tx(q_full, 4 * kTile);
+      for (int c = 0; c < 4; ++c) tma_load_4d(sQ + c * kTile, &mapQ, q_full, c0 + 64 * c, q0, b, 0);
+      if constexpr (SHORT) {
+        mbar_arrive_expect_tx(&kv_full[0], nblk * 2 * kOp256);
+      }
+      for (int j = 0; j < nblk; ++j) {
+        const int s = j % NKV;
+        uint8_t* kv = sKV + s * 2 * kOp256;
+        uint64_t* full = &kv_full[SHORT ? 0 : s];
+        if constexpr (!SHORT) {
+          mbar_wait(&kv_empty[s], ((j / NKV) & 1) ^ 1);
+          mbar_arrive_expect_tx(full, 2 * kOp256);
+        }
+        for (int c = 0; c < 4; ++c) {
+          tma_load_4d(kv + c * kChunk64, &mapK, full, c0 + 64 * c, j * 64, b, 0);
+          tma_load_4d(kv + kOp256 + c * kChunk64, &mapV, full, c0 + 64 * c, j * 64, b, 0);
+        }
+      }
+    }
+  } else {
+    consumer_regs();
+    const int wg = warp >> 2;
+    const int rq = (warp & 3) * 16 + (lane >> 2);      // fragment rows rq, rq + 8 of this warpgroup's 64
+    const int cq = 2 * (lane & 3);                     // fragment column offset inside each 8-column group
+    const uint32_t aQ = smem_u32(sQ) + wg * 8192;
+    const uint32_t aP = smem_u32(sP) + wg * kChunk64;
+    float m[2] = {-INFINITY, -INFINITY};               // running row maxima (log2 domain, scaled)
+    float l[2] = {0.f, 0.f};                           // running row sums over this thread's columns
+    float O[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) O[i] = 0.f;
+    mbar_wait(q_full, 0);
+    if constexpr (SHORT) mbar_wait(&kv_full[0], 0);
+
+    for (int j = 0; j < nblk; ++j) {
+      const int s = j % NKV;
+      if constexpr (!SHORT) mbar_wait(&kv_full[s], (j / NKV) & 1);
+      const uint32_t aK = smem_u32(sKV + s * 2 * kOp256), aV = aK + kOp256;
+      float S[32];                                     // the first K step overwrites it (scale_d = 0)
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        const uint32_t kc = (uint32_t)(k & 3) * 32;
+        wgmma_m64n64k16<0, 0>(S, gmma_desc_sw128(aQ + (k >> 2) * kTile + kc, 16, 1024),
+                              gmma_desc_sw128(aK + (k >> 2) * kChunk64 + kc, 16, 1024), k > 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // keys beyond Lk (TMA zero fill; only the last block can be partial) drop out as -inf logits
+      const int kvalid = p.Lk - j * 64;
+      if (kvalid < 64) {
+#pragma unroll
+        for (int g = 0; g < 8; ++g)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (8 * g + cq + e >= kvalid) S[4 * g + e] = S[4 * g + 2 + e] = -INFINITY;
+      }
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int g = 0; g < 8; ++g)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) mx[h] = fmaxf(mx[h], fmaxf(S[4 * g + 2 * h], S[4 * g + 2 * h + 1]));
+      float corr[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        const float m_new = fmaxf(m[h], mx[h] * p.scale_log2);
+        corr[h] = ex2(m[h] - m_new);                   // first block: exp2(-inf) = 0
+        m[h] = m_new;
+      }
+      // probabilities -> bf16 -> the K-major swizzled A tile of the PV MMA
+      float rs[2] = {0.f, 0.f};
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        float pe[4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            pe[2 * h + e] = ex2(fmaf(S[4 * g + 2 * h + e], p.scale_log2, -m[h]));
+            rs[h] += pe[2 * h + e];
+          }
+        st_frag_pair(aP, rq, 8 * g + cq, pack_bf16x2(pe[0], pe[1]));
+        st_frag_pair(aP, rq + 8, 8 * g + cq, pack_bf16x2(pe[2], pe[3]));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) l[h] = fmaf(l[h], corr[h], rs[h]);
+#pragma unroll
+      for (int g = 0; g < 32; ++g)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) O[4 * g + i] *= corr[i >> 1];
+      fence_proxy_async_smem();
+      named_bar_sync(1 + wg, 128);                     // every row of this warpgroup's P_j is in shared memory
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)                      // B = V_j, MN-major: 64-channel chunks kChunk64 apart
+        wgmma_m64n256k16<0, 1>(O, gmma_desc_sw128(aP + k * 32, 16, 1024),
+                               gmma_desc_sw128(aV + k * 2048, kChunk64, 1024));
+      wgmma_commit();
+      wgmma_wait<0>();
+      if constexpr (!SHORT) {
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[s]);
+      }
+    }
+    float inv[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+      inv[h] = 1.f / l[h];
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = q0 + wg * 64 + rq + 8 * h;
+      if (row < p.L) {
+        __nv_bfloat16* op = p.o + (long long)b * p.o_bs + (long long)row * p.o_ld + c0 + cq;
+#pragma unroll
+        for (int g = 0; g < 32; ++g)
+          *reinterpret_cast<uint32_t*>(op + 8 * g) = pack_bf16x2(O[4 * g + 2 * h] * inv[h], O[4 * g + 2 * h + 1] * inv[h]);
+        if (p.lse && (lane & 3) == 0) p.lse[((long long)b * p.heads + head) * p.L + row] = m[h] * kLn2 + logf(l[h]);
+      }
+    }
+  }
+}
+
+// backward at head width 256: the skeleton of fdx_attn_bwd128_kernel with 64-row steps on the column side.  Per
+// step each warpgroup computes 32 of the 64 columns of S and dP (m64n32, 16 + 16 registers) and writes its half
+// of E1 = P and E2 = dS; then
+//   dQ[:, 128 wg .. +128] += dS . K_j[:, 128 wg .. +128]   (m64n128 per warpgroup)    [ROWS_ARE_KEYS = false]
+//   dV += P^T . dO_i (warpgroup 0),  dK += dS^T . Q_i (warpgroup 1)   (m64n256)        [ROWS_ARE_KEYS = true]
+// Shared memory: R1, R2 2 x 32 KB, a ring of 2 x (C1, C2) 2 x 64 KB, E1, E2 2 x 8 KB.
+template <bool ROWS_ARE_KEYS>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+fdx_attn_bwd256_kernel(const __grid_constant__ CUtensorMap mapR1, const __grid_constant__ CUtensorMap mapR2,
+                       const __grid_constant__ CUtensorMap mapC1, const __grid_constant__ CUtensorMap mapC2,
+                       const AttnDev p) {
+  constexpr int RING = 2;
+  constexpr int AN = ROWS_ARE_KEYS ? 256 : 128;        // accumulator columns per warpgroup
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* sR1 = smem;                                 // [4 chunks][64 rows][64 ch]
+  uint8_t* sR2 = smem + kOp256;
+  uint8_t* sC = smem + 2 * kOp256;                     // RING x (C1, C2), each [4 chunks][64 rows][64 ch]
+  uint8_t* sE1 = sC + RING * 2 * kOp256;               // [64 rows][64 columns]
+  uint8_t* sE2 = sE1 + kChunk64;
+  float* sStat = reinterpret_cast<float*>(sE2 + kChunk64);       // 2 x (lse[64], dvec[64]) of the columns
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + 2 * 128);
+  uint64_t* r_full = bars;
+  uint64_t* c_full = bars + 1;            // [RING]
+  uint64_t* c_empty = c_full + RING;      // [RING]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int head = blockIdx.y, b = blockIdx.z;
+  const int r0 = blockIdx.x * 64;
+  const int nrows = ROWS_ARE_KEYS ? p.Lk : p.L;
+  const int ncols = ROWS_ARE_KEYS ? p.L : p.Lk;
+  const int nstep = (ncols + 63) / 64;
+  const int c0 = head * 256;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&mapR1); tma_prefetch_desc(&mapR2); tma_prefetch_desc(&mapC1); tma_prefetch_desc(&mapC2);
+    mbar_init(r_full, 1);
+    for (int i = 0; i < RING; ++i) { mbar_init(&c_full[i], 1); mbar_init(&c_empty[i], 2); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  // setmaxnreg sits inside each role's branch: issued before code both roles run, ptxas ignores it (C7507)
+  if (warp >= 8) {
+    producer_regs();
+    if (warp == 8 && lane == 0) {
+      mbar_arrive_expect_tx(r_full, 2 * kOp256);
+      for (int c = 0; c < 4; ++c) {
+        tma_load_4d(sR1 + c * kChunk64, &mapR1, r_full, c0 + 64 * c, r0, b, 0);
+        tma_load_4d(sR2 + c * kChunk64, &mapR2, r_full, c0 + 64 * c, r0, b, 0);
+      }
+      for (int j = 0; j < nstep; ++j) {
+        const int s = j % RING;
+        uint8_t* cp = sC + s * 2 * kOp256;
+        mbar_wait(&c_empty[s], ((j / RING) & 1) ^ 1);
+        mbar_arrive_expect_tx(&c_full[s], 2 * kOp256);
+        for (int c = 0; c < 4; ++c) {
+          tma_load_4d(cp + c * kChunk64, &mapC1, &c_full[s], c0 + 64 * c, j * 64, b, 0);
+          tma_load_4d(cp + kOp256 + c * kChunk64, &mapC2, &c_full[s], c0 + 64 * c, j * 64, b, 0);
+        }
+      }
+    }
+  } else {
+    consumer_regs();
+    const int wg = warp >> 2;                          // columns [32 wg, 32 wg + 32) of S / dP
+    const int rq = (warp & 3) * 16 + (lane >> 2);      // fragment rows rq, rq + 8
+    const int cq = 2 * (lane & 3);
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const long long stat_base = ((long long)b * p.heads + head) * p.L;
+    const bool row_in[2] = {r0 + rq < nrows, r0 + rq + 8 < nrows};
+    // dQ kernel: the statistics of this thread's two query rows; dK/dV kernel: they belong to the COLUMNS
+    float lse_r[2] = {0.f, 0.f}, d_r[2] = {0.f, 0.f};
+    if constexpr (!ROWS_ARE_KEYS) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (row_in[h]) {
+          lse_r[h] = p.lse[stat_base + r0 + rq + 8 * h] * kLog2e;
+          d_r[h] = p.dvec[stat_base + r0 + rq + 8 * h] * p.scale;
+        }
+    }
+    const uint32_t aR1 = smem_u32(sR1), aR2 = smem_u32(sR2);
+    const uint32_t aE1 = smem_u32(sE1), aE2 = smem_u32(sE2);
+    float A[AN / 2];                                   // dQ half | dV (warpgroup 0) or dK (warpgroup 1)
+#pragma unroll
+    for (int i = 0; i < AN / 2; ++i) A[i] = 0.f;
+    mbar_wait(r_full, 0);
+    for (int j = 0; j < nstep; ++j) {
+      const int s = j % RING;
+      const int cbase = j * 64;
+      if constexpr (ROWS_ARE_KEYS) {
+        // stage the query-side statistics of this step (parity buffer j & 1), 64 threads = 64 columns
+        if (threadIdx.x < 64) {
+          float* st = sStat + (j & 1) * 128;
+          const int t = threadIdx.x;
+          const bool ok = cbase + t < p.L;
+          st[t] = ok ? p.lse[stat_base + cbase + t] * kLog2e : 0.f;
+          st[64 + t] = ok ? p.dvec[stat_base + cbase + t] * p.scale : 0.f;
+        }
+      }
+      mbar_wait(&c_full[s], (j / RING) & 1);
+      const uint32_t aC1 = smem_u32(sC + s * 2 * kOp256), aC2 = aC1 + kOp256;
+      // S (or S^T) = R1 . C1^T ;  dP (or dP^T) = R2 . C2^T  - this warpgroup's 32 columns (rows 32 wg of C)
+      float Sa[16], Pa[16];                            // the first K step overwrites them (scale_d = 0)
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        const uint32_t ro = (uint32_t)((k >> 2) * kChunk64 + (k & 3) * 32);
+        const uint32_t co = ro + (uint32_t)wg * 4096;
+        wgmma_m64n32k16<0, 0>(Sa, gmma_desc_sw128(aR1 + ro, 16, 1024), gmma_desc_sw128(aC1 + co, 16, 1024), k > 0);
+        wgmma_m64n32k16<0, 0>(Pa, gmma_desc_sw128(aR2 + ro, 16, 1024), gmma_desc_sw128(aC2 + co, 16, 1024), k > 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      // the statistics are staged and the previous step's accumulation has consumed E1 / E2
+      named_bar_sync(1, 256);
+      const float* st = sStat + (j & 1) * 128;
+      // rows / columns outside the tensors (TMA zero fill; only the last row tile or step) drop out as -inf
+      // logits: P = 0 and dS = 0 there
+      const int col_lim = ncols - cbase - wg * 32;     // columns of this warpgroup inside the tensor
+      if (r0 + 64 > nrows || col_lim < 32) {
+#pragma unroll
+        for (int g = 0; g < 4; ++g)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (!(row_in[h] && 8 * g + cq + e < col_lim)) Sa[4 * g + 2 * h + e] = -INFINITY;
+      }
+      // P = exp2(s * scale*log2e - lse*log2e);  dS = P * (dP * scale - D * scale)
+#pragma unroll
+      for (int g = 0; g < 4; ++g) {
+        const int cl = wg * 32 + 8 * g + cq;           // column inside the step's 64
+        float lq[2][2], dq[2][2];                      // [h][e]
+        if constexpr (ROWS_ARE_KEYS) {
+          const float2 a2 = *reinterpret_cast<const float2*>(st + cl);
+          const float2 b2 = *reinterpret_cast<const float2*>(st + 64 + cl);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) { lq[h][0] = a2.x; lq[h][1] = a2.y; dq[h][0] = b2.x; dq[h][1] = b2.y; }
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) { lq[h][0] = lq[h][1] = lse_r[h]; dq[h][0] = dq[h][1] = d_r[h]; }
+        }
+        float pr[4], ds[4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int i = 4 * g + 2 * h + e;
+            pr[2 * h + e] = ex2(fmaf(Sa[i], p.scale_log2, -lq[h][e]));
+            ds[2 * h + e] = pr[2 * h + e] * fmaf(Pa[i], p.scale, -dq[h][e]);
+          }
+        if constexpr (ROWS_ARE_KEYS) {
+          st_frag_pair(aE1, rq, cl, pack_bf16x2(pr[0], pr[1]));
+          st_frag_pair(aE1, rq + 8, cl, pack_bf16x2(pr[2], pr[3]));
+        }
+        st_frag_pair(aE2, rq, cl, pack_bf16x2(ds[0], ds[1]));
+        st_frag_pair(aE2, rq + 8, cl, pack_bf16x2(ds[2], ds[3]));
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 256);                          // both halves of E1 / E2 are published
+      wgmma_fence();
+      if constexpr (ROWS_ARE_KEYS) {
+        // dV += P^T . dO_i (warpgroup 0) | dK += dS^T . Q_i (warpgroup 1); B MN-major, chunks kChunk64 apart
+        const uint32_t aE = wg == 0 ? aE1 : aE2;
+        const uint32_t aB = wg == 0 ? aC2 : aC1;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n256k16<0, 1>(A, gmma_desc_sw128(aE + k * 32, 16, 1024),
+                                 gmma_desc_sw128(aB + k * 2048, kChunk64, 1024));
+      } else {
+        // dQ[:, 128 wg ..] += dS . K_j[:, 128 wg ..]: B = channel chunks 2 wg, 2 wg + 1 of K_j
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n128k16<0, 1>(A, gmma_desc_sw128(aE2 + k * 32, 16, 1024),
+                                 gmma_desc_sw128(aC1 + wg * 2 * kChunk64 + k * 2048, kChunk64, 1024));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (wg_leader) mbar_arrive(&c_empty[s]);
+    }
+    // epilogue: fragment rows -> bf16
+    __nv_bfloat16* base;
+    long long ld;
+    if constexpr (ROWS_ARE_KEYS) {
+      base = wg == 0 ? p.dv + (long long)b * p.dv_bs : p.dk + (long long)b * p.dk_bs;
+      ld = wg == 0 ? p.dv_ld : p.dk_ld;
+      base += c0 + cq;
+    } else {
+      base = p.dq + (long long)b * p.dq_bs + c0 + wg * 128 + cq;
+      ld = p.dq_ld;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (row_in[h]) {
+        __nv_bfloat16* rp = base + (long long)(r0 + rq + 8 * h) * ld;
+#pragma unroll
+        for (int g = 0; g < AN / 8; ++g)
+          *reinterpret_cast<uint32_t*>(rp + 8 * g) = pack_bf16x2(A[4 * g + 2 * h], A[4 * g + 2 * h + 1]);
+      }
+    }
+  }
+}
+
 int make_map(CUtensorMap* m, const void* ptr, int hd, int rows, int B, long long ld, long long bs,
              int box_rows = 128) {
   uint64_t dims[4] = {(uint64_t)hd, (uint64_t)rows, (uint64_t)B, 1};
@@ -892,8 +1269,8 @@ int make_map(CUtensorMap* m, const void* ptr, int hd, int rows, int B, long long
 int check_desc(const fdx_attn_desc* a, const char* who) {
   FDX_REQUIRE(a && a->q && a->k && a->v, "%s: null tensor", who);
   FDX_REQUIRE(a->B > 0 && a->heads > 0 && a->L > 0 && a->Lk > 0, "%s: bad sizes", who);
-  FDX_REQUIRE(a->dh == 32 || a->dh == 64 || a->dh == 128,
-              "%s: head width %d (stored) must be 32 or 64, or 128 - zero-pad narrower heads", who, a->dh);
+  FDX_REQUIRE(a->dh == 32 || a->dh == 64 || a->dh == 128 || a->dh == 256,
+              "%s: head width %d (stored) must be 32 or 64, or 128 or 256 - zero-pad narrower heads", who, a->dh);
   FDX_REQUIRE((a->heads * a->dh) % 64 == 0, "%s: heads * dh must be a multiple of 64", who);
   FDX_REQUIRE(a->q_ld % 8 == 0, "%s: q_ld must be a multiple of 8 elements", who);
   FDX_REQUIRE(a->k_ld % 8 == 0, "%s: k_ld must be a multiple of 8 elements", who);
@@ -947,6 +1324,33 @@ int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
   int s = fwd_prepare(a, "attention_fwd", &mQ, &mK, &mV, &d);
   if (s != FDX_OK) return s;
   const bool short_keys = a->Lk <= 128;
+  if (a->dh == 256) {
+    // K and V come in 64-key blocks: their maps get 64-row boxes
+    CUtensorMap mK64, mV64;
+    if ((s = make_map(&mK64, a->k, a->heads * 256, a->Lk, a->B, a->k_ld, a->k_bs, 64)) != FDX_OK) return s;
+    if ((s = make_map(&mV64, a->v, a->heads * 256, a->Lk, a->B, a->v_ld, a->v_bs, 64)) != FDX_OK) return s;
+    const int smem256 = 4 * kTile + 2 * 2 * kOp256 + 2 * kChunk64 + 1024 + 64;
+    dim3 grid256((a->L + 127) / 128, a->heads, a->B);
+    static bool attr256[2] = {false, false};
+    if (short_keys) {
+      if (!attr256[0]) {
+        FDX_CUDA(cudaFuncSetAttribute(fdx_attn_fwd256_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      smem256));
+        attr256[0] = true;
+      }
+      fdx_attn_fwd256_kernel<true><<<grid256, kBwdThreads, smem256, (cudaStream_t)stream>>>(mQ, mK64, mV64, d);
+    } else {
+      if (!attr256[1]) {
+        FDX_CUDA(cudaFuncSetAttribute(fdx_attn_fwd256_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      smem256));
+        attr256[1] = true;
+      }
+      fdx_attn_fwd256_kernel<false><<<grid256, kBwdThreads, smem256, (cudaStream_t)stream>>>(mQ, mK64, mV64, d);
+    }
+    fdx_note_kernel(FDX_KERNEL_ATTN_FWD);
+    FDX_LAUNCH_CHECK();
+    return FDX_OK;
+  }
   if (a->dh == 128) {
     const int smem128 = (2 + 2 * (short_keys ? 1 : 2)) * kWTile + 1024 + 64;
     dim3 grid128((a->L + 127) / 128, a->heads, a->B);
@@ -996,8 +1400,8 @@ int fdx_attention_fwd(const fdx_attn_desc* a, void* stream) {
 }
 
 int fdx_attention_fwd_masked(const fdx_attn_desc* a, int causal, const int32_t* key_mask, void* stream) {
-  if (a && a->dh == 128) {
-    fdx_set_error("attention_fwd_masked: head width 128 is not supported (32 or 64)");
+  if (a && (a->dh == 128 || a->dh == 256)) {
+    fdx_set_error("attention_fwd_masked: head width %d is not supported (32 or 64)", a->dh);
     return FDX_ERR_UNSUPPORTED;
   }
   CUtensorMap mQ, mK, mV;
@@ -1062,6 +1466,33 @@ int fdx_attention_bwd(const fdx_attn_desc* a, void* stream) {
     const long long total = (long long)a->B * a->L * a->heads;
     attn_dvec_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d);
     FDX_LAUNCH_CHECK();
+  }
+  if (a->dh == 256) {
+    // both sides of both kernels come in 64-row blocks
+    CUtensorMap rQ, rK, rV, rDO;
+    if ((s = make_map(&rQ, a->q, hd, a->L, a->B, a->q_ld, a->q_bs, 64)) != FDX_OK) return s;
+    if ((s = make_map(&rK, a->k, hd, a->Lk, a->B, a->k_ld, a->k_bs, 64)) != FDX_OK) return s;
+    if ((s = make_map(&rV, a->v, hd, a->Lk, a->B, a->v_ld, a->v_bs, 64)) != FDX_OK) return s;
+    if ((s = make_map(&rDO, a->d_o, hd, a->L, a->B, a->do_ld, a->do_bs, 64)) != FDX_OK) return s;
+    const int smem256 = 2 * kOp256 + 2 * 2 * kOp256 + 2 * kChunk64 + 2 * 128 * 4 + 1024 + 64;
+    static bool attr256 = false;
+    if (!attr256) {
+      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_bwd256_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    smem256));
+      FDX_CUDA(cudaFuncSetAttribute(fdx_attn_bwd256_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    smem256));
+      attr256 = true;
+    }
+    // dQ: rows = queries (Q, dO), loop (K_j, V_j);  dK/dV: rows = keys (K, V), loop (Q_i, dO_i)
+    fdx_attn_bwd256_kernel<false><<<dim3((a->L + 63) / 64, a->heads, a->B), kBwdThreads, smem256, st>>>(
+        rQ, rDO, rK, rV, d);
+    fdx_note_kernel(FDX_KERNEL_ATTN_BWD);
+    FDX_LAUNCH_CHECK();
+    fdx_attn_bwd256_kernel<true><<<dim3((a->Lk + 63) / 64, a->heads, a->B), kBwdThreads, smem256, st>>>(
+        rK, rV, rQ, rDO, d);
+    fdx_note_kernel(FDX_KERNEL_ATTN_BWD);
+    FDX_LAUNCH_CHECK();
+    return FDX_OK;
   }
   if (a->dh == 128) {
     // the row side of a 64-row tile comes in 64-row boxes; the looped column side keeps the 128-row maps

@@ -44,7 +44,11 @@ ATTN_EPS = 1e-4     # TransformerBlock.norm_epsilon, models/attention.py:319
 
 
 def _attn_width(d: int) -> int:
-    """Stored head width for the fused attention kernels: 32, 64 or 128 (narrower heads are zero-padded)."""
+    """Stored head width for the fused attention kernels: 32, 64, 128 or 256 (narrower heads are zero-padded)."""
+    if d > 256:
+        raise FdxError(f"attention: head width {d} > 256 is not supported")
+    if d > 128:
+        return 256
     if d > 64:
         return 128
     return 32 if d <= 32 else 64
@@ -576,14 +580,13 @@ class Unet:
         """NormalAttention (models/attention.py:117-177) on 2-D token matrices: out = res + to_out(attn(
         to_q(xq), to_k(ctx), to_v(ctx))).  xq [B, L, C], ctx [B, Lk, Cc] bf16; res / out [B*L, C], row-strided.
         The projections are tensor-core GEMMs; the attention core is ONE fused kernel (fdx_attention_fwd: logits
-        and probabilities stay in registers / shared memory).  Heads narrower than 32 are zero-padded to 32, and
-        heads of 65 - 127 channels to 128 (the kernel stores heads 32, 64 or 128 wide)."""
+        and probabilities stay in registers / shared memory).  Heads narrower than 32 are zero-padded to 32,
+        heads of 65 - 127 channels to 128 and heads of 129 - 255 channels to 256 (the kernel stores heads 32, 64,
+        128 or 256 wide); wider heads are refused."""
         Bn, L, C = xq.shape
         Lk, Cc = ctx.shape[1], ctx.shape[2]
         d = C // heads
         dp = _attn_width(d)
-        if d > 128:
-            raise FdxError(f"attention: head width {d} > 128 is not supported")
         HD = heads * dp
         wq = self._pad_heads(W16[f"{base}/to_q/kernel"], 2, d, dp).reshape(C, HD)
         wk = self._pad_heads(W16[f"{base}/to_k/kernel"], 2, d, dp).reshape(Cc, HD)

@@ -350,7 +350,8 @@ int fdx_geglu_bwd(const void* u_bf16, const void* dg_bf16, long long rows, int i
  * Tensors: bf16 [B][rows][heads*dh], `*_ld` = elements between rows, `*_bs` = elements between images.  Every
  * `*_ld` and `*_bs` must be a multiple of 8 and q, k, v, o, d_o, dq, dk, dv 16-byte aligned (TMA boxes and
  * 16-byte vector accesses); otherwise FDX_ERR_INVALID_ARG, naming the field, before anything is launched.
- * dh (as STORED) is 32, 64 or 128 - narrower heads are zero-padded by the caller, `scale` = 1/sqrt(true width).
+ * dh (as STORED) is 32, 64, 128 or 256 - narrower heads are zero-padded by the caller, `scale` = 1/sqrt(true
+ * width).
  * lse: f32 [B][heads][L] (written by fwd, read by bwd); dvec_ws: f32 [B][heads][L] scratch (bwd). */
 typedef struct fdx_attn_desc {
   int B, heads, L, Lk, dh;
@@ -372,7 +373,8 @@ int fdx_attention_bwd(const fdx_attn_desc* a, void* stream);
 /* Forward with a key mask, as CLIPTextTransformer's self-attention (transformers' create_causal_mask over
  * `attention_mask`): key j is allowed for query i iff (!causal || j <= i) && key_mask[b][j] != 0.  key_mask is
  * int32 [B][Lk] of 0 / 1, or NULL (every key allowed).  A query row with no allowed key writes zeros (and
- * lse = -inf); the CLIP tokenizer never produces one.  dh 32 or 64; dh 128 gives FDX_ERR_UNSUPPORTED. */
+ * lse = -inf); the CLIP tokenizer never produces one.  dh 32 or 64 only; dh 128 or 256 gives
+ * FDX_ERR_UNSUPPORTED. */
 int fdx_attention_fwd_masked(const fdx_attn_desc* a, int causal, const int32_t* key_mask, void* stream);
 
 /* ---- CLIP text tower (fdx_clip.cu): FlaxCLIPTextModel of the text-conditioned trainer ------------------------
