@@ -83,7 +83,7 @@ class fdx_attn_desc(ctypes.Structure):
 
 GEMM_KK, GEMM_KMN, GEMM_MNMN = 0, 1, 2
 OPT_ADAM, OPT_LAMB = 0, 1
-ACT_QUICK_GELU, ACT_GELU = 0, 1          # fdx_bias_act
+ACT_QUICK_GELU, ACT_GELU, ACT_GELU_TANH = 0, 1, 2          # fdx_bias_act
 
 
 def _declare(lib) -> None:
@@ -98,6 +98,16 @@ def _declare(lib) -> None:
     lib.fdx_clip_vision_embed.argtypes = [vp, i, i, i, vp, vp, vp, vp, f, vp, vp]
     lib.fdx_clip_pool.argtypes = [vp, i, i, i, vp, vp, vp, f, vp, vp]
     lib.fdx_clip_similarity.argtypes = [vp, vp, i, i, vp, vp, vp]
+    lib.fdx_dit_adaln_fwd.argtypes = [vp, ll, i, i, vp, ll, i, i, vp, vp, f, vp, vp, vp, vp]
+    lib.fdx_dit_adaln_bwd.argtypes = [vp, vp, ll, i, i, vp, ll, i, vp, vp, vp, vp, vp, vp, i, vp, ll, vp, ll, i, i, vp]
+    lib.fdx_dit_gate_fwd.argtypes = [vp, vp, ll, i, i, vp, ll, vp, vp]
+    lib.fdx_dit_gate_bwd.argtypes = [vp, vp, ll, i, i, vp, ll, vp, vp, i, vp, ll, vp]
+    lib.fdx_dit_token_mean.argtypes = [vp, i, i, i, vp, i, vp, vp]
+    lib.fdx_dit_rope.argtypes = [vp, ll, i, ll, i, i, i, i, ll, i, vp]
+    lib.fdx_bias_act_bwd.argtypes = [vp, ll, i, vp, i, vp, vp, vp]
+    lib.fdx_dit_patchify.argtypes = [vp, i, i, i, i, i, i, i, vp, vp]
+    lib.fdx_dit_unpatchify.argtypes = [vp, i, i, i, i, i, i, vp, vp]
+    lib.fdx_dit_fourier.argtypes = [vp, i, vp, i, vp, vp]
 
 
 _lib: Optional[ctypes.CDLL] = None

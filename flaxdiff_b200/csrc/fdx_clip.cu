@@ -317,6 +317,9 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 
 
 }  // namespace
 
+// the tanh-gelu of the DiT's MLP lives with its backward in fdx_dit.cu
+int fdx_dit_bias_gelu_tanh(const void* x_bf16, long long rows, int C, const float* bias, void* y_bf16, void* stream);
+
 extern "C" {
 
 int fdx_token_embed(const int32_t* ids, int B, int T, const float* tok, int vocab, const float* pos, int D,
@@ -351,9 +354,11 @@ int fdx_layernorm_fwd(const void* x_bf16, long long rows, int C, const float* ga
 int fdx_bias_act(const void* x_bf16, long long rows, int C, const float* bias, int act, void* y_bf16, void* stream) {
   FDX_REQUIRE(x_bf16 && y_bf16, "bias_act: null pointer");
   FDX_REQUIRE(rows > 0 && C > 0 && C % 8 == 0, "bias_act: C=%d must be a multiple of 8", C);
-  FDX_REQUIRE(act == FDX_ACT_QUICK_GELU || act == FDX_ACT_GELU, "bias_act: unknown activation %d", act);
+  FDX_REQUIRE(act == FDX_ACT_QUICK_GELU || act == FDX_ACT_GELU || act == FDX_ACT_GELU_TANH,
+              "bias_act: unknown activation %d", act);
   FDX_REQUIRE(aligned16(x_bf16) && aligned16(y_bf16) && (!bias || aligned16(bias)),
               "bias_act: tensors must be 16-byte aligned");
+  if (act == FDX_ACT_GELU_TANH) return fdx_dit_bias_gelu_tanh(x_bf16, rows, C, bias, y_bf16, stream);
   const int grid = stream_grid(rows * (C / 8), 256);
   if (act == FDX_ACT_QUICK_GELU)
     bias_act_kernel<FDX_ACT_QUICK_GELU><<<grid, 256, 0, (cudaStream_t)stream>>>(

@@ -844,13 +844,141 @@ def layernorm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps:
 
 
 def bias_act(x: torch.Tensor, bias: Optional[torch.Tensor], act_kind: int, out=None) -> torch.Tensor:
-    """act(x + bias) over the last axis (_lib.ACT_QUICK_GELU / ACT_GELU); out may be x."""
+    """act(x + bias) over the last axis (_lib.ACT_QUICK_GELU / ACT_GELU / ACT_GELU_TANH); out may be x."""
     C = x.shape[-1]
     assert x.dtype == torch.bfloat16 and x.is_contiguous() and (bias is None or bias.dtype == torch.float32)
     if out is None:
         out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
     assert out.is_contiguous() and out.shape == x.shape
     check(load().fdx_bias_act(ptr(x), x.numel() // C, C, ptr(bias), act_kind, ptr(out), stream_ptr()), "bias_act")
+    return out
+
+
+def bias_act_bwd(x: torch.Tensor, bias: Optional[torch.Tensor], act_kind: int, dy: torch.Tensor, out=None) -> torch.Tensor:
+    """dx = dy * act'(x + bias) (act_kind = _lib.ACT_GELU_TANH)."""
+    C = x.shape[-1]
+    assert x.dtype == dy.dtype == torch.bfloat16 and x.is_contiguous() and dy.is_contiguous() and dy.shape == x.shape
+    if out is None:
+        out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
+    check(load().fdx_bias_act_bwd(ptr(x), x.numel() // C, C, ptr(bias), act_kind, ptr(dy), ptr(out), stream_ptr()),
+          "bias_act_bwd")
+    return out
+
+
+# --------------------------------------------------------------------------- SimpleDiT streaming kernels
+def _dit_chunks(B: int, L: int, C: int, device) -> int:
+    """Token chunks per sample of the two-stage column sums: enough blocks for eight per SM, chunks of >= 32 rows."""
+    sms = torch.cuda.get_device_properties(device).multi_processor_count
+    blocks = -(-C // 64) * B
+    return max(1, min(-(-L // 32), -(-8 * sms // blocks)))
+
+
+def _tokens(t: torch.Tensor, name: str):
+    assert t.dtype == torch.bfloat16 and t.dim() == 2 and t.is_contiguous(), (name, t.dtype, t.shape, t.stride())
+    return t.shape
+
+
+def dit_adaln_fwd(x: torch.Tensor, L: int, ada: Optional[torch.Tensor] = None, scale_off: int = 0,
+                  shift_off: int = 0, gamma=None, beta=None, eps: float = 1e-5, stats: bool = True, out=None):
+    """adaLN LayerNorm of the token rows x [B*L, C] -> (y bf16, mean f32 [rows] or None, rstd or None)."""
+    rows, C = _tokens(x, "x")
+    y = out if out is not None else torch.empty((rows, C), dtype=torch.bfloat16, device=x.device)
+    mean = torch.empty(rows, dtype=torch.float32, device=x.device) if stats else None
+    rstd = torch.empty_like(mean) if stats else None
+    a, ld = (ada, ada.stride(0)) if ada is not None else (None, 0)
+    check(load().fdx_dit_adaln_fwd(ptr(x), rows, L, C, ptr(a), ld, scale_off, shift_off, ptr(gamma), ptr(beta), eps,
+                                   ptr(y), ptr(mean), ptr(rstd), stream_ptr()), "dit_adaln_fwd")
+    return y, mean, rstd
+
+
+def dit_adaln_bwd(x, dy, L: int, mean, rstd, d0: torch.Tensor, d1: torch.Tensor, ada=None, scale_off: int = 0,
+                  gamma=None, addend=None, out=None, reduce_samples: bool = False, accumulate: bool = False):
+    """Backward of dit_adaln_fwd -> dx bf16 [rows, C] (+ addend).  d0 / d1: f32 [B, >= C] row views (the d(scale) /
+    d(shift) chunks of d_ada) or, reduce_samples, f32 [C] (d(gamma) / d(beta))."""
+    rows, C = _tokens(x, "x")
+    _tokens(dy, "dy")
+    B = rows // L
+    dx = out if out is not None else torch.empty((rows, C), dtype=torch.bfloat16, device=x.device)
+    nch = _dit_chunks(B, L, C, x.device)
+    ws = torch.empty(B * nch * 2 * C, dtype=torch.float32, device=x.device)
+    a, ld = (ada, ada.stride(0)) if ada is not None else (None, 0)
+    ld0 = d0.stride(0) if d0.dim() == 2 else 0
+    ld1 = d1.stride(0) if d1.dim() == 2 else 0
+    check(load().fdx_dit_adaln_bwd(ptr(x), ptr(dy), rows, L, C, ptr(a), ld, scale_off, ptr(gamma), ptr(mean),
+                                   ptr(rstd), ptr(addend), ptr(dx), ptr(ws), nch, ptr(d0), ld0, ptr(d1), ld1,
+                                   1 if reduce_samples else 0, 1 if accumulate else 0, stream_ptr()), "dit_adaln_bwd")
+    return dx
+
+
+def dit_gate_fwd(x: torch.Tensor, y: torch.Tensor, L: int, gate: torch.Tensor, out=None) -> torch.Tensor:
+    """x + gate[b] * y over token rows [B*L, C]; gate an f32 [B, C] row view (a chunk of the ada rows)."""
+    rows, C = _tokens(x, "x")
+    _tokens(y, "y")
+    assert gate.dtype == torch.float32 and gate.stride(1) == 1
+    out = out if out is not None else torch.empty((rows, C), dtype=torch.bfloat16, device=x.device)
+    check(load().fdx_dit_gate_fwd(ptr(x), ptr(y), rows, L, C, ptr(gate), gate.stride(0), ptr(out), stream_ptr()),
+          "dit_gate_fwd")
+    return out
+
+
+def dit_gate_bwd(dout: torch.Tensor, y: torch.Tensor, L: int, gate: torch.Tensor, dgate: torch.Tensor) -> torch.Tensor:
+    """-> dy = gate[b] * dout; writes dgate[b] = sum over the sample's tokens of dout * y (f32 [B, C] row view)."""
+    rows, C = _tokens(dout, "dout")
+    _tokens(y, "y")
+    B = rows // L
+    dy = torch.empty((rows, C), dtype=torch.bfloat16, device=dout.device)
+    nch = _dit_chunks(B, L, C, dout.device)
+    ws = torch.empty(B * nch * 2 * C, dtype=torch.float32, device=dout.device)
+    check(load().fdx_dit_gate_bwd(ptr(dout), ptr(y), rows, L, C, ptr(gate), gate.stride(0), ptr(dy), ptr(ws), nch,
+                                  ptr(dgate), dgate.stride(0), stream_ptr()), "dit_gate_bwd")
+    return dy
+
+
+def dit_token_mean(x: torch.Tensor) -> torch.Tensor:
+    """f32 [B, C] mean over the tokens of x bf16 [B, T, C]."""
+    B, T, C = x.shape
+    assert x.dtype == torch.bfloat16 and x.is_contiguous()
+    nch = _dit_chunks(B, T, C, x.device)
+    ws = torch.empty(B * nch * 2 * C, dtype=torch.float32, device=x.device)
+    out = torch.empty((B, C), dtype=torch.float32, device=x.device)
+    check(load().fdx_dit_token_mean(ptr(x), B, T, C, ptr(ws), nch, ptr(out), stream_ptr()), "dit_token_mean")
+    return out
+
+
+def dit_rope(t: torch.Tensor, L: int, heads: int, d: int, dp: int, nmat: int = 1, mat_off: int = 0,
+             inverse: bool = False) -> torch.Tensor:
+    """RoPE in place on nmat head matrices (mat_off columns apart) of the bf16 rows of t [rows, >= ...]."""
+    assert t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1
+    check(load().fdx_dit_rope(ptr(t), t.shape[0], L, t.stride(0), heads, d, dp, nmat, mat_off, 1 if inverse else 0,
+                              stream_ptr()), "dit_rope")
+    return t
+
+
+def dit_patchify(x: torch.Tensor, p: int, ld: int) -> torch.Tensor:
+    """(B, H, W, C) f32 / bf16 -> bf16 [B*(H/p)*(W/p), ld] patch rows (zeros past p*p*C)."""
+    B, H, W, C = x.shape
+    assert x.is_contiguous() and x.dtype in (torch.float32, torch.bfloat16)
+    out = torch.empty((B * (H // p) * (W // p), ld), dtype=torch.bfloat16, device=x.device)
+    check(load().fdx_dit_patchify(ptr(x), 1 if x.dtype == torch.float32 else 0, B, H, W, C, p, ld, ptr(out),
+                                  stream_ptr()), "dit_patchify")
+    return out
+
+
+def dit_unpatchify(y: torch.Tensor, B: int, H: int, W: int, C: int, p: int) -> torch.Tensor:
+    """f32 rows [B*L, ld] -> f32 (B, H, W, C)."""
+    assert y.dtype == torch.float32 and y.dim() == 2 and y.stride(1) == 1
+    out = torch.empty((B, H, W, C), dtype=torch.float32, device=y.device)
+    check(load().fdx_dit_unpatchify(ptr(y), y.stride(0), B, H, W, C, p, ptr(out), stream_ptr()), "dit_unpatchify")
+    return out
+
+
+def dit_fourier(t: torch.Tensor, freqs: torch.Tensor) -> torch.Tensor:
+    """bf16 [B, 2*len(freqs)] = [sin(2 pi t freqs), cos(2 pi t freqs)]."""
+    t = _f32c(t)
+    assert freqs.dtype == torch.float32 and freqs.is_contiguous()
+    out = torch.empty((t.numel(), 2 * freqs.numel()), dtype=torch.bfloat16, device=t.device)
+    check(load().fdx_dit_fourier(ptr(t), t.numel(), ptr(freqs), freqs.numel(), ptr(out), stream_ptr()),
+          "dit_fourier")
     return out
 
 

@@ -387,6 +387,7 @@ int fdx_attention_fwd_masked(const fdx_attn_desc* a, int causal, const int32_t* 
  *   fdx_bias_act      : y = act(x + bias) (bias f32 [C] or NULL; x == y allowed).  C a multiple of 8. */
 #define FDX_ACT_QUICK_GELU 0 /* z * sigmoid(1.702 z) */
 #define FDX_ACT_GELU 1       /* exact erf gelu */
+#define FDX_ACT_GELU_TANH 2  /* 0.5 z (1 + tanh(sqrt(2/pi) (z + 0.044715 z^3))): jax.nn.gelu's default (fdx_dit.cu) */
 int fdx_token_embed(const int32_t* ids, int B, int T, const float* tok, int vocab, const float* pos, int D,
                     void* out_bf16, void* stream);
 int fdx_layernorm_fwd(const void* x_bf16, long long rows, int C, const float* gamma, const float* beta, float eps,
@@ -423,6 +424,54 @@ int fdx_clip_vision_embed(const float* patch_f32, int B, int G2, int D, const fl
 int fdx_clip_pool(const void* x_bf16, int B, int T, int D, const int32_t* ids, const float* gamma, const float* beta,
                   float eps, void* out_bf16, void* stream);
 int fdx_clip_similarity(const float* img, const float* txt, int B, int P, float* cos, float* out2, void* stream);
+
+/* ---- SimpleDiT (fdx_dit.cu): flaxdiff/models/simple_dit.py:23-306 ---------------------------------------------------
+ * The dense layers run on fdx_gemm and the attention on fdx_attention_fwd / _bwd; these are the streaming passes
+ * around them.  Token matrices are bf16 [rows = B * L][C] (row stride C), L tokens per sample; `ada` is the f32
+ * [B][ada_ld] output of a block's ada_proj, whose six F-wide chunks a call addresses by column offset.  Column sums run
+ * in two ordered stages through ws = f32 [B][nchunk][2][C] (nchunk token chunks per sample): no atomics, the results
+ * are reproducible bit for bit.
+ *   fdx_dit_adaln_fwd   : y = (xhat * gamma + beta) * (1 + ada[b][scale_off + c]) + ada[b][shift_off + c], xhat the
+ *                         LayerNorm of the token (f32 statistics; mean / rstd f32 [rows] written when non-NULL).  A
+ *                         NULL ada, gamma or beta drops its term; ada and gamma exclusive.  C a multiple of 8, <= 1536.
+ *   fdx_dit_adaln_bwd   : its backward: dx = d/dx (+ addend; dx may alias addend); d0 / d1 (+)= the sums of dy * xhat
+ *                         and of dy over each sample's tokens, rows of d0_ld / d1_ld floats (d(scale), d(shift) into
+ *                         their chunks of a d_ada buffer) or, reduce_samples, over all rows (d(gamma), d(beta)).
+ *   fdx_dit_gate_fwd    : out = x + gate[b][c] * y (the gated residual; gate rows gate_ld floats apart; out may be x).
+ *   fdx_dit_gate_bwd    : dy = gate[b][c] * dout and dgate[b][c] = sum over the sample's tokens of dout * y.
+ *   fdx_dit_token_mean  : out[b][c] = mean over t of x[b][t][c] (f32 [B][C]); ws as above.
+ *   fdx_dit_rope        : RoPE in place on nmat matrices mat_off columns apart in rows of ld elements (q and k of the
+ *                         fused QKV output): per dp-wide head, pair (i, i + d/2), i < d/2, rotated by the angle
+ *                         (token index in its sample) * 10000^(-2i/d); `inverse` applies the transposed rotation (the
+ *                         backward).  Channels [d, dp) of each head are set to zero.  d even.
+ *   fdx_bias_act_bwd    : dx = dy * act'(x + bias), act = FDX_ACT_GELU_TANH.
+ *   fdx_dit_patchify    : src (B, H, W, C) f32 (src_f32) or bf16 -> dst bf16 [B * (H/p) * (W/p)][ld], row-major
+ *                         patches, columns (p1, p2, c), zeros from p*p*C to ld (a multiple of 8).  The patch-embedding
+ *                         GEMM's operand, and the transpose of fdx_dit_unpatchify (the final projection's gradient).
+ *   fdx_dit_unpatchify  : src f32 [B * L][ld] -> dst f32 (B, H, W, C): 'B (h w) (p1 p2 C) -> B (h p1) (w p2) C'
+ *                         (vit_common.py:10-17) over the first p*p*C columns; the transpose of fdx_dit_patchify.
+ *   fdx_dit_fourier     : out bf16 [B][2 half] = [sin(t_b 2 pi freqs), cos(t_b 2 pi freqs)] (models/common.py:97-110). */
+int fdx_dit_adaln_fwd(const void* x_bf16, long long rows, int L, int C, const float* ada, long long ada_ld,
+                      int scale_off, int shift_off, const float* gamma, const float* beta, float eps, void* y_bf16,
+                      float* mean, float* rstd, void* stream);
+int fdx_dit_adaln_bwd(const void* x_bf16, const void* dy_bf16, long long rows, int L, int C, const float* ada,
+                      long long ada_ld, int scale_off, const float* gamma, const float* mean, const float* rstd,
+                      const void* addend_bf16, void* dx_bf16, float* ws, int nchunk, float* d0, long long d0_ld,
+                      float* d1, long long d1_ld, int reduce_samples, int accumulate, void* stream);
+int fdx_dit_gate_fwd(const void* x_bf16, const void* y_bf16, long long rows, int L, int C, const float* gate,
+                     long long gate_ld, void* out_bf16, void* stream);
+int fdx_dit_gate_bwd(const void* dout_bf16, const void* y_bf16, long long rows, int L, int C, const float* gate,
+                     long long gate_ld, void* dy_bf16, float* ws, int nchunk, float* dgate, long long dgate_ld,
+                     void* stream);
+int fdx_dit_token_mean(const void* x_bf16, int B, int T, int C, float* ws, int nchunk, float* out, void* stream);
+int fdx_dit_rope(void* base_bf16, long long rows, int L, long long ld, int heads, int d, int dp, int nmat,
+                 long long mat_off, int inverse, void* stream);
+int fdx_bias_act_bwd(const void* x_bf16, long long rows, int C, const float* bias, int act, const void* dy_bf16,
+                     void* dx_bf16, void* stream);
+int fdx_dit_patchify(const void* src, int src_f32, int B, int H, int W, int C, int p, int ld, void* dst_bf16,
+                     void* stream);
+int fdx_dit_unpatchify(const float* src, int ld, int B, int H, int W, int C, int p, float* dst, void* stream);
+int fdx_dit_fourier(const float* t, int B, const float* freqs, int half, void* out_bf16, void* stream);
 
 #ifdef __cplusplus
 }
