@@ -108,6 +108,12 @@ def _declare(lib) -> None:
     lib.fdx_dit_patchify.argtypes = [vp, i, i, i, i, i, i, i, vp, vp]
     lib.fdx_dit_unpatchify.argtypes = [vp, i, i, i, i, i, i, vp, vp]
     lib.fdx_dit_fourier.argtypes = [vp, i, vp, i, vp, vp]
+    lib.fdx_ssm_discretize.argtypes = [vp, vp, vp, vp, vp, vp, vp, i, i, vp, i, i, vp, vp, vp]
+    lib.fdx_ssm_discretize_bwd.argtypes = [vp, vp, vp, vp, vp, i, i, vp, i, vp, vp, vp, i, i, vp, vp, vp, vp, vp, vp,
+                                           vp, vp]
+    lib.fdx_ssm_scan.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp]
+    lib.fdx_ssm_scan_bwd.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp]
+    lib.fdx_permute_rows.argtypes = [vp, vp, ll, i, ll, vp, vp]
 
 
 _lib: Optional[ctypes.CDLL] = None

@@ -48,6 +48,12 @@ def sincos_2d_table(F: int, HP: int, WP: int):
     return pos.reshape(HP * WP, F)
 
 
+def _lecun_normal(t: torch.Tensor, fan_in: int, gen: torch.Generator) -> None:
+    """flax's lecun_normal: a normal truncated at two standard deviations, rescaled to variance 1 / fan_in."""
+    std = math.sqrt(1.0 / fan_in) / 0.87962566103423978
+    torch.nn.init.trunc_normal_(t, mean=0.0, std=std, a=-2 * std, b=2 * std, generator=gen)
+
+
 class SimpleDiT:
     def __init__(self, output_channels: int = 3, patch_size: int = 16, emb_features: int = 768, num_layers: int = 12,
                  num_heads: int = 12, mlp_ratio: int = 4, dropout_rate: float = 0.0, dtype=None, precision=None,
@@ -96,27 +102,62 @@ class SimpleDiT:
 
     # ------------------------------------------------------------------ structure
     def param_specs(self):
-        F, h, p, E = self.emb_features, self.num_heads, self.patch_size, self.emb_features * self.mlp_ratio
-        d = F // h
+        F, p, E = self.emb_features, self.patch_size, self.emb_features * self.mlp_ratio
         nout = p * p * self.output_channels * (2 if self.learn_sigma else 1)
-        specs = [("patch_embed/Conv_0/kernel", (p, p, 3, F)), ("patch_embed/Conv_0/bias", (F,)),
+        specs = self._embed_specs() + [
                  ("time_embed/layers_1/DenseGeneral_0/kernel", (F, E)), ("time_embed/layers_1/DenseGeneral_0/bias", (E,)),
                  ("time_embed/layers_1/DenseGeneral_1/kernel", (E, E)), ("time_embed/layers_1/DenseGeneral_1/bias", (E,)),
                  ("time_embed/layers_2/kernel", (E, F)), ("time_embed/layers_2/bias", (F,))]
         if self.context_dim:
             specs += [("text_context_proj/kernel", (self.context_dim, F)), ("text_context_proj/bias", (F,))]
-        for i in range(self.num_layers):
-            n = f"dit_block_{i}"
-            specs += [(f"{n}/ada_params_module/ada_proj/kernel", (F, 6 * F)),
-                      (f"{n}/ada_params_module/ada_proj/bias", (6 * F,))]
-            for m in ("to_q", "to_k", "to_v"):
-                specs += [(f"{n}/attention/{m}/kernel", (F, h, d)), (f"{n}/attention/{m}/bias", (h, d))]
-            specs += [(f"{n}/attention/to_out_0/kernel", (h, d, F)), (f"{n}/attention/to_out_0/bias", (F,)),
-                      (f"{n}/mlp/layers_0/kernel", (F, E)), (f"{n}/mlp/layers_0/bias", (E,)),
-                      (f"{n}/mlp/layers_2/kernel", (E, F)), (f"{n}/mlp/layers_2/bias", (F,))]
+        for n, _, _ in self._blocks():
+            specs += self._block_specs(n)
         specs += [("final_norm/scale", (F,)), ("final_norm/bias", (F,)),
                   ("final_proj/kernel", (F, nout)), ("final_proj/bias", (nout,))]
         return specs
+
+    def _embed_name(self) -> str:
+        """The patch embedding's dense layer: PatchEmbedding's p x p stride-p conv."""
+        return "patch_embed/Conv_0"
+
+    def _embed_specs(self):
+        p, F = self.patch_size, self.emb_features
+        return [("patch_embed/Conv_0/kernel", (p, p, 3, F)), ("patch_embed/Conv_0/bias", (F,))]
+
+    def _block_specs(self, n):
+        """DiTBlock `n`'s parameters: ada_proj, the attention's q / k / v / out DenseGenerals and the MLP."""
+        F, h, E = self.emb_features, self.num_heads, self.emb_features * self.mlp_ratio
+        d = F // h
+        specs = [(f"{n}/ada_params_module/ada_proj/kernel", (F, 6 * F)),
+                 (f"{n}/ada_params_module/ada_proj/bias", (6 * F,))]
+        for m in ("to_q", "to_k", "to_v"):
+            specs += [(f"{n}/attention/{m}/kernel", (F, h, d)), (f"{n}/attention/{m}/bias", (h, d))]
+        specs += [(f"{n}/attention/to_out_0/kernel", (h, d, F)), (f"{n}/attention/to_out_0/bias", (F,)),
+                  (f"{n}/mlp/layers_0/kernel", (F, E)), (f"{n}/mlp/layers_0/bias", (E,)),
+                  (f"{n}/mlp/layers_2/kernel", (E, F)), (f"{n}/mlp/layers_2/bias", (F,))]
+        return specs
+
+    def _blocks(self):
+        """(name, forward, backward) of every block, in order."""
+        return [(f"dit_block_{i}", self._block_fwd, self._block_bwd) for i in range(self.num_layers)]
+
+    def _scan_indices(self, HP: int, WP: int):
+        """The patch order as row-major indices (token i is patch idx[i]), or None for raster order."""
+        return None
+
+    def _order(self, HP: int, WP: int, device):
+        """(index table, inverse) as int32 device tensors, or None for raster order."""
+        idx = self._scan_indices(HP, WP)
+        if idx is None:
+            return None
+        key = ("order", str(device), HP, WP)
+        if key not in self._consts:
+            import numpy as np
+            inv = np.empty_like(idx)
+            inv[idx] = np.arange(len(idx))
+            self._consts[key] = tuple(torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(device)
+                                      for a in (idx, inv))
+        return self._consts[key]
 
     def layout(self) -> ParamLayout:
         if self.context_dim not in self._layouts:
@@ -145,19 +186,22 @@ class SimpleDiT:
         gen = torch.Generator(device=device)
         gen.manual_seed(utils.key_to_seed(tuple(key)))
         for name, t in fp.named.items():
-            leaf = name.rsplit('/', 1)[1]
-            if leaf == "scale":
-                t.fill_(1.0)
-            elif leaf == "kernel" and not name.startswith("final_proj") and "ada_proj" not in name:
-                if name.endswith("to_out_0/kernel"):
-                    fan_in = t.shape[0] * t.shape[1]
-                elif t.dim() == 4:
-                    fan_in = t.shape[0] * t.shape[1] * t.shape[2]
-                else:
-                    fan_in = t.shape[0]
-                std = math.sqrt(1.0 / fan_in) / 0.87962566103423978
-                torch.nn.init.trunc_normal_(t, mean=0.0, std=std, a=-2 * std, b=2 * std, generator=gen)
+            self._init_leaf(name, t, gen)
         return fp
+
+    def _init_leaf(self, name: str, t: torch.Tensor, gen: torch.Generator) -> None:
+        """Fills one zero-initialised leaf (biases stay zero)."""
+        leaf = name.rsplit('/', 1)[1]
+        if leaf == "scale":
+            t.fill_(1.0)
+        elif leaf == "kernel" and not name.startswith("final_proj") and "ada_proj" not in name:
+            if name.endswith("to_out_0/kernel"):
+                fan_in = t.shape[0] * t.shape[1]
+            elif t.dim() == 4:
+                fan_in = t.shape[0] * t.shape[1] * t.shape[2]
+            else:
+                fan_in = t.shape[0]
+            _lecun_normal(t, fan_in, gen)
 
     def _const(self, kind: str, device, *shape) -> torch.Tensor:
         key = (kind, str(device)) + shape
@@ -165,8 +209,12 @@ class SimpleDiT:
             if kind == "freqs":   # FourierEmbedding.freqs: normal(PRNGKey(42), (F//2,)) * 16 (common.py:101-102)
                 f = utils.normal(utils.PRNGKey(42), self.emb_features // 2) * 16.0
                 self._consts[key] = torch.from_numpy(f.astype("float32")).to(device)
-            else:                 # the 2-D sin-cos position table, bf16 [L, F]
-                self._consts[key] = torch.from_numpy(sincos_2d_table(self.emb_features, *shape)).to(device, BF16)
+            else:                 # the 2-D sin-cos position table, bf16 [L, F], in the patch order
+                tab = sincos_2d_table(self.emb_features, *shape)
+                idx = self._scan_indices(*shape)
+                if idx is not None:
+                    tab = tab[idx]
+                self._consts[key] = torch.from_numpy(tab).to(device, BF16)
         return self._consts[key]
 
     def _fourier_freqs(self, device) -> torch.Tensor:
@@ -237,15 +285,20 @@ class SimpleDiT:
         K = p * p * C
         Kp = _round_up(K, 32)
         rows = ops.dit_patchify(x, p, Kp)
-        wpe = torch.nn.functional.pad(W16["patch_embed/Conv_0/kernel"].reshape(K, F), (0, 0, 0, Kp - K))
+        order = self._order(HP, WP, dev)
+        if order is not None:
+            rows = ops.permute_rows(rows, order[0])
+        emb = self._embed_name()
+        wpe = torch.nn.functional.pad(W16[emb + "/kernel"].reshape(K, F), (0, 0, 0, Kp - K))
         tok = torch.empty((M, F), dtype=BF16, device=dev)
         ops.gemm(ops.GEMM_KMN, rows, wpe, tok, L, F, Kp, Kp, F, F, batch1=B, a_s=(L * Kp, 0), d_s=(L * F, 0),
-                 bias=W32["patch_embed/Conv_0/bias"], res=self._const("pos", dev, HP, WP), r_ld=F, r_s=(0, 0))
+                 bias=W32[emb + "/bias"], res=self._const("pos", dev, HP, WP), r_ld=F, r_s=(0, 0))
         sv["patch_rows"] = rows
+        sv["order"] = order
 
         blocks = []
-        for i in range(self.num_layers):
-            tok, rec = self._block_fwd(f"dit_block_{i}", tok, cond16, W32, W16, B, L)
+        for n, fwd, _ in self._blocks():
+            tok, rec = fwd(n, tok, cond16, W32, W16, B, L)
             blocks.append(rec)
         sv["blocks"] = blocks
 
@@ -256,11 +309,19 @@ class SimpleDiT:
         wfp = torch.nn.functional.pad(W16["final_proj/kernel"][:, :P_], (0, Np - P_)).contiguous()
         bfp = torch.nn.functional.pad(W32["final_proj/bias"][:P_], (0, Np - P_)).contiguous()
         yf = ops.linear_fwd(xf, wfp, bias=bfp, out_dtype=F32)
+        if order is not None:
+            yf = ops.permute_rows(yf, order[1])
         out = ops.dit_unpatchify(yf, B, H, W, self.output_channels, p)
         if not save:
             return out, None
         sv.update(final=(tok, mf, rf, xf, wfp))
         return out, sv
+
+    def _rope(self) -> bool:
+        """RoPE in the attention blocks: off under the Hilbert / zigzag orders, where the reference sets cos = 1,
+        sin = 0 (ssm_dit.py:750-759).  The head channels [d, dp) stay zero without it: the QKV kernel and bias are
+        zero-padded there."""
+        return not (self.use_hilbert or self.use_zigzag)
 
     def _qkv_weights(self, n, W32, W16):
         """The fused QKV kernel [F, 3*heads*dp] bf16 and bias f32, heads zero-padded to the attention width dp."""
@@ -283,26 +344,36 @@ class SimpleDiT:
         dp = _attn_width(d)
         HD = heads * dp
         M = x.shape[0]
-        ada = ops.linear_fwd(cond16, W16[f"{n}/ada_params_module/ada_proj/kernel"],
-                             bias=W32[f"{n}/ada_params_module/ada_proj/bias"], out_dtype=F32)
+        ada = self._ada_fwd(n, cond16, W32, W16)
         n1, m1, r1 = ops.dit_adaln_fwd(x, L, ada, 3 * F, 4 * F, eps=eps)
         wqkv, bqkv, wo = self._qkv_weights(n, W32, W16)
         qkv = ops.linear_fwd(n1, wqkv, bias=bqkv)
         del n1
-        ops.dit_rope(qkv, L, heads, d, dp, nmat=2, mat_off=HD)
+        if self._rope():
+            ops.dit_rope(qkv, L, heads, d, dp, nmat=2, mat_off=HD)
         q3 = qkv.view(B, L, 3 * HD)
         q, k, v = q3[..., :HD], q3[..., HD:2 * HD], q3[..., 2 * HD:]
         o, lse = ops.attention_fwd(q, k, v, heads, dp, d ** -0.5)
         ya = ops.linear_fwd(o.view(M, HD), wo, bias=W32[f"{n}/attention/to_out_0/bias"])
         x1 = ops.dit_gate_fwd(x, ya, L, ada[:, 5 * F:])
-        n2, m2, r2 = ops.dit_adaln_fwd(x1, L, ada, 0, F, eps=eps)
+        x2, mlp = self._mlp_fwd(n, x1, ada, W32, W16, L)
+        return x2, (n, x, ada, m1, r1, qkv, o, lse, ya, x1, mlp, (wqkv, wo))
+
+    def _ada_fwd(self, n, cond16, W32, W16):
+        return ops.linear_fwd(cond16, W16[f"{n}/ada_params_module/ada_proj/kernel"],
+                              bias=W32[f"{n}/ada_params_module/ada_proj/bias"], out_dtype=F32)
+
+    def _mlp_fwd(self, n, x1, ada, W32, W16, L):
+        """The MLP half of a block: x2 = x1 + gate_mlp * (gelu(adaLN(x1) W0 + b0) W2 + b2)."""
+        F = self.emb_features
+        n2, m2, r2 = ops.dit_adaln_fwd(x1, L, ada, 0, F, eps=self.norm_epsilon)
         u = ops.linear_fwd(n2, W16[f"{n}/mlp/layers_0/kernel"], bias=W32[f"{n}/mlp/layers_0/bias"])
         del n2
         g = ops.bias_act(u, None, ACT_GELU_TANH)
         ym = ops.linear_fwd(g, W16[f"{n}/mlp/layers_2/kernel"], bias=W32[f"{n}/mlp/layers_2/bias"])
         del g
         x2 = ops.dit_gate_fwd(x1, ym, L, ada[:, 2 * F:3 * F])
-        return x2, (n, x, ada, m1, r1, qkv, o, lse, ya, x1, m2, r2, u, ym, (wqkv, wo))
+        return x2, (m2, r2, u, ym)
 
     # ------------------------------------------------------------------ backward program
     def backward(self, fp: FlatParams, saved: dict, dF: torch.Tensor, grads: FlatParams, on_ready=None):
@@ -321,6 +392,8 @@ class SimpleDiT:
         P_ = p * p * self.output_channels
         Np = wfp.shape[1]
         dY = ops.dit_patchify(dF.contiguous(), p, Np)
+        if saved["order"] is not None:
+            dY = ops.permute_rows(dY, saved["order"][0])
         gw = torch.zeros((F, Np), dtype=F32, device=dev)
         ops.gemm(GEMM_MNMN, xf, dY, gw, F, Np, xf.shape[0], F, Np, Np, atomic=True, reduce_batch=True)
         Gd["final_proj/kernel"][:, :P_].add_(gw[:, :P_])
@@ -335,18 +408,19 @@ class SimpleDiT:
 
         dcond = torch.zeros((B, F), dtype=F32, device=dev)
         four, u1, h1, u2, h2, ctxm16, cond16 = saved["temb"]
-        for rec in reversed(saved["blocks"]):
-            dx = self._block_bwd(rec, dx, cond16, dcond, W32, W16, Gd, B, L)
+        for (n, _, bwd), rec in zip(reversed(self._blocks()), reversed(saved["blocks"])):
+            dx = bwd(rec, dx, cond16, dcond, W32, W16, Gd, B, L)
             if on_ready is not None:
-                on_ready(lay.table[f"{rec[0]}/ada_params_module/ada_proj/kernel"][0], stream)
+                on_ready(lay.table[f"{n}/ada_params_module/ada_proj/kernel"][0], stream)
 
         # patch embedding: weight and bias gradients only (the image needs none)
         rows = saved["patch_rows"]
         K, Kp = p * p * 3, rows.shape[1]
         gpe = torch.zeros((Kp, F), dtype=F32, device=dev)
         ops.gemm(GEMM_MNMN, rows, dx, gpe, Kp, F, rows.shape[0], Kp, F, F, atomic=True, reduce_batch=True)
-        Gd["patch_embed/Conv_0/kernel"].view(K, F).add_(gpe[:K])
-        ops.colsum_rows(dx, Gd["patch_embed/Conv_0/bias"])
+        emb = self._embed_name()
+        Gd[emb + "/kernel"].view(K, F).add_(gpe[:K])
+        ops.colsum_rows(dx, Gd[emb + "/bias"])
 
         # conditioning: Dense(F) <- TimeProjection <- Fourier, and text_context_proj
         te = "time_embed/layers_"
@@ -368,30 +442,14 @@ class SimpleDiT:
             on_ready(0, stream)
 
     def _block_bwd(self, rec, dx2, cond16, dcond, W32, W16, Gd, B, L):
-        n, x, ada, m1, r1, qkv, o, lse, ya, x1, m2, r2, u, ym, (wqkv, wo) = rec
+        n, x, ada, m1, r1, qkv, o, lse, ya, x1, mlp, (wqkv, wo) = rec
         F, heads, eps = self.emb_features, self.num_heads, self.norm_epsilon
         d = F // heads
         dp = _attn_width(d)
         HD = heads * dp
         M = x.shape[0]
         dada = torch.empty((B, 6 * F), dtype=F32, device=x.device)
-        # MLP branch: x2 = x1 + gate_mlp * (gelu(n2 W0 + b0) W2 + b2)
-        dym = ops.dit_gate_bwd(dx2, ym, L, ada[:, 2 * F:3 * F], dada[:, 2 * F:3 * F])
-        g = ops.bias_act(u, None, ACT_GELU_TANH)
-        _dense_wgrad(Gd[f"{n}/mlp/layers_2/kernel"], g, dym)
-        ops.colsum_rows(dym, Gd[f"{n}/mlp/layers_2/bias"])
-        del g
-        dg = _dense_dgrad(dym, W16[f"{n}/mlp/layers_2/kernel"])
-        du = ops.bias_act_bwd(u, None, ACT_GELU_TANH, dg)
-        del dg
-        n2, _, _ = ops.dit_adaln_fwd(x1, L, ada, 0, F, eps=eps, stats=False)
-        _dense_wgrad(Gd[f"{n}/mlp/layers_0/kernel"], n2, du)
-        ops.colsum_rows(du, Gd[f"{n}/mlp/layers_0/bias"])
-        del n2
-        dn2 = _dense_dgrad(du, W16[f"{n}/mlp/layers_0/kernel"])
-        del du
-        dx1 = ops.dit_adaln_bwd(x1, dn2, L, m2, r2, dada[:, 0:F], dada[:, F:2 * F], ada=ada, scale_off=0, addend=dx2)
-        del dn2
+        dx1 = self._mlp_bwd(n, dx2, x1, ada, mlp, dada, W16, Gd, L)
         # attention branch: x1 = x + gate_attn * (attn(rope(n1 Wq + bq), rope(n1 Wk + bk), n1 Wv + bv) Wo + bo)
         dya = ops.dit_gate_bwd(dx1, ya, L, ada[:, 5 * F:], dada[:, 5 * F:])
         _dense_wgrad(Gd[f"{n}/attention/to_out_0/kernel"], o.view(M, HD), dya, 1, dp)
@@ -403,8 +461,9 @@ class SimpleDiT:
                                        d ** -0.5)
         del do
         dq2, dk2, dv2 = dq.view(M, HD), dk.view(M, HD), dv.view(M, HD)
-        ops.dit_rope(dq2, L, heads, d, dp, inverse=True)
-        ops.dit_rope(dk2, L, heads, d, dp, inverse=True)
+        if self._rope():
+            ops.dit_rope(dq2, L, heads, d, dp, inverse=True)
+            ops.dit_rope(dk2, L, heads, d, dp, inverse=True)
         n1, _, _ = ops.dit_adaln_fwd(x, L, ada, 3 * F, 4 * F, eps=eps, stats=False)
         bt = torch.empty(HD, dtype=F32, device=x.device)
         dn1 = None
@@ -420,10 +479,34 @@ class SimpleDiT:
         del n1, dq, dk, dv
         dx0 = ops.dit_adaln_bwd(x, dn1, L, m1, r1, dada[:, 3 * F:4 * F], dada[:, 4 * F:5 * F], ada=ada,
                                 scale_off=3 * F, addend=dx1)
-        # ada_proj: ada = cond W + b
+        self._ada_bwd(n, dada, cond16, dcond, Gd, W16)
+        return dx0
+
+    def _mlp_bwd(self, n, dx2, x1, ada, mlp, dada, W16, Gd, L):
+        """Backward of _mlp_fwd: -> dx1; writes the gate_mlp / scale_mlp / shift_mlp chunks of dada."""
+        m2, r2, u, ym = mlp
+        F, eps = self.emb_features, self.norm_epsilon
+        dym = ops.dit_gate_bwd(dx2, ym, L, ada[:, 2 * F:3 * F], dada[:, 2 * F:3 * F])
+        g = ops.bias_act(u, None, ACT_GELU_TANH)
+        _dense_wgrad(Gd[f"{n}/mlp/layers_2/kernel"], g, dym)
+        ops.colsum_rows(dym, Gd[f"{n}/mlp/layers_2/bias"])
+        del g
+        dg = _dense_dgrad(dym, W16[f"{n}/mlp/layers_2/kernel"])
+        du = ops.bias_act_bwd(u, None, ACT_GELU_TANH, dg)
+        del dg
+        n2, _, _ = ops.dit_adaln_fwd(x1, L, ada, 0, F, eps=eps, stats=False)
+        _dense_wgrad(Gd[f"{n}/mlp/layers_0/kernel"], n2, du)
+        ops.colsum_rows(du, Gd[f"{n}/mlp/layers_0/bias"])
+        del n2
+        dn2 = _dense_dgrad(du, W16[f"{n}/mlp/layers_0/kernel"])
+        del du
+        return ops.dit_adaln_bwd(x1, dn2, L, m2, r2, dada[:, 0:F], dada[:, F:2 * F], ada=ada, scale_off=0, addend=dx2)
+
+    def _ada_bwd(self, n, dada, cond16, dcond, Gd, W16):
+        """ada = cond W + b: the kernel and bias gradients, and dcond += dada W^T."""
+        F = self.emb_features
         dada16 = ops.cast_f32_bf16(dada)
         _dense_wgrad(Gd[f"{n}/ada_params_module/ada_proj/kernel"], cond16, dada16)
         ops.colsum_rows(dada16, Gd[f"{n}/ada_params_module/ada_proj/bias"])
-        ops.gemm(GEMM_KK, dada16, W16[f"{n}/ada_params_module/ada_proj/kernel"], dcond, B, F, 6 * F, 6 * F, 6 * F, F,
-                 atomic=True)
-        return dx0
+        ops.gemm(GEMM_KK, dada16, W16[f"{n}/ada_params_module/ada_proj/kernel"], dcond, dada.shape[0], F, 6 * F,
+                 6 * F, 6 * F, F, atomic=True)

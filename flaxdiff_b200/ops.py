@@ -982,6 +982,80 @@ def dit_fourier(t: torch.Tensor, freqs: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# --------------------------------------------------------------------------- S5 state-space layer
+def ssm_chunk(B: int, L: int, S: int, device) -> int:
+    """Tokens per scan chunk: enough (sample, chunk, state) threads to fill every SM twice, chunks of >= 8 tokens."""
+    sms = torch.cuda.get_device_properties(device).multi_processor_count
+    nchunk = max(1, min(-(-L // 8), -(-2048 * sms // (B * S))))
+    return -(-L // nchunk)
+
+
+def ssm_discretize(P: dict, N: int, F: int, wb: torch.Tensor, col0: int, wc: torch.Tensor, adt: torch.Tensor):
+    """One direction's discretisation from its f32 leaves P (log_A_real, A_imag, log_dt, B_re, B_im, C_re, C_im):
+    writes Bbar^T into columns [col0, col0 + 2N) of wb bf16 [F, ldb], wc bf16 [2N, F] and adt[col0:col0 + 2N]."""
+    assert wb.dtype == wc.dtype == torch.bfloat16 and wb.is_contiguous() and wc.is_contiguous()
+    assert tuple(wc.shape) == (2 * N, F) and wb.shape[0] == F and adt.dtype == torch.float32
+    check(load().fdx_ssm_discretize(ptr(P["log_A_real"]), ptr(P["A_imag"]), ptr(P["log_dt"]), ptr(P["B_re"]),
+                                    ptr(P["B_im"]), ptr(P["C_re"]), ptr(P["C_im"]), N, F, ptr(wb), wb.shape[1], col0,
+                                    ptr(wc), ptr(adt), stream_ptr()), "ssm_discretize")
+
+
+def ssm_discretize_bwd(P: dict, G: dict, N: int, F: int, dwb: torch.Tensor, col0: int, dwc: torch.Tensor,
+                       dabar: torch.Tensor, dgbar: torch.Tensor):
+    """Accumulates one direction's parameter gradients into G (the same leaf names as P) from dwb f32 [>= col0 + 2N, F],
+    dwc f32 [2N, F] and the adjoint scan's partial sums dabar / dgbar f32 [parts, ld]."""
+    assert dwb.dtype == dwc.dtype == dabar.dtype == dgbar.dtype == torch.float32 and dgbar.shape == dabar.shape
+    assert dwb.is_contiguous() and dwc.is_contiguous() and dabar.is_contiguous() and dgbar.is_contiguous()
+    assert dwb.shape[1] == F
+    check(load().fdx_ssm_discretize_bwd(ptr(P["log_A_real"]), ptr(P["A_imag"]), ptr(P["log_dt"]), ptr(P["B_re"]),
+                                        ptr(P["B_im"]), N, F, ptr(dwb), col0, ptr(dwc), ptr(dabar), ptr(dgbar),
+                                        dabar.shape[0],
+                                        dabar.shape[1], ptr(G["log_A_real"]), ptr(G["A_imag"]), ptr(G["log_dt"]),
+                                        ptr(G["B_re"]), ptr(G["B_im"]), ptr(G["C_re"]), ptr(G["C_im"]), stream_ptr()),
+          "ssm_discretize_bwd")
+
+
+def ssm_scan(bu: torch.Tensor, adt: torch.Tensor, B: int, N: int, ndir: int, chunk: int, out=None):
+    """bu f32 [B*L, 2*ndir*N] -> (states f32 (into `out`, which may be bu), their bf16 copy)."""
+    rows, S2 = bu.shape
+    assert bu.dtype == torch.float32 and bu.is_contiguous() and S2 == 2 * ndir * N and rows % B == 0
+    L = rows // B
+    x = torch.empty_like(bu) if out is None else out
+    assert x.shape == bu.shape and x.dtype == torch.float32 and x.is_contiguous()
+    x16 = torch.empty((rows, S2), dtype=torch.bfloat16, device=bu.device)
+    ws = torch.empty(B * -(-L // chunk) * S2, dtype=torch.float32, device=bu.device)
+    check(load().fdx_ssm_scan(ptr(bu), ptr(x), ptr(x16), ptr(adt), B, L, N, ndir, chunk, ptr(ws), stream_ptr()),
+          "ssm_scan")
+    return x, x16
+
+
+def ssm_scan_bwd(dx: torch.Tensor, x: torch.Tensor, bu: torch.Tensor, adt: torch.Tensor, B: int, N: int, ndir: int,
+                 chunk: int):
+    """-> (lambda bf16 [B*L, 2*ndir*N], partial sums f32 [B*nchunk, 2*ndir*N] of lambda conj(x_prev) = d(Abar) and of
+    lambda conj(bu))."""
+    rows, S2 = dx.shape
+    assert dx.dtype == x.dtype == bu.dtype == torch.float32 and x.shape == dx.shape == bu.shape
+    assert dx.is_contiguous() and x.is_contiguous() and bu.is_contiguous()
+    L = rows // B
+    nch = -(-L // chunk)
+    lam = torch.empty((rows, S2), dtype=torch.bfloat16, device=dx.device)
+    ws = torch.empty(B * nch * S2, dtype=torch.float32, device=dx.device)
+    dab = torch.empty((B * nch, S2), dtype=torch.float32, device=dx.device)
+    dgb = torch.empty_like(dab)
+    check(load().fdx_ssm_scan_bwd(ptr(dx), ptr(x), ptr(bu), ptr(adt), B, L, N, ndir, chunk, ptr(ws), ptr(lam),
+                                  ptr(dab), ptr(dgb), stream_ptr()), "ssm_scan_bwd")
+    return lam, dab, dgb
+
+
+def permute_rows(src: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
+    """dst[b*L + i] = src[b*L + idx[i]] over the rows of a contiguous 2-D tensor (L = len(idx), int32 on the device)."""
+    assert src.dim() == 2 and src.is_contiguous() and idx.dtype == torch.int32 and idx.is_contiguous()
+    dst = torch.empty_like(src)
+    check(load().fdx_permute_rows(ptr(src), ptr(dst), src.shape[0], idx.numel(), src.shape[1] * src.element_size(),
+                                  ptr(idx), stream_ptr()), "permute_rows")
+    return dst
+
+
 # --------------------------------------------------------------------------- CLIP metrics
 def clip_image_prep(x: torch.Tensor, tables: torch.Tensor, ksize_y: int, ksize_x: int, lut: torch.Tensor, crop: int,
                     patch: int, ld: int, u8_out: Optional[torch.Tensor] = None) -> torch.Tensor:

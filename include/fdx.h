@@ -473,6 +473,44 @@ int fdx_dit_patchify(const void* src, int src_f32, int B, int H, int W, int C, i
 int fdx_dit_unpatchify(const float* src, int ld, int B, int H, int W, int C, int p, float* dst, void* stream);
 int fdx_dit_fourier(const float* t, int B, const float* freqs, int half, void* out_bf16, void* stream);
 
+/* ---- S5 state-space layer (fdx_ssm.cu): flaxdiff/models/ssm_dit.py:58-286, hilbert.py:87-370 -----------------------
+ * One S5 layer has ndir (1, or 2 when bidirectional) directions of N complex states over F features.  Its per-token
+ * complex values (Bu, the states x, their gradients) are f32 or bf16 rows of 2 * ndir * N columns: direction d owns
+ * [2dN, 2dN + 2N), real parts at 2dN + n, imaginary parts at 2dN + N + n.  The dense products run on fdx_gemm.
+ *   fdx_ssm_discretize     : ZOH discretisation of one direction (ssm_dit.py:154-169): dt = exp(log_dt),
+ *                            A = -exp(log_a_real) + i a_imag, Abar = exp(A dt), Bbar = (Abar - 1) / (A + 1e-8) B.
+ *                            Writes wb[f][col0 + n] = Re Bbar[n][f] and wb[f][col0 + N + n] = Im Bbar[n][f] (bf16, rows
+ *                            of ldb: both directions' Bu = u Bbar^T as one product), wc = [C_re^T; -C_im^T] bf16 [2N][F]
+ *                            (y = Re(C x) = x_cols wc) and adt[col0 + n] = Re(A dt), adt[col0 + N + n] = Im(A dt) / pi.
+ *   fdx_ssm_scan           : bu f32 [B * L][2 ndir N] -> states x f32 (x may alias bu), x_k = Abar x_{k-1} + bu_k,
+ *                            direction 0 from token 0, direction 1 from token L - 1 (the states sit at their tokens);
+ *                            x_bf16 receives a bf16 copy.  Sequence-parallel over chunks of `chunk` tokens; ws f32
+ *                            [B][nchunk][2 ndir N].
+ *   fdx_ssm_scan_bwd       : the adjoint lambda_k = dx_k + conj(Abar) lambda_{k+1} (in each direction's step order) from
+ *                            dx f32, the saved f32 states x and bu: lambda -> lam_bf16, and per (sample, chunk) partial
+ *                            sums of lambda_k conj(x_{k-1}) -> dabar and of lambda_k conj(bu_k) -> dgbar (f32
+ *                            [B][nchunk][2 ndir N]).  ws as fdx_ssm_scan's.
+ *   fdx_ssm_discretize_bwd : for one direction, from dwb = d(Bbar) f32 rows [col0 + n] (real) / [col0 + N + n] (imag)
+ *                            of F, dwc = d(wc) f32 [2N][F] and the nparts rows of dabar / dgbar (ld_part floats apart):
+ *                            accumulates (+=) the gradients of log_a_real, a_imag, log_dt, B_re, B_im, C_re and C_im.
+ *                            Complex gradients follow d = d/dRe + i d/dIm.  Fixed-order sums, no atomics.
+ *   fdx_permute_rows       : dst[b * L + i] = src[b * L + idx[i]] over rows of row_bytes (a multiple of 16): the
+ *                            Hilbert / zigzag patch order and its inverse. */
+int fdx_ssm_discretize(const float* log_a_real, const float* a_imag, const float* log_dt, const float* b_re,
+                       const float* b_im, const float* c_re, const float* c_im, int N, int F, void* wb_bf16, int ldb,
+                       int col0, void* wc_bf16, float* adt, void* stream);
+int fdx_ssm_discretize_bwd(const float* log_a_real, const float* a_imag, const float* log_dt, const float* b_re,
+                           const float* b_im, int N, int F, const float* dwb, int col0, const float* dwc,
+                           const float* dabar, const float* dgbar, int nparts, int ld_part, float* g_log_a_real,
+                           float* g_a_imag, float* g_log_dt, float* g_b_re, float* g_b_im, float* g_c_re,
+                           float* g_c_im, void* stream);
+int fdx_ssm_scan(const float* bu, float* x, void* x_bf16, const float* adt, int B, int L, int N, int ndir, int chunk,
+                 float* ws, void* stream);
+int fdx_ssm_scan_bwd(const float* dx, const float* x, const float* bu, const float* adt, int B, int L, int N, int ndir,
+                     int chunk, float* ws, void* lam_bf16, float* dabar, float* dgbar, void* stream);
+int fdx_permute_rows(const void* src, void* dst, long long rows, int L, long long row_bytes, const int32_t* idx,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif
