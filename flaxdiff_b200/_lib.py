@@ -114,6 +114,12 @@ def _declare(lib) -> None:
     lib.fdx_ssm_scan.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp]
     lib.fdx_ssm_scan_bwd.argtypes = [vp, vp, vp, vp, i, i, i, i, i, vp, vp, vp, vp, vp]
     lib.fdx_permute_rows.argtypes = [vp, vp, ll, i, ll, vp, vp]
+    lib.fdx_mmdit_adaln_fwd.argtypes = [vp, ll, i, i, vp, ll, f, vp, vp, vp, vp, vp]
+    lib.fdx_mmdit_adaln_bwd.argtypes = [vp, vp, vp, ll, i, i, vp, ll, vp, vp, vp, vp, vp, i, vp, ll, vp]
+    lib.fdx_mmdit_gate_fwd.argtypes = [vp, vp, vp, ll, i, i, vp, ll, vp, vp]
+    lib.fdx_mmdit_gate_bwd.argtypes = [vp, vp, vp, ll, i, i, vp, ll, vp, vp, vp, i, vp, ll, vp]
+    lib.fdx_layernorm_rows_fwd.argtypes = [i, vp, vp, ll, i, i, i, i, vp, vp, f, vp, vp, vp, vp]
+    lib.fdx_layernorm_rows_bwd.argtypes = [i, vp, vp, vp, ll, i, i, i, i, vp, vp, vp, vp, i, vp, i, vp, i, vp, vp, vp]
 
 
 _lib: Optional[ctypes.CDLL] = None

@@ -982,6 +982,119 @@ def dit_fourier(t: torch.Tensor, freqs: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# --------------------------------------------------------------------------- SimpleMMDiT streaming kernels
+def _ada_rows(ada: torch.Tensor, C: int, name: str):
+    assert ada.dtype == torch.float32 and ada.dim() == 2 and ada.stride(1) == 1 and ada.shape[1] >= 6 * C, name
+    return ada.stride(0)
+
+
+def mmdit_adaln_fwd(x: torch.Tensor, L: int, ada: torch.Tensor, eps: float = 1e-5, stats: bool = True):
+    """One LayerNorm of the token rows x [B*L, C], modulated twice by the ada rows f32 [B, 6C] -> (y_attn bf16,
+    y_mlp bf16 (clipped mlp chunks), mean f32 [rows] or None, rstd or None)."""
+    rows, C = _tokens(x, "x")
+    ya = torch.empty((rows, C), dtype=torch.bfloat16, device=x.device)
+    ym = torch.empty_like(ya)
+    mean = torch.empty(rows, dtype=torch.float32, device=x.device) if stats else None
+    rstd = torch.empty_like(mean) if stats else None
+    check(load().fdx_mmdit_adaln_fwd(ptr(x), rows, L, C, ptr(ada), _ada_rows(ada, C, "ada"), eps, ptr(ya), ptr(ym),
+                                     ptr(mean), ptr(rstd), stream_ptr()), "mmdit_adaln_fwd")
+    return ya, ym, mean, rstd
+
+
+def mmdit_adaln_bwd(x, dya, dym, L: int, ada: torch.Tensor, mean, rstd, dada: torch.Tensor, addend=None, out=None):
+    """Backward of mmdit_adaln_fwd -> dx bf16 [rows, C] (+ addend); writes the scale / shift chunks of both
+    modulations into dada f32 [B, 6C]."""
+    rows, C = _tokens(x, "x")
+    _tokens(dya, "dy_attn")
+    _tokens(dym, "dy_mlp")
+    B = rows // L
+    dx = out if out is not None else torch.empty((rows, C), dtype=torch.bfloat16, device=x.device)
+    nch = _dit_chunks(B, L, C, x.device)
+    ws = torch.empty(B * nch * 4 * C, dtype=torch.float32, device=x.device)
+    check(load().fdx_mmdit_adaln_bwd(ptr(x), ptr(dya), ptr(dym), rows, L, C, ptr(ada), _ada_rows(ada, C, "ada"),
+                                     ptr(mean), ptr(rstd), ptr(addend), ptr(dx), ptr(ws), nch, ptr(dada),
+                                     _ada_rows(dada, C, "dada"), stream_ptr()), "mmdit_adaln_bwd")
+    return dx
+
+
+def mmdit_gate_fwd(x: torch.Tensor, ya: torch.Tensor, ym: torch.Tensor, L: int, ada: torch.Tensor,
+                   out=None) -> torch.Tensor:
+    """x + gate_attn[b] * ya + gate_mlp[b] * ym over token rows [B*L, C] (out may be x)."""
+    rows, C = _tokens(x, "x")
+    _tokens(ya, "y_attn")
+    _tokens(ym, "y_mlp")
+    out = out if out is not None else torch.empty((rows, C), dtype=torch.bfloat16, device=x.device)
+    check(load().fdx_mmdit_gate_fwd(ptr(x), ptr(ya), ptr(ym), rows, L, C, ptr(ada), _ada_rows(ada, C, "ada"),
+                                    ptr(out), stream_ptr()), "mmdit_gate_fwd")
+    return out
+
+
+def mmdit_gate_bwd(dout: torch.Tensor, ya: torch.Tensor, ym: torch.Tensor, L: int, ada: torch.Tensor,
+                   dada: torch.Tensor):
+    """-> (dy_attn = gate_attn[b] * dout, dy_mlp = gate_mlp[b] * dout); writes the gate chunks of dada f32 [B, 6C]
+    (the sample's sums of dout * ya and dout * ym)."""
+    rows, C = _tokens(dout, "dout")
+    _tokens(ya, "y_attn")
+    _tokens(ym, "y_mlp")
+    B = rows // L
+    dya = torch.empty((rows, C), dtype=torch.bfloat16, device=dout.device)
+    dym = torch.empty_like(dya)
+    nch = _dit_chunks(B, L, C, dout.device)
+    ws = torch.empty(B * nch * 2 * C, dtype=torch.float32, device=dout.device)
+    check(load().fdx_mmdit_gate_bwd(ptr(dout), ptr(ya), ptr(ym), rows, L, C, ptr(ada), _ada_rows(ada, C, "ada"),
+                                    ptr(dya), ptr(dym), ptr(ws), nch, ptr(dada), _ada_rows(dada, C, "dada"),
+                                    stream_ptr()), "mmdit_gate_bwd")
+    return dya, dym
+
+
+LN_GATHER, LN_CONCAT, LN_SCATTER = 0, 1, 2       # fdx_layernorm_rows modes
+
+
+def layernorm_rows_fwd(mode: int, src0: torch.Tensor, src1: Optional[torch.Tensor], rows: int, C: int,
+                       gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5, grid=(0, 0)):
+    """Affine LayerNorm over logical rows of C columns assembled by `mode` (fdx_layernorm_rows_fwd):
+    LN_GATHER - the 2x2 merge of src0's fine rows over the coarse grid `grid` = (HPc, WPc) -> y bf16 [rows, C];
+    LN_CONCAT - [src0, src1] -> y bf16 [rows, C]; LN_SCATTER - src0 [rows, C] -> y bf16 fine rows [4 rows, C / 4].
+    -> (y, mean f32 [rows], rstd)."""
+    for t in (src0, src1):
+        assert t is None or (t.dtype == torch.bfloat16 and t.is_contiguous())
+    assert gamma.dtype == beta.dtype == torch.float32 and gamma.numel() == C
+    C0 = src0.shape[-1] if mode == LN_CONCAT else 0
+    shape = (4 * rows, C // 4) if mode == LN_SCATTER else (rows, C)
+    y = torch.empty(shape, dtype=torch.bfloat16, device=src0.device)
+    mean = torch.empty(rows, dtype=torch.float32, device=src0.device)
+    rstd = torch.empty_like(mean)
+    check(load().fdx_layernorm_rows_fwd(mode, ptr(src0), ptr(src1), rows, C, C0, grid[0], grid[1], ptr(gamma),
+                                        ptr(beta), eps, ptr(y), ptr(mean), ptr(rstd), stream_ptr()),
+          "layernorm_rows_fwd")
+    return y, mean, rstd
+
+
+def layernorm_rows_bwd(mode: int, src0, src1, dy: torch.Tensor, rows: int, C: int, gamma, mean, rstd,
+                       dgamma: torch.Tensor, dbeta: torch.Tensor, grid=(0, 0), dx0=None, dx1=None,
+                       accumulate0: bool = False, accumulate1: bool = False):
+    """Backward of layernorm_rows_fwd: dx into dx0 (src0's layout) and, LN_CONCAT, dx1 (src1's), each overwritten or
+    added to; dgamma / dbeta f32 [C] += the sums over all rows.  Missing destinations are allocated. -> (dx0, dx1)."""
+    assert dy.dtype == torch.bfloat16 and dy.is_contiguous()
+    if dx0 is None:
+        assert not accumulate0
+        dx0 = torch.empty_like(src0)
+    if mode == LN_CONCAT and dx1 is None:
+        assert not accumulate1
+        dx1 = torch.empty_like(src1)
+    for t, like in ((dx0, src0), (dx1, src1)):
+        assert t is None or (t.dtype == torch.bfloat16 and t.is_contiguous() and t.shape == like.shape)
+    C0 = src0.shape[-1] if mode == LN_CONCAT else 0
+    sms = torch.cuda.get_device_properties(dy.device).multi_processor_count
+    nch = max(1, min(rows, 2 * sms))
+    ws = torch.empty(nch * 2 * C, dtype=torch.float32, device=dy.device)
+    check(load().fdx_layernorm_rows_bwd(mode, ptr(src0), ptr(src1), ptr(dy), rows, C, C0, grid[0], grid[1],
+                                        ptr(gamma), ptr(mean), ptr(rstd), ptr(dx0), int(accumulate0), ptr(dx1),
+                                        int(accumulate1), ptr(ws), nch, ptr(dgamma), ptr(dbeta), stream_ptr()),
+          "layernorm_rows_bwd")
+    return dx0, dx1
+
+
 # --------------------------------------------------------------------------- S5 state-space layer
 def ssm_chunk(B: int, L: int, S: int, device) -> int:
     """Tokens per scan chunk: enough (sample, chunk, state) threads to fill every SM twice, chunks of >= 8 tokens."""

@@ -511,6 +511,53 @@ int fdx_ssm_scan_bwd(const float* dx, const float* x, const float* bu, const flo
 int fdx_permute_rows(const void* src, void* dst, long long rows, int L, long long row_bytes, const int32_t* idx,
                      void* stream);
 
+/* ---- SimpleMMDiT (flaxdiff/models/simple_mmdit.py:17-331) --------------------------------------------------------
+ * The MMDiT block is a parallel block: one LayerNorm of the block input (MMAdaLNZero, :17-90) is modulated twice and
+ * both branches are added onto the same residual (MMDiTBlock, :137-158).  Token rows are bf16 [rows = B * L][C],
+ * C a multiple of 8, <= 1536 for the LayerNorm pair.  ada is the block's f32 [B][ada_ld] modulation, six C-wide chunks
+ * in the reference's split order: scale_mlp 0, shift_mlp 1, gate_mlp 2, scale_attn 3, shift_attn 4, gate_attn 5; the
+ * mlp scale and shift enter clipped to [-10, 10], the attention chunks as they are.  d_ada has the same layout.  Column
+ * sums run in two ordered stages through ws = f32 [B][nchunk][4][C]: no atomics, reproducible bit for bit.
+ *   fdx_mmdit_adaln_fwd : y_attn = xhat (1 + scale_attn) + shift_attn and y_mlp = xhat (1 + clip(scale_mlp)) +
+ *                         clip(shift_mlp) from one read of x; mean / rstd f32 [rows] written when non-NULL.
+ *   fdx_mmdit_adaln_bwd : dx = d/dx of both (+ addend; dx may alias addend) and the scale_attn, shift_attn,
+ *                         scale_mlp, shift_mlp chunks of d_ada (per-sample sums over tokens).  The clip's derivative
+ *                         is 1 inside (-10, 10), 0 outside and 1/2 at exactly -10 or 10.
+ *   fdx_mmdit_gate_fwd  : out = x + gate_attn y_attn + gate_mlp y_mlp, one rounding (out may be x).
+ *   fdx_mmdit_gate_bwd  : dy_attn = gate_attn dout, dy_mlp = gate_mlp dout, and the gate_attn / gate_mlp chunks of
+ *                         d_ada = the sample's sums of dout y_attn / dout y_mlp, in one pass over dout. */
+int fdx_mmdit_adaln_fwd(const void* x_bf16, long long rows, int L, int C, const float* ada, long long ada_ld,
+                        float eps, void* y_attn_bf16, void* y_mlp_bf16, float* mean, float* rstd, void* stream);
+int fdx_mmdit_adaln_bwd(const void* x_bf16, const void* dy_attn_bf16, const void* dy_mlp_bf16, long long rows, int L,
+                        int C, const float* ada, long long ada_ld, const float* mean, const float* rstd,
+                        const void* addend_bf16, void* dx_bf16, float* ws, int nchunk, float* d_ada,
+                        long long d_ada_ld, void* stream);
+int fdx_mmdit_gate_fwd(const void* x_bf16, const void* y_attn_bf16, const void* y_mlp_bf16, long long rows, int L,
+                       int C, const float* ada, long long ada_ld, void* out_bf16, void* stream);
+int fdx_mmdit_gate_bwd(const void* dout_bf16, const void* y_attn_bf16, const void* y_mlp_bf16, long long rows, int L,
+                       int C, const float* ada, long long ada_ld, void* dy_attn_bf16, void* dy_mlp_bf16, float* ws,
+                       int nchunk, float* d_ada, long long d_ada_ld, void* stream);
+
+/* ---- HierarchicalMMDiT (flaxdiff/models/simple_mmdit.py:336-730): affine LayerNorm over rows up to 6144 wide -------
+ * A logical row of C columns (C a multiple of 8, <= 6144; f32 statistics, mean / rstd f32 [rows]) is assembled by mode:
+ *   0 gather  (PatchMerging, :348-382): row r = coarse patch (b, h, w) of an HPc x WPc grid, columns (p1, p2, c) read
+ *             from fine row b (2HPc)(2WPc) + (2h + p1)(2WPc) + 2w + p2 of src0 [.][C/4]; y [rows][C].
+ *   1 concat  (the decoder fusion, :693-696): columns [0, C0) from src0 [rows][C0], the rest from src1; y [rows][C].
+ *   2 scatter (PatchExpanding, :396-429): src0 [rows][C]; column (p1, p2, c) goes to that fine row of y [.][C/4].
+ * The 2x2 modes need C a multiple of 32 and rows a multiple of HPc * WPc.
+ *   fdx_layernorm_rows_fwd : y = xhat * gamma + beta.
+ *   fdx_layernorm_rows_bwd : dx back through the same assembly into dx0 (gather: the fine rows; concat: the first C0
+ *                            columns; scatter: [rows][C]) and, concat, dx1; each destination is overwritten or, with
+ *                            its accumulate flag, added to.  dgamma / dbeta (+)= the sums over all rows, formed in
+ *                            nchunk row chunks (ws f32 [nchunk][2][C]) and added in chunk order: no atomics. */
+int fdx_layernorm_rows_fwd(int mode, const void* src0_bf16, const void* src1_bf16, long long rows, int C, int C0,
+                           int HPc, int WPc, const float* gamma, const float* beta, float eps, void* y_bf16,
+                           float* mean, float* rstd, void* stream);
+int fdx_layernorm_rows_bwd(int mode, const void* src0_bf16, const void* src1_bf16, const void* dy_bf16,
+                           long long rows, int C, int C0, int HPc, int WPc, const float* gamma, const float* mean,
+                           const float* rstd, void* dx0_bf16, int accumulate0, void* dx1_bf16, int accumulate1,
+                           float* ws, int nchunk, float* dgamma, float* dbeta, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
