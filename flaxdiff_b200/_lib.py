@@ -91,6 +91,7 @@ def _declare(lib) -> None:
     as Python ints (ctypes would otherwise truncate them)."""
     vp, i, ll, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
     lib.fdx_attention_fwd_masked.argtypes = [ctypes.POINTER(fdx_attn_desc), i, vp, vp]
+    lib.fdx_gemm_cat.argtypes = [ctypes.POINTER(fdx_gemm_desc), vp, ll, i, vp]
     lib.fdx_token_embed.argtypes = [vp, i, i, vp, i, vp, i, vp, vp]
     lib.fdx_layernorm_fwd.argtypes = [vp, ll, i, vp, vp, f, vp, vp]
     lib.fdx_bias_act.argtypes = [vp, ll, i, vp, i, vp, vp]

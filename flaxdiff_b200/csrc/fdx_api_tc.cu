@@ -320,13 +320,13 @@ int fdx_conv1x1_dgrad(const fdx_act* dy, const void* w_io, const fdx_act* dx, in
   return fdx_tc_launch(L, (cudaStream_t)stream);
 }
 
-int fdx_gemm(const fdx_gemm_desc* g, void* stream) {
+// fdx_gemm's launch descriptor for g (checked), shared with fdx_gemm_cat
+static int gemm_launch_desc(const fdx_gemm_desc* g, TcLaunch& L) {
   FDX_REQUIRE(g && g->A && g->B && g->D, "gemm: null pointer");
   FDX_REQUIRE(g->mode >= 0 && g->mode <= 2, "gemm: bad mode");
   FDX_REQUIRE(g->M > 0 && g->N > 0 && g->K > 0, "gemm: bad dims");
   FDX_REQUIRE(g->N % 32 == 0, "gemm: N=%d must be a multiple of 32", g->N);
   const int b1 = g->batch1 > 0 ? g->batch1 : 1, b2 = g->batch2 > 0 ? g->batch2 : 1;
-  TcLaunch L{};
   L.mode = g->mode;
   L.gemm_like = 1;
   L.es = 1;
@@ -382,6 +382,38 @@ int fdx_gemm(const fdx_gemm_desc* g, void* stream) {
     L.splits = (g->reduce_batch && g->d_atomic) ? 0 : 1;
     FDX_REQUIRE(!g->res, "gemm: residual unsupported in MNMN mode");
   }
+  return FDX_OK;
+}
+
+int fdx_gemm(const fdx_gemm_desc* g, void* stream) {
+  TcLaunch L{};
+  const int s = gemm_launch_desc(g, L);
+  if (s != FDX_OK) return s;
+  return fdx_tc_launch(L, (cudaStream_t)stream);
+}
+
+int fdx_gemm_cat(const fdx_gemm_desc* g, const void* A1, long long a1_ld, int K0, void* stream) {
+  FDX_REQUIRE(g && g->A && A1 && g->B && g->D, "gemm_cat: null pointer");
+  FDX_REQUIRE(g->mode == FDX_GEMM_KK || g->mode == FDX_GEMM_KMN,
+              "gemm_cat: mode %d: a two-source A exists in the KK and KMN modes only", g->mode);
+  FDX_REQUIRE(g->batch1 <= 1 && g->batch2 <= 1, "gemm_cat: batch %d x %d: flat row matrices only (batch 1)",
+              g->batch1, g->batch2);
+  FDX_REQUIRE(K0 > 0 && K0 < g->K && K0 % 64 == 0,
+              "gemm_cat: K0=%d must be a multiple of 64 with 0 < K0 < K=%d", K0, g->K);
+  FDX_REQUIRE(reinterpret_cast<uintptr_t>(g->A) % 16 == 0 && reinterpret_cast<uintptr_t>(A1) % 16 == 0,
+              "gemm_cat: A0 and A1 must be 16-byte aligned");
+  FDX_REQUIRE(g->a_ld >= K0 && g->a_ld % 8 == 0, "gemm_cat: a_ld=%lld must be >= K0 and a multiple of 8", g->a_ld);
+  FDX_REQUIRE(a1_ld >= g->K - K0 && a1_ld % 8 == 0, "gemm_cat: a1_ld=%lld must be >= K - K0 and a multiple of 8",
+              a1_ld);
+  TcLaunch L{};
+  const int s = gemm_launch_desc(g, L);
+  if (s != FDX_OK) return s;
+  L.A.dims[0] = K0;
+  L.A1.ptr = A1;
+  L.A1.dims[0] = g->K - K0; L.A1.dims[1] = g->M; L.A1.dims[2] = 1; L.A1.dims[3] = 1;
+  L.A1.strides[0] = 1; L.A1.strides[1] = a1_ld;
+  L.A1.strides[2] = L.A1.strides[3] = (uint64_t)a1_ld * g->M;
+  L.cat_k0 = K0;
   return fdx_tc_launch(L, (cudaStream_t)stream);
 }
 

@@ -66,6 +66,10 @@ struct TcLaunch {
   // gn_ws without gn_ab (TC_KMN only): per-(image, output channel) sum / sum of squares of the stored
   // values, gn_ws = [gn_slots][N][2][ws_ld] already offset to this launch's first channel.
   int ws_ld;
+  // Two-source A (one-tap K-major GEMMs): k < cat_k0 reads A, k >= cat_k0 reads A1 at k - cat_k0.  cat_k0 is a
+  // multiple of 64, so every 64-deep k chunk comes from one source.  A1.ptr == nullptr = one source.
+  TcOperand A1;
+  int cat_k0;
 };
 
 int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream);

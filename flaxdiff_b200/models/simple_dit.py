@@ -55,6 +55,9 @@ def _lecun_normal(t: torch.Tensor, fan_in: int, gen: torch.Generator) -> None:
 
 
 class SimpleDiT:
+    # the text projection's module name (mean-pooled over tokens; SimpleUDiT names it text_proj)
+    _text_proj = "text_context_proj"
+
     def __init__(self, output_channels: int = 3, patch_size: int = 16, emb_features: int = 768, num_layers: int = 12,
                  num_heads: int = 12, mlp_ratio: int = 4, dropout_rate: float = 0.0, dtype=None, precision=None,
                  use_flash_attention: bool = False, force_fp32_for_softmax: bool = True, norm_epsilon: float = 1e-5,
@@ -109,7 +112,7 @@ class SimpleDiT:
                  ("time_embed/layers_1/DenseGeneral_1/kernel", (E, E)), ("time_embed/layers_1/DenseGeneral_1/bias", (E,)),
                  ("time_embed/layers_2/kernel", (E, F)), ("time_embed/layers_2/bias", (F,))]
         if self.context_dim:
-            specs += [("text_context_proj/kernel", (self.context_dim, F)), ("text_context_proj/bias", (F,))]
+            specs += [(f"{self._text_proj}/kernel", (self.context_dim, F)), (f"{self._text_proj}/bias", (F,))]
         for n, _, _ in self._blocks():
             specs += self._block_specs(n)
         specs += [("final_norm/scale", (F,)), ("final_norm/bias", (F,)),
@@ -249,7 +252,7 @@ class SimpleDiT:
             raise FdxError(f"{type(self).__name__}: textcontext width {tuple(textcontext.shape)} does not match the parameters "
                            f"(context_dim={self.context_dim}); build / init the model with it")
         if textcontext is None and self.context_dim is not None:
-            raise FdxError(f"{type(self).__name__}: parameters were built with text_context_proj but textcontext is None")
+            raise FdxError(f"{type(self).__name__}: parameters were built with {self._text_proj} but textcontext is None")
         W32, W16 = fp.named, fp.shadow()
         dev = x.device
         HP, WP = H // p, W // p
@@ -265,16 +268,20 @@ class SimpleDiT:
         tok, sv["patch_rows"] = self._embed_fwd(x, W32, W16, HP, WP, order)
         sv["order"] = order
 
-        blocks = []
-        for n, fwd, _ in self._blocks():
-            tok, rec = fwd(n, tok, cond16, W32, W16, B, L)
-            blocks.append(rec)
-        sv["blocks"] = blocks
+        tok, sv["blocks"] = self._trunk_fwd(tok, cond16, W32, W16, B, L)
 
         out, sv["final"] = self._final_fwd(tok, W32, W16, B, H, W, L, order)
         if not save:
             return out, None
         return out, sv
+
+    def _trunk_fwd(self, tok, cond16, W32, W16, B: int, L: int):
+        """The blocks between the patch embedding and final_norm -> (tokens, tape)."""
+        blocks = []
+        for n, fwd, _ in self._blocks():
+            tok, rec = fwd(n, tok, cond16, W32, W16, B, L)
+            blocks.append(rec)
+        return tok, blocks
 
     def _embed_fwd(self, x, W32, W16, HP: int, WP: int, order):
         """Patch rows (in the patch order) x the patch embedding [+ the position table] -> (tokens bf16, patch rows)."""
@@ -379,6 +386,11 @@ class SimpleDiT:
     def _cond_width(self) -> int:
         return self.emb_features
 
+    @staticmethod
+    def _pool_text(tc16: torch.Tensor) -> torch.Tensor:
+        """The text tokens [B, S, D] mean-pooled to bf16 [B, D]."""
+        return ops.cast_f32_bf16(ops.dit_token_mean(tc16))
+
     def _cond_fwd(self, W32, W16, temb, textcontext, B: int, dev):
         """The blocks' conditioning: bf16 [B, F] = time_embed(t) [+ mean over tokens of text_context_proj(ctx)]."""
         F = self.emb_features
@@ -391,10 +403,10 @@ class SimpleDiT:
             tc16 = self._text_rows(textcontext, B)
             # mean_t(ctx W + b) = mean_t(ctx) W + b: the token mean first, then one [B, Dc] x [Dc, F] product added
             # onto the time embedding's last dense layer (both biases in that layer's epilogue)
-            ctxm16 = ops.cast_f32_bf16(ops.dit_token_mean(tc16))
-            cond = ops.linear_fwd(h2, W16[te + "2/kernel"], bias=W32[te + "2/bias"] + W32["text_context_proj/bias"],
+            ctxm16 = self._pool_text(tc16)
+            cond = ops.linear_fwd(h2, W16[te + "2/kernel"], bias=W32[te + "2/bias"] + W32[self._text_proj + "/bias"],
                                   out_dtype=F32)
-            ops.gemm(ops.GEMM_KMN, ctxm16, W16["text_context_proj/kernel"], cond, B, F, ctxm16.shape[1],
+            ops.gemm(ops.GEMM_KMN, ctxm16, W16[self._text_proj + "/kernel"], cond, B, F, ctxm16.shape[1],
                      ctxm16.shape[1], F, F, atomic=True)
         cond16 = ops.cast_f32_bf16(cond)
         return cond16, (tt, h2, ctxm16)
@@ -407,8 +419,8 @@ class SimpleDiT:
         _dense_wgrad(Gd[te + "2/kernel"], h2, dc16)
         ops.colsum_rows(dc16, Gd[te + "2/bias"])
         if ctxm16 is not None:
-            _dense_wgrad(Gd["text_context_proj/kernel"], ctxm16, dc16)
-            Gd["text_context_proj/bias"].copy_(Gd[te + "2/bias"])
+            _dense_wgrad(Gd[self._text_proj + "/kernel"], ctxm16, dc16)
+            Gd[self._text_proj + "/bias"].copy_(Gd[te + "2/bias"])
         dh2 = _dense_dgrad(dc16, W16[te + "2/kernel"])
         self._time_mlp_bwd("time_embed", tt, dh2, W16, Gd)
 
@@ -498,16 +510,24 @@ class SimpleDiT:
 
         dcond = torch.zeros((B, self._cond_width()), dtype=F32, device=dev)
         cond16 = saved["cond16"]
-        for (n, _, bwd), rec in zip(reversed(self._blocks()), reversed(saved["blocks"])):
-            dx = bwd(rec, dx, cond16, dcond, W32, W16, Gd, B, L)
+
+        def ready(leaf: str) -> None:
             if on_ready is not None:
-                on_ready(lay.table[self._ada_leaf(n)][0], stream)
+                on_ready(lay.table[leaf][0], stream)
+        dx = self._trunk_bwd(saved["blocks"], dx, cond16, dcond, W32, W16, Gd, B, L, ready)
 
         self._embed_bwd(saved["patch_rows"], dx, Gd)
 
         self._cond_bwd(saved["temb"], dcond, W16, Gd)
         if on_ready is not None:
             on_ready(0, stream)
+
+    def _trunk_bwd(self, tape, dx, cond16, dcond, W32, W16, Gd, B: int, L: int, ready):
+        """Backward of _trunk_fwd -> d(its input tokens); ready(leaf) announces every gradient from `leaf` on final."""
+        for (n, _, bwd), rec in zip(reversed(self._blocks()), reversed(tape)):
+            dx = bwd(rec, dx, cond16, dcond, W32, W16, Gd, B, L)
+            ready(self._ada_leaf(n))
+        return dx
 
     def _ada_leaf(self, n: str) -> str:
         """Block n's first parameter in the layout: its gradients are final once the block's backward has run."""

@@ -117,6 +117,14 @@ def gemm(mode: int, A: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N
          bias: Optional[torch.Tensor] = None, res: Optional[torch.Tensor] = None,
          r_ld: int = 0, r_s=(0, 0), atomic: bool = False, reduce_batch: bool = False) -> torch.Tensor:
     """Generic (batched) bf16 GEMM on the tensor-core engine; see include/fdx.h fdx_gemm_desc."""
+    g = _gemm_desc(mode, A, B, D, M, N, K, a_ld, b_ld, d_ld, batch1, batch2, a_s, b_s, d_s, alpha, bias, res, r_ld,
+                   r_s, atomic, reduce_batch)
+    check(load().fdx_gemm(ctypes.byref(g), stream_ptr()), "gemm")
+    return D
+
+
+def _gemm_desc(mode, A, B, D, M, N, K, a_ld, b_ld, d_ld, batch1, batch2, a_s, b_s, d_s, alpha, bias, res, r_ld, r_s,
+               atomic, reduce_batch):
     g = _lib.fdx_gemm_desc()
     g.mode = mode
     g.M, g.N, g.K = M, N, K
@@ -130,8 +138,29 @@ def gemm(mode: int, A: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N
     g.alpha = alpha
     g.bias = ptr(bias)
     g.res, g.r_ld, g.r_s1, g.r_s2 = ptr(res), r_ld, r_s[0], r_s[1]
-    check(load().fdx_gemm(ctypes.byref(g), stream_ptr()), "gemm")
+    return g
+
+
+def gemm_cat(mode: int, A0: torch.Tensor, A1: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N: int, K: int,
+             K0: int, a_ld: int, a1_ld: int, b_ld: int, d_ld: int, bias: Optional[torch.Tensor] = None,
+             res: Optional[torch.Tensor] = None, r_ld: int = 0) -> torch.Tensor:
+    """gemm (KK or KMN, batch 1) with A = [A0 | A1] along k - k < K0 from A0, the rest from A1 - without writing the
+    concatenation; bit for bit gemm on torch.cat([A0, A1], 1).  See include/fdx.h fdx_gemm_cat."""
+    g = _gemm_desc(mode, A0, B, D, M, N, K, a_ld, b_ld, d_ld, 1, 1, (0, 0), (0, 0), (0, 0), 1.0, bias, res, r_ld,
+                   (0, 0), False, False)
+    check(load().fdx_gemm_cat(ctypes.byref(g), ptr(A1), a1_ld, K0, stream_ptr()), "gemm_cat")
     return D
+
+
+def linear_cat_fwd(x0: torch.Tensor, x1: torch.Tensor, w_kn: torch.Tensor, bias: Optional[torch.Tensor] = None,
+                   out_dtype=torch.bfloat16) -> torch.Tensor:
+    """y = [x0 | x1] @ w (+ bias): a Dense over the concatenation of two row matrices, w [K0 + K1, N]."""
+    M, K0 = x0.shape
+    K = K0 + x1.shape[1]
+    assert x1.shape[0] == M and w_kn.shape[0] == K and x0.stride(1) == 1 and x1.stride(1) == 1 and w_kn.is_contiguous()
+    N = w_kn.shape[1]
+    out = torch.empty((M, N), dtype=out_dtype, device=x0.device)
+    return gemm_cat(GEMM_KMN, x0, x1, w_kn, out, M, N, K, K0, x0.stride(0), x1.stride(0), N, N, bias=bias)
 
 
 def linear_fwd(x2d: torch.Tensor, w_kn: torch.Tensor, out: Optional[torch.Tensor] = None,

@@ -108,6 +108,13 @@ typedef struct {
 /* 1x1 conv (common.py:324-333), nn.DenseGeneral (attention.py:132-154, common.py:300-305),
  * and the QK^T / PV / backward products of nn.dot_product_attention (attention.py:170-174). */
 int fdx_gemm(const fdx_gemm_desc* g, void* stream);
+/* fdx_gemm with an A operand from two row matrices, as over the concatenation [A0 | A1] along k without writing it:
+ * A[m][k] = A0[m][k] (g->A, row stride g->a_ld) for k < K0 and A1[m][k - K0] (row stride a1_ld) for k >= K0.  The
+ * product runs fdx_gemm's k-block order and single f32 accumulation, so D is bit for bit fdx_gemm's on the
+ * materialised concatenation (same bias, res, output type).  KK and KMN modes, batch 1, 0 < K0 < K with K0 a multiple
+ * of 64; A0 and A1 16-byte aligned, row strides multiples of 8.  The skip-connection Dense of SimpleUDiT
+ * (simple_vit.py:427-430) and its float32 output projection (as [x | x] x [W_hi; W_lo]). */
+int fdx_gemm_cat(const fdx_gemm_desc* g, const void* A1, long long a1_ld, int K0, void* stream);
 
 /* Upsample = jax.image.resize(nearest, x2) + ConvLayer 3x3 (models/common.py:210-226) without materialising
  * the upsampled tensor: four output parities, each a 2x2 convolution of the LOW-resolution input with
