@@ -121,6 +121,11 @@ def _declare(lib) -> None:
     lib.fdx_mmdit_gate_bwd.argtypes = [vp, vp, vp, ll, i, i, vp, ll, vp, vp, vp, i, vp, ll, vp]
     lib.fdx_layernorm_rows_fwd.argtypes = [i, vp, vp, ll, i, i, i, i, vp, vp, f, vp, vp, vp, vp]
     lib.fdx_layernorm_rows_bwd.argtypes = [i, vp, vp, vp, ll, i, i, i, i, vp, vp, vp, vp, i, vp, i, vp, i, vp, vp, vp]
+    lib.fdx_uvit_assemble_fwd.argtypes = [vp, vp, vp, vp, i, i, i, i, vp, vp]
+    lib.fdx_uvit_assemble_bwd.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, i, vp, vp]
+    lib.fdx_uvit_head_norm_fwd.argtypes = [vp, ll, vp, vp, f, i, vp, vp]
+    lib.fdx_uvit_head_norm_bwd.argtypes = [vp, vp, ll, vp, vp, f, i, vp, vp, i, vp, vp, vp]
+    lib.fdx_im2col3x3_c6.argtypes = [vp, i, vp, i, i, i, i, vp, vp]
 
 
 _lib: Optional[ctypes.CDLL] = None

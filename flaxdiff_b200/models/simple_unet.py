@@ -645,7 +645,10 @@ class Unet:
             h = h + net_2(GEGLU(net_0.proj(norm3(h))))
             out = xn + project_out(h)                            [use_projection, else out = xn + h]
         or, with only_pure_attention, h = Attention2(px, textcontext or px).  Without projections the pure block's
-        output GEMM writes out = xn + Attention2(xn, ...) straight into the destination, xn as its residual."""
+        output GEMM writes out = xn + Attention2(xn, ...) straight into the destination, xn as its residual.
+        acfg may also set the block's norm_epsilon ("eps", default ATTN_EPS), norm_inputs=False (xn = x) and
+        explicitly_add_residual=False (out = project_out(h) or h, for the non-pure block); UViT runs the block so on
+        token rows viewed as [B, L, 1, C]."""
         x = xin.t
         Bn, hh, ww, C = x.shape
         L, M = hh * ww, Bn * hh * ww
@@ -653,16 +656,18 @@ class Unet:
         pure = acfg.get("only_pure_attention", True)
         proj = acfg.get("use_projection", False)
         both = acfg.get("use_self_and_cross", True)
+        eps = acfg.get("eps", ATTN_EPS)
+        resid = pure or acfg.get("explicitly_add_residual", True)
         pre = f"{name}/Attention"
         dev = x.device
-        xn = ops.rmsnorm_fwd(x, W[f"{name}/RMSNorm_0/scale"], ATTN_EPS)
+        xn = ops.rmsnorm_fwd(x, W[f"{name}/RMSNorm_0/scale"], eps) if acfg.get("norm_inputs", True) else x
         xn2 = xn.view(M, C)
         px = ops.linear_fwd(xn2, W16[f"{name}/project_in/kernel"]) if proj else xn2
         ctx = px.view(Bn, L, C) if ctx16 is None else ctx16
         sv = {"xn": xn, "ctx_is_px": ctx16 is None}
 
         def rms(t2, pname):
-            return ops.rmsnorm_fwd(t2.view(Bn, hh, ww, C), W[pname], ATTN_EPS).view(M, C)
+            return ops.rmsnorm_fwd(t2.view(Bn, hh, ww, C), W[pname], eps).view(M, C)
 
         if pure:
             if proj:
@@ -684,15 +689,17 @@ class Unet:
             n3 = rms(h2, f"{pre}/norm3/scale")
             u = ops.linear_fwd(n3, W16[f"{pre}/ff/net_0/proj/kernel"], bias=W[f"{pre}/ff/net_0/proj/bias"])
             g = ops.geglu_fwd(u)
-            h3 = ops.linear_fwd(g, W16[f"{pre}/ff/net_2/kernel"], bias=W[f"{pre}/ff/net_2/bias"], res=h2)
+            last = not (proj or resid)          # h3 is the block's output: written into the destination
+            h3 = ops.linear_fwd(g, W16[f"{pre}/ff/net_2/kernel"], bias=W[f"{pre}/ff/net_2/bias"], res=h2,
+                                out=dst.t.view(M, C) if last else None)
             sv.update(h2=h2, n3=n3, u=u, g=g)
             h = h3
         sv["h_last"] = h
         # out = xn + project_out(h)   (written straight into the destination slot)
         if proj:
             ops.gemm(GEMM_KMN, h, W16[f"{name}/project_out/kernel"], dst.t, M, C, C, C, C, dst.t.stride(2),
-                     res=xn, r_ld=C)
-        elif not pure:
+                     res=xn if resid else None, r_ld=C if resid else 0)
+        elif not pure and resid:
             ops.act_add(xn, h.view(Bn, hh, ww, C), dst.t)
         return ("tblock", name, xin, dst, acfg, sv)
 
@@ -704,6 +711,9 @@ class Unet:
         pure = acfg.get("only_pure_attention", True)
         proj = acfg.get("use_projection", False)
         both = acfg.get("use_self_and_cross", True)
+        eps = acfg.get("eps", ATTN_EPS)
+        norm_in = acfg.get("norm_inputs", True)
+        resid = pure or acfg.get("explicitly_add_residual", True)
         pre = f"{name}/Attention"
         dout = grad_of(dst)                                   # [B,h,w,C], possibly a slot view
         xn = sv["xn"]
@@ -712,7 +722,7 @@ class Unet:
         def rms_bwd_into(x2, dy2, pname, dx2):
             """dx2 += d/dx RMSNorm(x2) given dy2 (accumulates in place)."""
             v4 = lambda t: t.view(Bn, hh, ww, C)
-            ops.rmsnorm_bwd(v4(x2), v4(dy2), W[pname], ATTN_EPS, v4(dx2), Gd[pname], True)
+            ops.rmsnorm_bwd(v4(x2), v4(dy2), W[pname], eps, v4(dx2), Gd[pname], True)
 
         if pure and not proj:
             # out = xn + Attention2(xn, ctx): d xn = dout (added in the dq GEMM's epilogue) + dq Wq^T
@@ -752,14 +762,19 @@ class Unet:
             if dctx_px is not None:                                        # context = px (textcontext is None)
                 self._add2d(dpx, dctx_px, dpx)
             # px = project_in(xn);  d xn = dout (residual) + d px . W_in^T
-            dxn = torch.empty((M, C), dtype=BF16, device=x.device)
             if proj:
+                dxn = torch.empty((M, C), dtype=BF16, device=x.device)
                 _dense_wgrad(Gd[f"{name}/project_in/kernel"], xn.view(M, C), dpx)
-                _dense_dgrad(dpx, W16[f"{name}/project_in/kernel"], out=dxn, res=dout2)
-            else:
+                _dense_dgrad(dpx, W16[f"{name}/project_in/kernel"], out=dxn, res=dout2 if resid else None)
+            elif resid:
+                dxn = torch.empty((M, C), dtype=BF16, device=x.device)
                 self._add2d(dpx, dout2, dxn)
+            else:
+                dxn = dpx
+        if not norm_in:             # xn = x: d x is d xn, handed back as bf16 [M, C] instead of written through want
+            return dxn
         dx, acc = want(xin)
-        ops.rmsnorm_bwd(x, dxn.view(Bn, hh, ww, C), W[f"{name}/RMSNorm_0/scale"], ATTN_EPS, dx,
+        ops.rmsnorm_bwd(x, dxn.view(Bn, hh, ww, C), W[f"{name}/RMSNorm_0/scale"], eps, dx,
                         Gd[f"{name}/RMSNorm_0/scale"], acc)
 
     # ------------------------------------------------------------------ backward program

@@ -699,8 +699,13 @@ def conv_out_fwd(x: torch.Tensor, w: torch.Tensor, bias) -> torch.Tensor:
     wr[:, :27] = w.reshape(9, cin, 3).permute(1, 0, 2).reshape(cin, 27)       # [ci][(t,k)]
     col = torch.empty((n * h * w_, 32), dtype=torch.float32, device=x.device)
     gemm(GEMM_KMN, x, cast_f32_bf16(wr), col, n * h * w_, 32, cin, x.stride(2), 32, 32)
-    y = torch.empty((n, h, w_, 3), dtype=torch.float32, device=x.device)
-    check(load().fdx_col2im3x3_c3(ptr(col), ptr(bias), ctypes.c_int(n), ctypes.c_int(h), ctypes.c_int(w_),
+    return col2im3(col, bias, n, h, w_)
+
+
+def col2im3(col: torch.Tensor, bias, n: int, h: int, w: int) -> torch.Tensor:
+    """y f32 (n, h, w, 3) = bias + the nine taps' partial sums of col f32 [n*h*w, 32] (column t*3+k), SAME padding."""
+    y = torch.empty((n, h, w, 3), dtype=torch.float32, device=col.device)
+    check(load().fdx_col2im3x3_c3(ptr(col), ptr(bias), ctypes.c_int(n), ctypes.c_int(h), ctypes.c_int(w),
                                   ptr(y), stream_ptr()), "col2im3x3_c3")
     return y
 
@@ -1295,3 +1300,83 @@ def softmax_bwd(P: torch.Tensor, dP: torch.Tensor, scale: float, valid: Optional
     check(load().fdx_softmax_bwd(ptr(P), ptr(dP), ctypes.c_longlong(P.numel() // Lp), ctypes.c_int(L),
                                  ctypes.c_int(Lp), ctypes.c_float(scale), ptr(dS), stream_ptr()), "softmax_bwd")
     return dS
+
+
+# --------------------------------------------------------------------------- UViT
+def uvit_assemble_fwd(patch: torch.Tensor, pos: torch.Tensor, time_tok: torch.Tensor, text: Optional[torch.Tensor],
+                      B: int, N: int, T: int) -> torch.Tensor:
+    """The bf16 stream [B * (N + 1 + T), F]: per sample, bf16(patch + pos) rows, the time token, the text rows."""
+    F = patch.shape[1]
+    assert patch.dtype == torch.bfloat16 and patch.is_contiguous() and patch.shape[0] == B * N
+    assert pos.dtype == torch.float32 and pos.is_contiguous() and pos.shape[-1] == F and pos.numel() >= N * F
+    assert time_tok.dtype == torch.bfloat16 and time_tok.is_contiguous() and tuple(time_tok.shape) == (B, F)
+    if T:
+        assert text.dtype == torch.bfloat16 and text.is_contiguous() and tuple(text.shape) == (B * T, F)
+    out = torch.empty((B * (N + 1 + T), F), dtype=torch.bfloat16, device=patch.device)
+    check(load().fdx_uvit_assemble_fwd(ptr(patch), ptr(pos), ptr(time_tok), ptr(text if T else None), B, N, T, F,
+                                       ptr(out), stream_ptr()), "uvit_assemble_fwd")
+    return out
+
+
+def uvit_pos_splits(B: int, N: int, F: int) -> int:
+    """Sample splits of the position gradient's first stage: enough (N * F / 8)-thread slabs to fill the GPU, at most
+    B.  A function of the shape only, so the summation order is too."""
+    return max(1, min(B, (1 << 20) // max(1, N * F // 8)))
+
+
+def uvit_assemble_bwd(dx: torch.Tensor, B: int, N: int, T: int, dpos: torch.Tensor, want_time: bool = True,
+                      want_text: bool = True):
+    """-> (dpatch bf16 [B * N, F], dtime f32 [B, F] or None, dtext bf16 [B * T, F] or None); dpos f32 [N, F]
+    (a row-contiguous view) += the sum over samples of the patch rows' gradient."""
+    F = dx.shape[1]
+    assert dx.dtype == torch.bfloat16 and dx.is_contiguous() and dx.shape[0] == B * (N + 1 + T)
+    assert dpos.dtype == torch.float32 and dpos.is_contiguous() and tuple(dpos.shape) == (N, F)
+    dev = dx.device
+    dpatch = torch.empty((B * N, F), dtype=torch.bfloat16, device=dev)
+    dtime = torch.empty((B, F), dtype=torch.float32, device=dev) if want_time else None
+    dtext = torch.empty((B * T, F), dtype=torch.bfloat16, device=dev) if (want_text and T) else None
+    nsplit = uvit_pos_splits(B, N, F)
+    ws = torch.empty((nsplit, N, F), dtype=torch.float32, device=dev)
+    check(load().fdx_uvit_assemble_bwd(ptr(dx), B, N, T, F, ptr(dpatch), ptr(dtime), ptr(dtext), ptr(ws), nsplit,
+                                       ptr(dpos), stream_ptr()), "uvit_assemble_bwd")
+    return dpatch, dtime, dtext
+
+
+def uvit_head_norm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, act_code: int):
+    """act(LayerNorm(x) gamma + beta) per pixel of x bf16 [..., 64] (act 1 = swish, 2 = mish) -> bf16, same shape."""
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.shape[-1] == 64
+    y = torch.empty_like(x)
+    check(load().fdx_uvit_head_norm_fwd(ptr(x), x.numel() // 64, ptr(gamma), ptr(beta), eps, act_code, ptr(y),
+                                        stream_ptr()), "uvit_head_norm_fwd")
+    return y
+
+
+def uvit_head_norm_chunks(pixels: int) -> int:
+    """Pixel chunks of the head LayerNorm backward's first stage: 256 pixels or more each, at most 528 (four per SM of
+    a 132-SM H100).  A function of the size only, so the summation order is too."""
+    return max(1, min(528, -(-pixels // 256)))
+
+
+def uvit_head_norm_bwd(x: torch.Tensor, dy: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float,
+                       act_code: int, dgamma: torch.Tensor, dbeta: torch.Tensor) -> torch.Tensor:
+    """-> dx bf16; dgamma / dbeta f32 [64] += the sums over pixels (fixed order)."""
+    assert x.dtype == dy.dtype == torch.bfloat16 and x.is_contiguous() and dy.is_contiguous() and x.shape == dy.shape
+    pixels = x.numel() // 64
+    nchunk = uvit_head_norm_chunks(pixels)
+    ws = torch.empty((nchunk, 2, 64), dtype=torch.float32, device=x.device)
+    dx = torch.empty_like(x)
+    check(load().fdx_uvit_head_norm_bwd(ptr(x), ptr(dy), pixels, ptr(gamma), ptr(beta), eps, act_code, ptr(dx),
+                                        ptr(ws), nchunk, ptr(dgamma), ptr(dbeta), stream_ptr()), "uvit_head_norm_bwd")
+    return dx
+
+
+def im2col3_c6(src0: torch.Tensor, src1: torch.Tensor) -> torch.Tensor:
+    """final_conv1's bf16 operand [n*h*w, 64] over concat([src0, src1], -1) (two dense (n, h, w, 3) tensors, f32 or
+    bf16): src0's 27 taps in columns 0..26, src1's in 32..58, zeros elsewhere."""
+    n, h, w, c = src0.shape
+    assert c == 3 and tuple(src1.shape) == (n, h, w, 3) and src0.is_contiguous() and src1.is_contiguous()
+    assert src0.dtype in (torch.float32, torch.bfloat16) and src1.dtype in (torch.float32, torch.bfloat16)
+    col = torch.empty((n * h * w, 64), dtype=torch.bfloat16, device=src0.device)
+    check(load().fdx_im2col3x3_c6(ptr(src0), int(src0.dtype == torch.float32), ptr(src1),
+                                  int(src1.dtype == torch.float32), n, h, w, ptr(col), stream_ptr()), "im2col3x3_c6")
+    return col

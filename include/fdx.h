@@ -565,6 +565,36 @@ int fdx_layernorm_rows_bwd(int mode, const void* src0_bf16, const void* src1_bf1
                            const float* rstd, void* dx0_bf16, int accumulate0, void* dx1_bf16, int accumulate1,
                            float* ws, int nchunk, float* dgamma, float* dbeta, void* stream);
 
+/* ---- UViT (flaxdiff/models/simple_vit.py:18-250): the sequence assembly and the output head (fdx_uvit.cu) ---------
+ * The token stream is bf16 [B * L][F] with L = N + 1 + T (N patches, the time token, T text tokens; F a multiple of 8).
+ *   fdx_uvit_assemble_fwd : replaces `x_patches + pos_encoding[:, :N]` and `concat([patches, time, text], 1)`
+ *                           (:194-210): row b L + s is bf16(f32(patch[b N + s]) + pos[s]) for s < N (patch bf16
+ *                           [B * N][F], pos f32 rows), time[b] for s = N (bf16 [B][F]) and text[b T + s - N - 1]
+ *                           (bf16 [B * T][F]; NULL when T = 0).
+ *   fdx_uvit_assemble_bwd : splits the stream gradient dx into dpatch (bf16 [B * N][F]), dtime (f32 [B][F]; skipped
+ *                           when NULL) and dtext (bf16 [B * T][F]; skipped when NULL), and adds dpos[s] += sum_b dx[b L
+ *                           + s] for s < N (f32 [N][F]) in two ordered stages through ws = f32 [nsplit][N][F]: sample
+ *                           splits of ceil(B / nsplit), then the partials in split order.  No atomics.
+ *   fdx_uvit_head_norm_fwd: final_norm_conv + activation (:240-241): per pixel of x bf16 [pixels][64],
+ *                           y = act(LayerNorm(x) gamma + beta), f32 statistics, act 1 = swish, 2 = mish.
+ *   fdx_uvit_head_norm_bwd: its backward: dx bf16 and dgamma / dbeta (+)= the sums over pixels, formed in nchunk
+ *                           pixel chunks (ws f32 [nchunk][2][64]) and added in chunk order.  No atomics.
+ *   fdx_im2col3x3_c6      : final_conv1's operand over concat([src0, src1], -1) (:236-239) without the concat:
+ *                           col[p][t*3+k] = bf16(src0[p + d(t)][k]), col[p][32 + t*3+k] = bf16(src1[p + d(t)][k]),
+ *                           zero outside the image and in columns 27..31, 59..63; bf16 [N*H*W][64].  Sources are
+ *                           dense [N][H][W][3], f32 or bf16 as flagged. */
+int fdx_uvit_assemble_fwd(const void* patch_bf16, const float* pos, const void* time_bf16, const void* text_bf16,
+                          int B, int N, int T, int F, void* out_bf16, void* stream);
+int fdx_uvit_assemble_bwd(const void* dx_bf16, int B, int N, int T, int F, void* dpatch_bf16, float* dtime,
+                          void* dtext_bf16, float* ws, int nsplit, float* dpos, void* stream);
+int fdx_uvit_head_norm_fwd(const void* x_bf16, long long pixels, const float* gamma, const float* beta, float eps,
+                           int act, void* y_bf16, void* stream);
+int fdx_uvit_head_norm_bwd(const void* x_bf16, const void* dy_bf16, long long pixels, const float* gamma,
+                           const float* beta, float eps, int act, void* dx_bf16, float* ws, int nchunk, float* dgamma,
+                           float* dbeta, void* stream);
+int fdx_im2col3x3_c6(const void* src0, int src0_is_f32, const void* src1, int src1_is_f32, int N, int H, int W,
+                     void* col_bf16, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
