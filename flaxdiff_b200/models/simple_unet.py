@@ -382,7 +382,12 @@ class Unet:
     # ------------------------------------------------------------------ forward program
     def forward(self, fp: FlatParams, x_bf16: torch.Tensor, temb: torch.Tensor, textcontext=None,
                 save: bool = True):
-        """Returns (F f32 [B,H,W,3], tape or None)."""
+        """Returns (F f32 [B,H,W,3], tape or None).  save=False is the inference forward (apply, the samplers): the
+        same launches in the same order on the same streams, but no tape - each intermediate is released once the
+        launch that last reads it is enqueued, and each concat buffer once the up-path block that reads it is.
+        Every launch is on the current stream, so the caching allocator hands a released block only to work queued
+        after its last reader, in eager runs and inside a graph capture alike.  The activation peak is then the
+        concat buffers (allocated up front: every skip is live at the middle block) plus one block's working set."""
         has_attn = any(c is not None for c in self.attention_configs)
         ctx16 = None
         if textcontext is not None and has_attn:
@@ -487,7 +492,8 @@ class Unet:
                 dst = cat_nodes[0][2]
                 ops.conv_in_fwd(x_bf16, W[name + "/conv/kernel"], W[name + "/conv/bias"], dst.t,
                                 w_bf16=W16[name + "/conv/kernel"])
-                tape.append(("conv_in", name, x_bf16, dst))
+                if save:
+                    tape.append(("conv_in", name, x_bf16, dst))
                 pop_stack.append(0)
                 skip_idx = 1
                 cur = dst
@@ -497,21 +503,29 @@ class Unet:
             elif kind == "cat":
                 k = pop_stack.pop()
                 cur = cat_nodes[k][0]
+                if not save:                      # released after the block that reads it (below)
+                    del cat_nodes[k]
             elif kind == "res":
                 dst = out_node(idx, h, w, cout)
-                rec = self._res_fwd(name, cur, dst, emb16, W, W16, G, RES_EPS)
-                tape.append(rec)
+                rec = self._res_fwd(name, cur, dst, emb16, W, W16, G, RES_EPS, record=save)
+                if save:
+                    tape.append(rec)
+                elif cur.kids:                    # a concat buffer: its slots point back at it, so break that
+                    cur.kids.clear()              # cycle and the buffer is freed with the last reference below
                 cur = dst
             elif kind == "attn":
                 dst = out_node(idx, h, w, cin)
-                tape.append(self._tblock_fwd(name, cur, dst, cout, W, W16, ctx16))
+                rec = self._tblock_fwd(name, cur, dst, cout, W, W16, ctx16, record=save)
+                if save:
+                    tape.append(rec)
                 cur = dst
             elif kind == "down":
                 h, w = h // 2, w // 2
                 dst = out_node(idx, h, w, cout)
                 ops.conv3x3_fwd(cur.t, W16[name + "/ConvLayer_0/conv/kernel"],
                                 W[name + "/ConvLayer_0/conv/bias"], out=dst.t, stride=2, colstats=dst.colstats())
-                tape.append(("down", name, cur, dst))
+                if save:
+                    tape.append(("down", name, cur, dst))
                 cur = dst
             elif kind == "up":
                 # nearest-2x + conv3x3 as four 2x2 parity convolutions of the low-resolution tensor
@@ -521,25 +535,33 @@ class Unet:
                 weff = ops.upconv3x3_pack(W[name + "/ConvLayer_0/conv/kernel"])
                 cs = dst.colstats() if cur.t.shape[1] * cur.t.shape[2] >= ops.COLSTATS_MIN_PIXELS else None
                 ops.upconv3x3_fwd(cur.t, weff, W[name + "/ConvLayer_0/conv/bias"], dst.t, colstats=cs)
-                tape.append(("up", name, cur, dst, weff if save else None))
+                if save:
+                    tape.append(("up", name, cur, dst, weff))
+                del weff
                 cur = dst
             elif kind == "conv":
                 dst = out_node(idx, h, w, cout)
                 ops.conv3x3_fwd(cur.t, W16[name + "/conv/kernel"], W[name + "/conv/bias"], out=dst.t,
                                 colstats=dst.colstats())
-                tape.append(("conv", name, cur, dst))
+                if save:
+                    tape.append(("conv", name, cur, dst))
                 cur = dst
             elif kind == "out":
                 a, st = cur.norm_apply(G, W[self._nout + "/scale"], W[self._nout + "/bias"], OUT_EPS, self._act)
                 Fo = ops.conv_out_fwd(a, W[name + "/conv/kernel"], W[name + "/conv/bias"])
-                tape.append(("out", name, cur, st, a))
+                if save:
+                    tape.append(("out", name, cur, st, a))
+                del a
                 cur = None
         if not save:
             return Fo, None
         return Fo, {"tape": tape, "emb16": emb16, "temb_saved": temb_saved, "B": B}
 
     # ------------------------------------------------------------------ blocks: forward
-    def _res_fwd(self, name, xin: Node, dst: Node, emb16, W, W16, G, eps):
+    def _res_fwd(self, name, xin: Node, dst: Node, emb16, W, W16, G, eps, record: bool = True):
+        """ResidualBlock (models/common.py:284-338) from xin into dst.  record=False (the inference forward) runs the
+        same launches, keeps no record and returns None: a1 is released after conv1, hmid after norm2's apply, a2
+        and the 1x1 residual after conv2."""
         x = xin.t
         cin, cout = x.shape[-1], dst.t.shape[-1]
         a1, st1 = xin.norm_apply(G, W[f"{name}/{self._n1}/scale"], W[f"{name}/{self._n1}/bias"], eps, self._act)
@@ -554,7 +576,11 @@ class Unet:
         hnode = Node(torch.empty((x.shape[0], x.shape[1], x.shape[2], cout), dtype=BF16, device=x.device))
         hmid = ops.conv3x3_fwd(a1, W16[f"{name}/conv1/conv/kernel"], W[f"{name}/conv1/conv/bias"], rowvec=row,
                                out=hnode.t, colstats=hnode.colstats())
+        if not record:
+            del a1
         a2, st2 = hnode.norm_apply(G, W[f"{name}/{self._n2}/scale"], W[f"{name}/{self._n2}/bias"], eps, self._act)
+        if not record:
+            del hnode, hmid
         if cin != cout:
             Bn, hh, ww, _ = x.shape
             r = torch.empty((Bn, hh, ww, cout), dtype=BF16, device=x.device)
@@ -564,7 +590,7 @@ class Unet:
             r = x
         ops.conv3x3_fwd(a2, W16[f"{name}/conv2/conv/kernel"], W[f"{name}/conv2/conv/bias"], res=r, out=dst.t,
                         colstats=dst.colstats())
-        return ("res", name, xin, dst, st1, a1, hmid, st2, a2)
+        return ("res", name, xin, dst, st1, a1, hmid, st2, a2) if record else None
 
     @staticmethod
     def _pad_heads(w: torch.Tensor, axis: int, d: int, dp: int) -> torch.Tensor:
@@ -648,8 +674,8 @@ class Unet:
         output GEMM writes out = xn + Attention2(xn, ...) straight into the destination, xn as its residual.
         acfg may also set the block's norm_epsilon ("eps", default ATTN_EPS), norm_inputs=False (xn = x) and
         explicitly_add_residual=False (out = project_out(h) or h, for the non-pure block); UViT runs the block so on
-        token rows viewed as [B, L, 1, C].  record=False (UViT's inference forward) runs the same launches, keeps no
-        record and returns None: each intermediate is released once its last reader is enqueued."""
+        token rows viewed as [B, L, 1, C].  record=False (the UNet's and UViT's inference forwards) runs the same
+        launches, keeps no record and returns None: each intermediate is released once its last reader is enqueued."""
         x = xin.t
         Bn, hh, ww, C = x.shape
         L, M = hh * ww, Bn * hh * ww
@@ -675,7 +701,10 @@ class Unet:
                 res, h = torch.zeros((M, C), dtype=BF16, device=dev), torch.empty((M, C), dtype=BF16, device=dev)
             else:       # a channel slot viewed as [M, C] has row stride = pixel stride
                 res, h = xn2, dst.t.view(M, C)
-            sv["a2"] = self._mha_fwd(f"{pre}/Attention2", px.view(Bn, L, C), ctx, heads, W16, res, h)
+            a2 = self._mha_fwd(f"{pre}/Attention2", px.view(Bn, L, C), ctx, heads, W16, res, h)
+            if record:
+                sv["a2"] = a2
+            del a2, res
         else:
             h = px
             if both:
@@ -691,7 +720,7 @@ class Unet:
             a2 = self._mha_fwd(f"{pre}/Attention2", n2.view(Bn, L, C), ctx, heads, W16, h, h2)
             if record:
                 sv["h1"], sv["a2"] = h, a2
-            del n2, a2, h
+            del n2, a2, h, px, ctx
             n3 = rms(h2, f"{pre}/norm3/scale")
             u = ops.linear_fwd(n3, W16[f"{pre}/ff/net_0/proj/kernel"], bias=W[f"{pre}/ff/net_0/proj/bias"])
             if not record:
