@@ -275,11 +275,30 @@ class DiffusionSampler:
                          diffusion_steps: int = 1000, start_step: int = None, end_step: int = 0,
                          steps_override=None, priors=None, rngstate: RandomMarkovState = None,
                          conditioning=None, model_conditioning_inputs: Tuple = None, device=None):
+        """`conditioning`: raw inputs (e.g. prompts), one entry per sample, encoded here by the encoders of
+        `input_config` (see _encode_conditioning); `model_conditioning_inputs`: the embeddings themselves.  At most
+        one of the two may be given."""
         if sequence_length is not None:
             raise FdxError("video sampling (sequence_length) is outside the supported hot path")
+        B = num_samples if priors is None else int(priors.shape[0])
         if conditioning is not None:
-            raise FdxError("raw conditioning needs an encoder; pass model_conditioning_inputs (embeddings)")
+            if self.input_config is None or not self.input_config.conditions:
+                raise FdxError("raw conditioning needs an encoder: this sampler's input_config has no conditions; "
+                               "pass model_conditioning_inputs (embeddings)")
+            if model_conditioning_inputs is not None:
+                raise ValueError("Cannot provide both conditioning and model_conditioning_inputs")
+            if len(conditioning) != B:
+                raise ValueError(f"conditioning has {len(conditioning)} entries for {B} samples: pass one entry per "
+                                 "sample")
         device = torch.device(device) if device is not None else torch.device("cuda")
+        if conditioning is not None:
+            model_conditioning_inputs = self._encode_conditioning(conditioning, device)
+        # The models read B (2 B with guidance) rows of every conditioning tensor, broadcasting only a batch of 1;
+        # with guidance a batch of 1 would be paired with one null row, so there it must be B as well.
+        for c in model_conditioning_inputs or ():
+            if not (int(c.shape[0]) == B or (int(c.shape[0]) == 1 and self.guidance_scale <= 0)):
+                raise ValueError(f"a conditioning input of batch {int(c.shape[0])} for {B} samples: its batch must be "
+                                 f"the number of samples{'' if self.guidance_scale > 0 else ' or 1'}")
         if rngstate is None:
             rngstate = RandomMarkovState(utils.PRNGKey(42))
         if start_step is None:
@@ -326,6 +345,27 @@ class DiffusionSampler:
                 cur = torch.full((samples.shape[0],), current_step, device=device)
                 samples, _, _ = sample_model_fn(samples, cur, *model_conditioning_inputs)
         return self.post_process(samples)
+
+    def _encode_conditioning(self, conditioning, device) -> tuple:
+        """Raw conditioning -> one embedding per condition of `input_config` (samplers/common.py:315-349).  An entry
+        that is a tuple or list is matched to the conditions by position, a dict by encoder key, anything else goes
+        to every condition; each condition's encoder then encodes its whole list in one call."""
+        conds = self.input_config.conditions
+        separated = {c.encoder.key: [] for c in conds}
+        for vals in conditioning:
+            if isinstance(vals, (tuple, list)):
+                for c, v in zip(conds, vals):
+                    separated[c.encoder.key].append(v)
+            elif isinstance(vals, dict):
+                for c in conds:
+                    if c.encoder.key not in vals:
+                        raise ValueError(f"Conditioning input {c.encoder.key} not found in provided dictionary")
+                    separated[c.encoder.key].append(vals[c.encoder.key])
+            else:
+                for c in conds:
+                    separated[c.encoder.key].append(vals)
+        # the engine's text tower returns bf16 on the device already; .to() is then the same tensor
+        return tuple(c.encoder(separated[c.encoder.key]).to(device) for c in conds)
 
     def _get_noise_parameters(self, resolution, start_step, device):
         a, s = self.noise_schedule.get_rates(torch.as_tensor(self.scale_steps(start_step), device=device))
