@@ -81,6 +81,13 @@ static int conv3x3_fwd_impl(const fdx_act* x, const void* w_hwio, const float* b
   }
   if (cs) {
     FDX_REQUIRE(cs->ws && cs->slots > 0 && cs->slots <= 64 && cs->ld >= y->c, "conv3x3_fwd_stats: bad workspace");
+    // the pixels-as-M epilogue adds its sums with 16-byte vector reductions
+    FDX_REQUIRE(reinterpret_cast<uintptr_t>(cs->ws) % 16 == 0 && cs->ld % 4 == 0,
+                "conv3x3_fwd_stats: the workspace must be 16-byte aligned and ld=%d a multiple of 4", cs->ld);
+    if ((long long)y->h * y->w < 128) {
+      fdx_set_error("conv3x3_fwd_stats: fewer than 128 pixels per image of y (%dx%d)", y->w, y->h);
+      return FDX_ERR_UNSUPPORTED;
+    }
     L.gn_ws = cs->ws;
     L.gn_slots = cs->slots;
     L.ws_ld = cs->ld;

@@ -138,10 +138,13 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
   // ---- pixel box ----------------------------------------------------------
   int TW, TH, TN;
   if (!L.gemm_like) {
-    // conv: a 16 x 8 (or 16 x 4) pixel patch; small images pack several per tile
+    // conv: a 16 x 8 (or 16 x 4) pixel patch; small images pack several per tile.  Not under per-image column
+    // sums, whose epilogue adds all rows of a tile into one image's sums: there the box is one image deep
+    // (TN = 1) and as tall as it takes, its rows below the image zero-filled by TMA and invalid in the epilogue.
+    // Where the packed box already has TN = 1 both rules give the same box.
     TW = pow2_floor(L.W < 16 ? L.W : 16);
     int rem = rows_per_tile / TW;
-    TH = pow2_floor(L.H < rem ? L.H : rem);
+    TH = L.gn_ws ? rem : pow2_floor(L.H < rem ? L.H : rem);
     TN = rem / TH;
   } else {
     // GEMM: rows along x only; (y, n) are batch coordinates. A box taller than the
@@ -158,10 +161,6 @@ int fdx_tc_launch(const TcLaunch& L, cudaStream_t stream) {
     };
     FDX_REQUIRE(span(L.os_x, L.os_y, L.os_n) < (1LL << 31) && span(L.rs_x, L.rs_y, L.rs_n) < (1LL << 31),
                 "tc: the rows of one output tile span 2^31 elements or more");
-  }
-  if (L.gn_ws && TN != 1) {
-    fdx_set_error("tc: fused per-image column sums need at least 128 pixels per image (got %dx%d)", L.W, L.H);
-    return FDX_ERR_UNSUPPORTED;
   }
   d.nxb = (L.W + TW - 1) / TW;
   d.nyb = (L.H + TH - 1) / TH;

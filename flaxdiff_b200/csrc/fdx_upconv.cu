@@ -107,6 +107,16 @@ static int upconv_fwd_impl(const fdx_act* x, const void* weff_bf16, const float*
   int s = check_pair(x, y, "upconv3x3_fwd");
   if (s != FDX_OK) return s;
   FDX_REQUIRE(weff_bf16, "upconv3x3_fwd: null weights");
+  if (cs) {
+    FDX_REQUIRE(cs->ws && cs->slots > 0 && cs->slots <= 64 && cs->ld >= y->c, "upconv3x3_fwd_stats: bad workspace");
+    // the pixels-as-M epilogue adds its sums with 16-byte vector reductions
+    FDX_REQUIRE(reinterpret_cast<uintptr_t>(cs->ws) % 16 == 0 && cs->ld % 4 == 0,
+                "upconv3x3_fwd_stats: the workspace must be 16-byte aligned and ld=%d a multiple of 4", cs->ld);
+    if ((long long)y->h * y->w < 128) {
+      fdx_set_error("upconv3x3_fwd_stats: fewer than 128 pixels per image of y (%dx%d)", y->w, y->h);
+      return FDX_ERR_UNSUPPORTED;
+    }
+  }
   const int cin = x->c, cout = y->c;
   for (int ph = 0; ph < 4; ++ph) {
     const int py = ph >> 1, px = ph & 1;
@@ -135,8 +145,6 @@ static int upconv_fwd_impl(const fdx_act* x, const void* weff_bf16, const float*
     L.alpha = 1.f;
     L.bias = bias;
     if (cs) {   // the four parities add their quarter of the pixels to the same sums
-      FDX_REQUIRE(cs->ws && cs->slots > 0 && cs->slots <= 64 && cs->ld >= y->c,
-                  "upconv3x3_fwd_stats: bad workspace");
       L.gn_ws = cs->ws;
       L.gn_slots = cs->slots;
       L.ws_ld = cs->ld;

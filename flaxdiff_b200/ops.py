@@ -21,7 +21,7 @@ def _opt_act(t: Optional[torch.Tensor], name: str):
 
 # --------------------------------------------------------------------------- conv
 COLSTATS_SLOTS = 4
-COLSTATS_MIN_PIXELS = 128     # the fused epilogue sums need one image per 128-pixel output tile
+COLSTATS_MIN_PIXELS = 128     # the engines accumulate fused per-image sums on images of >= 128 pixels
 
 
 class ColStats:
@@ -246,7 +246,7 @@ def groupnorm_bwd(x, dy, groups, stats, gamma, beta, eps, act_fn, dgamma, dbeta,
 
 
 GN_FUSE_SLOTS = 8
-GN_FUSE_MIN_PIXELS = 128    # fdx_conv3x3_dgrad_gn needs one image per 128-pixel tile
+GN_FUSE_MIN_PIXELS = 128    # fdx_conv3x3_dgrad_gn fuses on images of >= 128 pixels
 # Mish fuses by default only on images of at most 16 x 16 pixels: at 32^2 and 64^2 its epilogue (an exponential and a
 # reciprocal per element) made the fused backward 2-5 % slower than the two passes on an H100 SXM (DESIGN 3.2).
 GN_FUSE_MISH_MAX_PIXELS = 256

@@ -60,9 +60,11 @@ int fdx_conv3x3_fwd(const fdx_act* x, const void* w_hwio, const float* bias, con
 /* Same convolution, additionally accumulating per (image, output channel) the sum and the sum of
  * squares of the stored bf16 values - the statistics of the GroupNorm that consumes y
  * (models/common.py:273-288), so that norm needs no pass of its own over y.
- * cs->ws = f32 [slots][N][2][ld], zeroed by the caller, pre-offset to y's first channel inside the
- * destination buffer (ld = that buffer's channel count).  FDX_ERR_UNSUPPORTED when an image of y has
- * fewer than 128 pixels.  fdx_groupnorm_stats_from_cols turns the sums into fdx_groupnorm_stats' output. */
+ * cs->ws = f32 [slots][N][2][ld], zeroed by the caller (the sums are added onto what it holds), pre-offset to
+ * y's first channel inside the destination buffer (ld = that buffer's channel count); 1 <= slots <= 64, cs->ws
+ * 16-byte aligned and ld a multiple of 4, else FDX_ERR_INVALID_ARG.
+ * FDX_ERR_UNSUPPORTED when an image of y has fewer than 128 pixels.  fdx_groupnorm_stats_from_cols turns the
+ * sums into fdx_groupnorm_stats' output. */
 typedef struct fdx_colstats {
   float* ws;
   int slots;

@@ -117,7 +117,7 @@ class GnFwd:
     """Closed-form GroupNorm (flax: f32 statistics, var = max(0, E[x^2] - E[x]^2), y = (x - mean) rstd gamma + beta)
     with optional SiLU, and the f32 error of the statistics the kernels derive from fdx_groupnorm_stats."""
 
-    def __init__(self, x, gamma_, beta_, G: int, eps: float, silu: bool):
+    def __init__(self, x, gamma_, beta_, G: int, eps: float, silu: bool, depth=None):
         self.G, self.silu, self.shape = G, silu, x.shape
         N, H, W, C = x.shape
         self.HW, self.cpg = H * W, C // G
@@ -135,8 +135,10 @@ class GnFwd:
         #   dmu <= (D+1) u mean|x|,   drstd/rstd <= (D+3) u (E[x^2] + mean^2) / (var + eps) + 5u
         # D covers both producers of the sums: gn_stats_kernel (gn_stats_ref) and the per-channel column sums
         # of fdx_groupnorm_apply_cols (each rounded once to f32, then 4 slots x ceil(cpg/32) per lane and a
-        # 5-level warp tree)
-        D = max(8 * math.ceil(self.HW * self.cpg / 8 / 256) + 13, 4 * math.ceil(self.cpg / 32) + 6)
+        # 5-level warp tree).  `depth` replaces it for sums that took a longer chain, such as the convolution
+        # engines' fused column sums (colstats_depth, then the slot and lane loop of apply_cols).
+        D = depth if depth is not None else max(8 * math.ceil(self.HW * self.cpg / 8 / 256) + 13,
+                                                 4 * math.ceil(self.cpg / 32) + 6)
         self.dmu = gamma(D + 1) * _gmean(xg.abs())
         self.rho_r = gamma(D + 3) * (ex2 + mu * mu) / (var + eps) + RSQRT + U32
         self.dxh = self.r * ((xg - mu).abs() * self.rho_r + self.dmu)      # error of the kernel's normalised x
@@ -157,8 +159,8 @@ class GnFwd:
         return y.reshape(self.shape), delta.reshape(self.shape)
 
 
-def gn_forward_ref(x, gamma_, beta_, G, eps, silu):
-    return GnFwd(x, gamma_, beta_, G, eps, silu).forward()
+def gn_forward_ref(x, gamma_, beta_, G, eps, silu, depth=None):
+    return GnFwd(x, gamma_, beta_, G, eps, silu, depth).forward()
 
 
 def gn_backward_ref(x, dy, gamma_, beta_, G, eps, silu, dy_delta=None):
@@ -354,17 +356,74 @@ def tc_bn(ncols: int) -> int:
     return min((256, 128, 64), key=lambda bn: math.ceil(ncols / bn) * (bn + 64))
 
 
+def tc_pixel_box(W: int, H: int, colstats: bool = False, rows: int = 128):
+    """fdx_tc_launch's pixel box (TW, TH, TN) of a convolution tile of `rows` pixels (128; 64 in TC_MNMN):
+    TW = the largest power of two <= min(W, 16), TH the largest <= min(H, rows / TW), and small images pack
+    TN = rows / (TW TH) images per tile.  With fused per-image column sums the box is one image deep instead:
+    TH = rows / TW, TN = 1."""
+    TW = _pow2_floor(min(W, 16))
+    rem = rows // TW
+    TH = rem if colstats else _pow2_floor(min(H, rem))
+    return TW, TH, rem // TH
+
+
+def launch_route(W, H, N, K, Ncols, es=1, halo=True, sms=132):
+    """fdx_tc_launch hands a pixels-as-M launch (forward or data gradient) to fdx_tct_launch when es = 1, Ncols
+    is a multiple of 64 but not of 256 and at most 512, and W, H, K are multiples of 16, 16, 64 (fdx_tct.cu);
+    the halo variant serves the standard 3x3 tap set and keeps its weights resident when K = 64 and a grid of
+    whole column-block groups idles no SM that the plain grid would use.  Elsewhere fdx_tc_kernel with the
+    column tile of its cost model."""
+    if es == 1 and Ncols % 64 == 0 and Ncols % 256 != 0 and Ncols <= 512 and W % 16 == 0 and H % 16 == 0 \
+            and K % 64 == 0:
+        if not halo:
+            return "tct-pertap"
+        cblks = Ncols // 64
+        ntiles = cblks * (W // 16) * (H // 16) * N
+        if K == 64 and min(ntiles, sms // cblks * cblks) == min(ntiles, sms):
+            return "tct-halo-resident"
+        return "tct-halo-streamed"
+    return f"tc-bn{tc_bn(Ncols)}"
+
+
+def colstats_depth(route: str, W: int, H: int, Ncols: int, slots: int, launches: int = 1) -> int:
+    """Longest chain of f32 additions behind one element of a fused column-sum workspace (fdx_conv3x3_fwd_stats,
+    fdx_upconv3x3_fwd_stats) from one launch over W x H pixels per image (an upconv's low-resolution input, whose
+    four parity launches, `launches` = 4, add into the same sums):
+      * tct (fdx_tct.cu): a lane adds its 64 values of a tile's channel in one chain, two shuffle levels combine
+        the quad, one atomicAdd per (tile, channel);
+      * tc (fdx_epilogue.cuh): a lane adds 8 rows in one chain, two shuffle levels combine the warp's 32 rows, and
+        each of the 4 warps of a tile adds that with one red.global.add.
+    Tile t goes to slot t % slots, t = pixel block * column blocks + column block, and the pixel blocks of one
+    image are consecutive: they visit the slots with period p = slots / gcd(column blocks, slots), so one slot
+    receives at most ceil(blocks per image / p) tiles of an image per launch."""
+    if route.startswith("tct"):
+        chain, per_tile, blocks, cblks = 64 + 2, 1, (W // 16) * (H // 16), Ncols // 64
+    else:
+        TW, TH, _ = tc_pixel_box(W, H, colstats=True)
+        chain, per_tile = 8 + 2, 4
+        blocks, cblks = math.ceil(W / TW) * math.ceil(H / TH), math.ceil(Ncols / tc_bn(Ncols))
+    p = slots // math.gcd(cblks, slots)
+    return chain + launches * per_tile * math.ceil(blocks / p)
+
+
+def colstats_ref(y, prior=None):
+    """Per (image, channel) sum and sum of squares of the stored bf16 tensor y (N, H, W, C), on top of the summed
+    slots of `prior` ([slots][N][2][C] or None) -> (value, sum of |terms|), each (N, 2, C) float64."""
+    y = y.to(torch.float64)
+    s1 = (y * y).sum((1, 2))
+    val, mag = torch.stack([y.sum((1, 2)), s1], 1), torch.stack([y.abs().sum((1, 2)), s1], 1)
+    if prior is not None:
+        p = prior.to(torch.float64)
+        val, mag = val + p.sum(0), mag + p.abs().sum(0)
+    return val, mag
+
+
 def mnmn_depth(W: int, H: int, N: int, M: int, Ncols: int, ntaps: int, sms: int, gemm: bool = False,
                b_view: bool = False, splits: int = 0, mn_batched: bool = False) -> int:
     """fdx_tc_launch in TC_MNMN (the generic weight gradient and the GEMM_MNMN reductions): 64-row pixel tiles
     (a TW x TH x TN box for convolutions, 64 rows of K for GEMMs), split over the pixel blocks (`splits` 0 =
     the wave-aware count); depth = rows per split + one level per split + the prior."""
-    if gemm:
-        TW, TH, TN = 64, 1, 1
-    else:
-        TW = _pow2_floor(min(W, 16))
-        TH = _pow2_floor(min(H, 64 // TW))
-        TN = 64 // TW // TH
+    TW, TH, TN = (64, 1, 1) if gemm else tc_pixel_box(W, H, rows=64)
     nxb, nyb, nnb = math.ceil(W / TW), math.ceil(H / TH), math.ceil(N / TN)
     tpp = 2 if (M <= 64 and ntaps > 1 and not b_view) else 1
     base = math.ceil(ntaps / tpp) * math.ceil(M / 128) * math.ceil(Ncols / tc_bn(Ncols))

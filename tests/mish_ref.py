@@ -71,9 +71,9 @@ def _mish_eval_err(z, t, q):
     return q.abs() * e_w + 12 * U32 * (t.abs() + (z * q).abs()) + 4 * FTZ
 
 
-def gn_mish_forward_ref(x, gamma_, beta_, G, eps):
-    """fdx_groupnorm_apply(act = 2) -> (y, delta) as (N, H, W, C)."""
-    f = GnFwd(x, gamma_, beta_, G, eps, False)
+def gn_mish_forward_ref(x, gamma_, beta_, G, eps, depth=None):
+    """fdx_groupnorm_apply(act = 2) -> (y, delta) as (N, H, W, C); `depth` as in GnFwd."""
+    f = GnFwd(x, gamma_, beta_, G, eps, False, depth)
     z = f.z
     t, q, d1, _ = _mish_parts(z)
     y = z * t

@@ -105,6 +105,56 @@ def test_attention_rejects_misaligned_strides_and_pointers(lib):
         assert status == -1 and msg.startswith(f"{who}: {field} must be"), (entry, field, status, msg)
 
 
+_COLSTATS_CHILD = r"""
+import ctypes, json, sys
+from flaxdiff_b200 import _lib
+lib = _lib.load()
+base = 1 << 40                                   # fake, 16-byte aligned addresses: nothing is ever dereferenced
+vp = ctypes.c_void_p
+
+
+def act(i, hw, c):
+    return ctypes.byref(_lib.fdx_act(base + (i << 30), 2, hw, hw, c, c))
+
+
+out = []
+for entry, ws_off, ld, hw in json.loads(sys.argv[1]):
+    cs = ctypes.byref(_lib.fdx_colstats(base + (3 << 30) + ws_off, 4, ld))
+    if entry == "conv":
+        st = lib.fdx_conv3x3_fwd_stats(act(0, hw, 64), vp(base + (1 << 30)), None, None, None, act(2, hw, 64),
+                                       ctypes.c_int(1), cs, None)
+    else:
+        st = lib.fdx_upconv3x3_fwd_stats(act(0, hw // 2, 64), vp(base + (1 << 30)), None, act(2, hw, 64), cs, None)
+    out.append([st, lib.fdx_last_error().decode()])
+print(json.dumps(out))
+"""
+
+
+def test_colstats_rejects_misaligned_workspace_and_small_images(lib):
+    """fdx_conv3x3_fwd_stats / fdx_upconv3x3_fwd_stats refuse a workspace off a 16-byte boundary or with a row
+    length (ld) that is not a multiple of 4 floats - the pixels-as-M epilogue adds its sums with 16-byte vector
+    reductions - and, as include/fdx.h documents, outputs of fewer than 128 pixels per image.  The calls run in a
+    child process that sees no GPU, on fake addresses: a check that let one through could launch nothing."""
+    import json
+    import subprocess
+    import sys
+    cases, want = [], []
+    for entry, who in (("conv", "conv3x3_fwd_stats"), ("upconv", "upconv3x3_fwd_stats")):
+        for ws_off, ld, hw in ((8, 320, 16), (4, 320, 16), (0, 322, 16), (0, 318, 16)):
+            cases.append((entry, ws_off, ld, hw))
+            want.append((-1, f"{who}: the workspace must be 16-byte aligned"))
+        for hw in (8, 10) if entry == "upconv" else (8, 11):    # 64, 100 / 121 pixels
+            cases.append((entry, 0, 320, hw))
+            want.append((-2, f"{who}: fewer than 128 pixels per image"))
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    r = subprocess.run([sys.executable, "-c", _COLSTATS_CHILD, json.dumps(cases)], capture_output=True, text=True,
+                       env=env, cwd=ROOT, timeout=300)
+    assert r.returncode == 0, r.stderr[-3000:]
+    res = json.loads(r.stdout.strip().splitlines()[-1])
+    for case, (status, msg), (st, prefix) in zip(cases, res, want):
+        assert status == st and msg.startswith(prefix), (case, status, msg)
+
+
 def test_product_does_not_import_oracle():
     """The oracle is test infrastructure: nothing under flaxdiff_b200/ may reference it."""
     for dp, _, fs in os.walk(os.path.join(ROOT, "flaxdiff_b200")):

@@ -53,24 +53,6 @@ def assert_route(route):
 
 
 # ----------------------------------------------------------------------------------------------- routes
-def launch_route(W, H, N, K, Ncols, es=1, halo=True):
-    """fdx_tc_launch hands a pixels-as-M launch (forward or data gradient) to fdx_tct_launch when es = 1, Ncols
-    is a multiple of 64 but not of 256 and at most 512, and W, H, K are multiples of 16, 16, 64 (fdx_tct.cu);
-    the halo variant serves the standard 3x3 tap set and keeps its weights resident when K = 64 and a grid of
-    whole column-block groups idles no SM that the plain grid would use.  Elsewhere fdx_tc_kernel with the
-    column tile of its cost model."""
-    if es == 1 and Ncols % 64 == 0 and Ncols % 256 != 0 and Ncols <= 512 and W % 16 == 0 and H % 16 == 0 \
-            and K % 64 == 0:
-        if not halo:
-            return "tct-pertap"
-        cblks = Ncols // 64
-        ntiles = cblks * (W // 16) * (H // 16) * N
-        if K == 64 and min(ntiles, SMS // cblks * cblks) == min(ntiles, SMS):
-            return "tct-halo-resident"
-        return "tct-halo-streamed"
-    return f"tc-bn{R.tc_bn(Ncols)}"
-
-
 def wgrad_route(H, W, stride):
     """fdx_conv3x3_wgrad: fdx_wgrad9_launch at stride 1 on power-of-two images with W >= 8 and H >= 64 / TW
     (TW = 16 for W >= 16, else 8), the generic TC_MNMN split-K launch otherwise."""
@@ -177,7 +159,7 @@ FWD = [
 def _fwd_id(c):
     N, H, W, Ci, Co, s, epi = c
     Ho, Wo = -(-H // s), -(-W // s)
-    r = launch_route(Wo, Ho, N, Ci, Co, s, s == 1)
+    r = R.launch_route(Wo, Ho, N, Ci, Co, s, s == 1, sms=SMS)
     return f"{r}-B{N}-{H}x{W}-{Ci}to{Co}-s{s}" + (f"-{epi}" if epi else "")
 
 
@@ -221,7 +203,7 @@ DGRAD = [
 
 def _dgrad_id(c):
     N, H, W, Ci, Co, s, acc = c
-    r = launch_route(W // s, H // s, N, Co, Ci, 1, s == 1)
+    r = R.launch_route(W // s, H // s, N, Co, Ci, 1, s == 1, sms=SMS)
     return ("s2parity-" if s == 2 else "") + f"{r}-B{N}-{H}x{W}-{Ci}from{Co}" + ("-accumulate" if acc else "")
 
 
@@ -419,7 +401,8 @@ UPCONV = [(8, 16, 16, 128, 128), (32, 32, 32, 64, 64), (4, 8, 8, 256, 256), (2, 
 
 def _up_id(c, what):
     N, h, w, Ci, Co = c
-    r = {"fwd": launch_route(w, h, N, Ci, Co, halo=False), "dgrad": f"tc-bn{R.tc_bn(Ci)}", "wgrad": "tc-mnmn"}[what]
+    r = {"fwd": R.launch_route(w, h, N, Ci, Co, halo=False, sms=SMS), "dgrad": f"tc-bn{R.tc_bn(Ci)}",
+         "wgrad": "tc-mnmn"}[what]
     return f"{r}-B{N}-{h}x{w}-{Ci}to{Co}"
 
 

@@ -369,40 +369,3 @@ def test_upconv3x3_subpixel_fwd_dgrad_wgrad(shape):
     assert rel(dw, wr.grad) < 5e-3
     ops.upconv3x3_wgrad(x, dy, dw)                              # accumulates
     assert rel(dw, 2 * wr.grad) < 5e-3
-
-
-@pytest.mark.parametrize("case", [(2, 16, 16, 64, 64, 1, 0), (3, 32, 32, 128, 192, 1, 64), (2, 32, 32, 64, 128, 2, 128),
-                                  (2, 16, 8, 320, 64, 1, 0)])
-def test_conv_fwd_fused_groupnorm_statistics(case):
-    """fdx_conv3x3_fwd_stats / fdx_upconv3x3_fwd_stats: the per-image channel sums accumulated by the
-    epilogue reproduce fdx_groupnorm_stats of the stored bf16 output (same values, different order)."""
-    torch.manual_seed(5)
-    B, h, w, cin, cout, stride, coff = case
-    x = torch.randn(B, h, w, cin, device=dev).bfloat16()
-    wt = (torch.randn(3, 3, cin, cout, device=dev) / math.sqrt(9 * cin)).bfloat16()
-    bias = torch.randn(cout, device=dev) * 0.3
-    ho, wo = h // stride, w // stride
-    buf = torch.zeros(B, ho, wo, coff + cout + 64, device=dev, dtype=torch.bfloat16)
-    y = buf[..., coff:coff + cout]
-    res = torch.randn(B, ho, wo, cout, device=dev).bfloat16() if stride == 1 else None
-    cs = ops.ColStats(B, buf.shape[-1], dev)
-    ops.conv3x3_fwd(x, wt, bias, res=res, out=y, stride=stride, colstats=(cs, coff))
-    y2 = torch.empty(B, ho, wo, cout, device=dev, dtype=torch.bfloat16)
-    ops.conv3x3_fwd(x, wt, bias, res=res, out=y2, stride=stride)
-    assert torch.equal(y, y2)                                   # the statistics do not change the output
-    st = ops.groupnorm_stats_from_cols(cs, 8, coff, cout)
-    ref = ops.groupnorm_stats(y, 8)
-    assert rel(st, ref) < 1e-5
-    # GroupNorm(+SiLU) straight from the column sums (fdx_groupnorm_apply_cols) = stats_from_cols + apply
-    gamma, beta = 1 + 0.2 * torch.randn(cout, device=dev), 0.2 * torch.randn(cout, device=dev)
-    a_ref = ops.groupnorm_apply(y, 8, st, gamma, beta, 1e-4, True)
-    a_one, st_one = ops.groupnorm_apply_cols(y, 8, cs, coff, gamma, beta, 1e-4, True)
-    assert rel(st_one, st) < 1e-6 and rel(a_one, a_ref) < 1e-3
-    # the sub-pixel upsample convolution: four parity launches add up to the same sums
-    wf = torch.randn(3, 3, cin, cout, device=dev) / math.sqrt(9 * cin)
-    weff = ops.upconv3x3_pack(wf)
-    ubuf = torch.zeros(B, 2 * h, 2 * w, coff + cout, device=dev, dtype=torch.bfloat16)
-    yu = ubuf[..., coff:]
-    cs2 = ops.ColStats(B, ubuf.shape[-1], dev)
-    ops.upconv3x3_fwd(x, weff, bias, yu, colstats=(cs2, coff))
-    assert rel(ops.groupnorm_stats_from_cols(cs2, 8, coff, cout), ops.groupnorm_stats(yu, 8)) < 1e-5

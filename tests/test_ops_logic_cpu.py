@@ -1,6 +1,7 @@
 """Host-side dispatch rules of flaxdiff_b200.ops that decide which kernel arrangement runs (no GPU needed)."""
 import torch
 
+import elementwise_ref as R
 from flaxdiff_b200 import ops
 
 
@@ -27,3 +28,27 @@ def test_groupnorm_backward_fusion_follows_the_transposed_engine():
 
 def test_colstats_constants():
     assert ops.COLSTATS_SLOTS >= 1 and ops.COLSTATS_MIN_PIXELS == 128 and ops.GN_FUSE_MIN_PIXELS == 128
+
+
+def test_fused_column_sums_take_a_one_image_pixel_box():
+    """fdx_tc_launch's pixel box (restated in elementwise_ref.tc_pixel_box) on every output of an input of
+    W, H <= 64 at strides 1 and 2.  The packed box of the other launches holds several small images per tile, which
+    per-image column sums cannot use; with sums the box is one image deep, so every image of >= 128 pixels is
+    served.  Where the packed box already holds one image the two boxes agree, so no launch that ran before
+    changes geometry; and every TMA box dimension (the box times the stride) stays within 256."""
+    refused = set()
+    for s in (1, 2):
+        for H in range(1, 65):
+            for W in range(1, 65):
+                Ho, Wo = -(-H // s), -(-W // s)
+                old = R.tc_pixel_box(Wo, Ho)
+                new = R.tc_pixel_box(Wo, Ho, colstats=True)
+                assert new[2] == 1 and new[0] * new[1] == 128, (W, H, s, new)
+                assert new[0] * s <= 256 and new[1] * s <= 256, (W, H, s, new)
+                if old[2] == 1:
+                    assert new == old, (W, H, s, old, new)
+                elif Ho * Wo >= ops.COLSTATS_MIN_PIXELS:
+                    refused.add((Wo, Ho))
+    # the images of >= 128 pixels the packed box could not serve: every square of 12 to 15 pixels a side
+    assert {w for w, h in refused if w == h} == {12, 13, 14, 15}
+    assert (6, 24) in refused and (26, 5) in refused

@@ -48,7 +48,8 @@ def cpu_params(fp, grad=False):
     return {k: v.detach().cpu().clone().requires_grad_(grad) for k, v in fp.named.items()}
 
 
-@pytest.mark.parametrize("res,B,attn", [(32, 2, False), (64, 2, True), (16, 3, False), (64, 1, True)])
+@pytest.mark.parametrize("res,B,attn", [(32, 2, False), (64, 2, True), (16, 3, False), (64, 1, True),
+                                        (48, 2, False)])
 def test_unet_forward_backward_vs_oracle(res, B, attn):
     torch.manual_seed(0)
     model, fp, acfg = make_model(attn)
