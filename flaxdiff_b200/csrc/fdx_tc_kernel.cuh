@@ -248,6 +248,8 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
       long long obase, rbase = 0;
       int img = 0;
       bool has_acc = true;
+      bool first_split = true;   // split-K: only split 0 adds the bias and row vector (each split's red.global.add
+                                 // lands on the same outputs)
       int nk;
       if constexpr (!A_MN) {
         nt = tile % p.nblks;
@@ -283,6 +285,7 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
           obase += (long long)(mt_.bz % p.nyb) * p.os_y + (long long)(mt_.bz / p.nyb) * p.os_n;
         nk = mt_.pb1 - mt_.pb0;
         has_acc = nk > 0;
+        first_split = mt_.sp == 0;
       }
       // main loop: the MMAs of stage s are retired (and s released to the producer) while those of s+1 run
       auto mainloop = [&]() {
@@ -339,11 +342,11 @@ fdx_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         if (valid && has_acc && col0 < p.Ncols) {
 #pragma unroll
           for (int j = 0; j < 32; ++j) f[j] *= p.alpha;
-          if (p.bias) {
+          if (p.bias && first_split) {
 #pragma unroll
             for (int j = 0; j < 32; ++j) f[j] += __ldg(p.bias + col0 + j);
           }
-          if (p.rowvec) {
+          if (p.rowvec && first_split) {
             const float* rv = p.rowvec + (long long)img * p.Ncols + col0;
 #pragma unroll
             for (int j = 0; j < 32; ++j) f[j] += __ldg(rv + j);

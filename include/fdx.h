@@ -104,7 +104,7 @@ typedef struct {
   int d_atomic;            /* f32 atomicAdd into D (split-K allowed) */
   int reduce_batch;        /* MNMN only: also reduce over the batch dims (dense weight grads) */
   float alpha;
-  const float* bias;       /* [N] or NULL */
+  const float* bias;       /* [N] or NULL; added once per output, also under split-K */
   const void* res; long long r_ld, r_s1, r_s2; /* bf16 residual added to D, or NULL */
 } fdx_gemm_desc;
 /* 1x1 conv (common.py:324-333), nn.DenseGeneral (attention.py:132-154, common.py:300-305),

@@ -418,11 +418,11 @@ def colstats_ref(y, prior=None):
     return val, mag
 
 
-def mnmn_depth(W: int, H: int, N: int, M: int, Ncols: int, ntaps: int, sms: int, gemm: bool = False,
-               b_view: bool = False, splits: int = 0, mn_batched: bool = False) -> int:
+def mnmn_splits(W: int, H: int, N: int, M: int, Ncols: int, ntaps: int, sms: int, gemm: bool = False,
+                b_view: bool = False, splits: int = 0, mn_batched: bool = False):
     """fdx_tc_launch in TC_MNMN (the generic weight gradient and the GEMM_MNMN reductions): 64-row pixel tiles
     (a TW x TH x TN box for convolutions, 64 rows of K for GEMMs), split over the pixel blocks (`splits` 0 =
-    the wave-aware count); depth = rows per split + one level per split + the prior."""
+    the wave-aware count) -> (splits, pixel blocks)."""
     TW, TH, TN = (64, 1, 1) if gemm else tc_pixel_box(W, H, rows=64)
     nxb, nyb, nnb = math.ceil(W / TW), math.ceil(H / TH), math.ceil(N / TN)
     tpp = 2 if (M <= 64 and ntaps > 1 and not b_view) else 1
@@ -430,6 +430,14 @@ def mnmn_depth(W: int, H: int, N: int, M: int, Ncols: int, ntaps: int, sms: int,
     kblocks = nxb if mn_batched else nxb * nyb * nnb
     nbz = nyb * nnb if mn_batched else 1
     sp = split_count(sms, base * nbz, kblocks) if splits <= 0 else min(splits, kblocks)
+    return sp, kblocks
+
+
+def mnmn_depth(W: int, H: int, N: int, M: int, Ncols: int, ntaps: int, sms: int, gemm: bool = False,
+               b_view: bool = False, splits: int = 0, mn_batched: bool = False) -> int:
+    """The longest addition chain of a TC_MNMN launch (mnmn_splits): rows per split + one level per split + the
+    prior."""
+    sp, kblocks = mnmn_splits(W, H, N, M, Ncols, ntaps, sms, gemm, b_view, splits, mn_batched)
     return 64 * math.ceil(kblocks / sp) + sp + 1
 
 

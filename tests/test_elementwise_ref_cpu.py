@@ -840,3 +840,59 @@ def test_conv_comparator_rejects_what_relative_l2_accepts():
     assert rel(buf[..., 8:72], val[:2, :4, :4]) < 5e-3
     with pytest.raises(AssertionError, match="outside its channel slot"):
         R.assert_guard_intact(buf, 8, 64, -1234.0)
+
+
+def test_gemm_comparator_rejects_what_relative_l2_accepts():
+    """Five faults of the dense GEMM engine at shapes the models issue, each inside 5e-3 relative L2 (the tolerance
+    of test_tc_epilogue_gpu.py) and each caught by the exact integer case of test_gemm_layers_elementwise_gpu.py:
+    one 64-deep k-chunk dropped in one output tile of a K = 4F = 3072 projection, one split of the wave-aware
+    split-K weight gradient dropped or added twice (UNet c4's 128 x 128 attention projections, 32768 rows, 132
+    splits) in a gradient accumulated onto a prior, the ragged last 64-column tile of N = 576 = 2 x 256 + 64 left
+    holding a previous step's output, the bias added by every split of a split-K launch (the GPU file's fixed
+    split-K bias cases, since no model passes a bias to a split-K reduction), and a residual read at the wrong row
+    stride."""
+    g = torch.Generator().manual_seed(11)
+    sms = 132
+
+    def caught(got, exact):
+        assert rel(got, exact) < 5e-3
+        assert not torch.equal(got, exact)
+
+    # KMN, K = 3072 (48 k-chunks): chunk 17 missing from the tile of rows 256..383 and columns 256..511
+    M, N, K = 1024, 768, 3072
+    a, b = _ints((M, K), g, 0, 2), _ints((K, N), g, 0, 2)
+    exact = a @ b
+    assert R.exact_case_ok(exact) and R.tc_bn(N) == 256
+    got = exact.clone()
+    got[256:384, 256:512] -= a[256:384, 17 * 64:18 * 64] @ b[17 * 64:18 * 64, 256:512]
+    caught(got, exact)
+    # MNMN weight gradient dW = x^T dy over 32768 rows, split-K onto a prior
+    rows, F = 32768, 128
+    x, dy = _ints((rows, F), g, 0, 2), _ints((rows, F), g, 0, 2)
+    splits, kblocks = R.mnmn_splits(rows, 1, 1, F, F, 1, sms, gemm=True)
+    assert splits == 132 and kblocks == rows // 64
+    prior = (x.T @ dy).flip(1)
+    exact = x.T @ dy + prior
+    assert R.exact_case_ok(exact)
+    r0, r1 = 64 * (kblocks * 7 // splits), 64 * (kblocks * 8 // splits)
+    part = x[r0:r1].T @ dy[r0:r1]
+    caught(exact - part, exact)
+    caught(exact + part, exact)
+    # the bias of a split-K launch added by every split
+    bias = _ints((F,), g)
+    caught(exact + splits * bias, exact + bias)
+    # N = 576: the last column tile [512, 576) of one row tile keeps the output of a step earlier (weights 1e-3 off)
+    M, N, K = 512, 576, 768
+    a, b = _ints((M, K), g, 0, 2), _ints((K, N), g, 0, 2)
+    exact = a @ b
+    assert R.tc_bn(N) == 256 and N % 256 == 64
+    got = exact.clone()
+    got[128:256, 512:] = a[128:256] @ (b[:, 512:] * (1 - 1e-3))
+    caught(got, exact)
+    # KK data gradient with a residual [M][r_ld = N + 64] read at row stride N
+    M, N, K = 512, 768, 3072
+    a, w = _ints((M, K), g, 0, 2), _ints((N, K), g, 0, 2)
+    resbuf = _ints((M, N + 64), g)
+    exact = a @ w.T + resbuf[:, :N]
+    got = a @ w.T + resbuf.reshape(-1)[:M * N].reshape(M, N)
+    caught(got, exact)
