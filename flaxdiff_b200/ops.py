@@ -16,7 +16,7 @@ from ._lib import GEMM_KK, GEMM_KMN, GEMM_MNMN, act, check, load, ptr, stream_pt
 
 
 def _opt_act(t: Optional[torch.Tensor], name: str):
-    return None if t is None else ctypes.byref(act(t, name))
+    return None if t is None else act(t, name)
 
 
 # --------------------------------------------------------------------------- conv
@@ -41,10 +41,8 @@ def groupnorm_stats_from_cols(cs: ColStats, groups: int, c0: int = 0, channels: 
     """fdx_groupnorm_stats' output for channels [c0, c0 + channels) of the buffer, from its epilogue sums."""
     channels = cs.channels - c0 if channels is None else channels
     stats = torch.empty((cs.n, groups, 2), dtype=torch.float32, device=cs.ws.device)
-    check(load().fdx_groupnorm_stats_from_cols(ptr(cs.ws), ctypes.c_int(cs.slots), ctypes.c_int(cs.n),
-                                               ctypes.c_int(cs.channels), ctypes.c_int(c0), ctypes.c_int(channels),
-                                               ctypes.c_int(groups), ptr(stats), stream_ptr()),
-          "groupnorm_stats_from_cols")
+    check(load().fdx_groupnorm_stats_from_cols(ptr(cs.ws), cs.slots, cs.n, cs.channels, c0, channels, groups,
+                                               ptr(stats), stream_ptr()), "groupnorm_stats_from_cols")
     return stats
 
 
@@ -62,32 +60,25 @@ def conv3x3_fwd(x: torch.Tensor, w_hwio: torch.Tensor, bias: Optional[torch.Tens
         out = torch.empty((n, ho, wo, cout), dtype=torch.bfloat16, device=x.device)
     if colstats is not None:
         d = colstats[0].desc(colstats[1])
-        check(load().fdx_conv3x3_fwd_stats(ctypes.byref(act(x, "x")), ptr(w_hwio), ptr(bias), ptr(rowvec),
-                                           _opt_act(res, "res"), ctypes.byref(act(out, "out")),
-                                           ctypes.c_int(stride), ctypes.byref(d), stream_ptr()),
-              "conv3x3_fwd_stats")
+        check(load().fdx_conv3x3_fwd_stats(act(x, "x"), ptr(w_hwio), ptr(bias), ptr(rowvec), _opt_act(res, "res"),
+                                           act(out, "out"), stride, d, stream_ptr()), "conv3x3_fwd_stats")
         return out
-    check(load().fdx_conv3x3_fwd(ctypes.byref(act(x, "x")), ptr(w_hwio), ptr(bias), ptr(rowvec),
-                                 _opt_act(res, "res"), ctypes.byref(act(out, "out")),
-                                 ctypes.c_int(stride), stream_ptr()), "conv3x3_fwd")
+    check(load().fdx_conv3x3_fwd(act(x, "x"), ptr(w_hwio), ptr(bias), ptr(rowvec), _opt_act(res, "res"),
+                                 act(out, "out"), stride, stream_ptr()), "conv3x3_fwd")
     return out
 
 
 def conv3x3_dgrad(dy: torch.Tensor, w_hwio: torch.Tensor, dx: torch.Tensor, stride: int = 1,
                   accumulate: bool = False) -> torch.Tensor:
-    check(load().fdx_conv3x3_dgrad(ctypes.byref(act(dy, "dy")), ptr(w_hwio),
-                                   ctypes.byref(act(dx, "dx")), ctypes.c_int(stride),
-                                   ctypes.c_int(1 if accumulate else 0), stream_ptr()),
-          "conv3x3_dgrad")
+    check(load().fdx_conv3x3_dgrad(act(dy, "dy"), ptr(w_hwio), act(dx, "dx"), stride, int(accumulate),
+                                   stream_ptr()), "conv3x3_dgrad")
     return dx
 
 
 def conv3x3_wgrad(x: torch.Tensor, dy: torch.Tensor, dw_hwio: torch.Tensor, stride: int = 1) -> torch.Tensor:
     """Accumulates d(loss)/dw (f32 HWIO) into dw_hwio."""
     assert dw_hwio.dtype == torch.float32 and dw_hwio.is_contiguous()
-    check(load().fdx_conv3x3_wgrad(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")),
-                                   ptr(dw_hwio), ctypes.c_int(stride), stream_ptr()),
-          "conv3x3_wgrad")
+    check(load().fdx_conv3x3_wgrad(act(x, "x"), act(dy, "dy"), ptr(dw_hwio), stride, stream_ptr()), "conv3x3_wgrad")
     return dw_hwio
 
 
@@ -99,14 +90,14 @@ def conv1x1_fwd(x: torch.Tensor, w_io: torch.Tensor, bias: Optional[torch.Tensor
     assert w_io.dtype == torch.bfloat16 and w_io.is_contiguous() and w_io.numel() == cin * cout
     if out is None:
         out = torch.empty((n, h, w, cout), dtype=torch.bfloat16, device=x.device)
-    check(load().fdx_conv1x1_fwd(ctypes.byref(act(x, "x")), ptr(w_io), ptr(bias), _opt_act(res, "res"),
-                                 ctypes.byref(act(out, "out")), stream_ptr()), "conv1x1_fwd")
+    check(load().fdx_conv1x1_fwd(act(x, "x"), ptr(w_io), ptr(bias), _opt_act(res, "res"),
+                                 act(out, "out"), stream_ptr()), "conv1x1_fwd")
     return out
 
 
 def conv1x1_dgrad(dy: torch.Tensor, w_io: torch.Tensor, dx: torch.Tensor, accumulate: bool = False) -> torch.Tensor:
-    check(load().fdx_conv1x1_dgrad(ctypes.byref(act(dy, "dy")), ptr(w_io), ctypes.byref(act(dx, "dx")),
-                                   ctypes.c_int(1 if accumulate else 0), stream_ptr()), "conv1x1_dgrad")
+    check(load().fdx_conv1x1_dgrad(act(dy, "dy"), ptr(w_io), act(dx, "dx"), int(accumulate), stream_ptr()),
+          "conv1x1_dgrad")
     return dx
 
 
@@ -119,7 +110,7 @@ def gemm(mode: int, A: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N
     """Generic (batched) bf16 GEMM on the tensor-core engine; see include/fdx.h fdx_gemm_desc."""
     g = _gemm_desc(mode, A, B, D, M, N, K, a_ld, b_ld, d_ld, batch1, batch2, a_s, b_s, d_s, alpha, bias, res, r_ld,
                    r_s, atomic, reduce_batch)
-    check(load().fdx_gemm(ctypes.byref(g), stream_ptr()), "gemm")
+    check(load().fdx_gemm(g, stream_ptr()), "gemm")
     return D
 
 
@@ -132,9 +123,9 @@ def _gemm_desc(mode, A, B, D, M, N, K, a_ld, b_ld, d_ld, batch1, batch2, a_s, b_
     g.A, g.a_ld, g.a_s1, g.a_s2 = ptr(A), a_ld, a_s[0], a_s[1]
     g.B, g.b_ld, g.b_s1, g.b_s2 = ptr(B), b_ld, b_s[0], b_s[1]
     g.D, g.d_ld, g.d_s1, g.d_s2 = ptr(D), d_ld, d_s[0], d_s[1]
-    g.d_f32 = 1 if D.dtype == torch.float32 else 0
-    g.d_atomic = 1 if atomic else 0
-    g.reduce_batch = 1 if reduce_batch else 0
+    g.d_f32 = int(D.dtype == torch.float32)
+    g.d_atomic = int(atomic)
+    g.reduce_batch = int(reduce_batch)
     g.alpha = alpha
     g.bias = ptr(bias)
     g.res, g.r_ld, g.r_s1, g.r_s2 = ptr(res), r_ld, r_s[0], r_s[1]
@@ -148,7 +139,7 @@ def gemm_cat(mode: int, A0: torch.Tensor, A1: torch.Tensor, B: torch.Tensor, D: 
     concatenation; bit for bit gemm on torch.cat([A0, A1], 1).  See include/fdx.h fdx_gemm_cat."""
     g = _gemm_desc(mode, A0, B, D, M, N, K, a_ld, b_ld, d_ld, 1, 1, (0, 0), (0, 0), (0, 0), 1.0, bias, res, r_ld,
                    (0, 0), False, False)
-    check(load().fdx_gemm_cat(ctypes.byref(g), ptr(A1), a1_ld, K0, stream_ptr()), "gemm_cat")
+    check(load().fdx_gemm_cat(g, ptr(A1), a1_ld, K0, stream_ptr()), "gemm_cat")
     return D
 
 
@@ -191,8 +182,7 @@ def _act_code(a) -> int:
 
 def groupnorm_stats(x: torch.Tensor, groups: int) -> torch.Tensor:
     stats = torch.empty((x.shape[0], groups, 2), dtype=torch.float32, device=x.device)
-    check(load().fdx_groupnorm_stats(ctypes.byref(act(x, "x")), ctypes.c_int(groups), ptr(stats),
-                                     stream_ptr()), "groupnorm_stats")
+    check(load().fdx_groupnorm_stats(act(x, "x"), groups, ptr(stats), stream_ptr()), "groupnorm_stats")
     return stats
 
 
@@ -200,10 +190,8 @@ def groupnorm_apply(x, groups, stats, gamma, beta, eps: float, act_fn, out=None)
     """y = act_fn(GroupNorm(x)); act_fn = ACT_NONE / ACT_SILU / ACT_MISH (or False / True)."""
     if out is None:
         out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
-    check(load().fdx_groupnorm_apply(ctypes.byref(act(x, "x")), ctypes.c_int(groups), ptr(stats),
-                                     ptr(gamma), ptr(beta), ctypes.c_float(eps),
-                                     ctypes.c_int(_act_code(act_fn)), ctypes.byref(act(out, "out")),
-                                     stream_ptr()), "groupnorm_apply")
+    check(load().fdx_groupnorm_apply(act(x, "x"), groups, ptr(stats), ptr(gamma), ptr(beta), eps, _act_code(act_fn),
+                                     act(out, "out"), stream_ptr()), "groupnorm_apply")
     return out
 
 
@@ -213,11 +201,9 @@ def groupnorm_apply_cols(x, groups, cs: "ColStats", c0: int, gamma, beta, eps: f
     if out is None:
         out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
     stats = torch.empty((cs.n, groups, 2), dtype=torch.float32, device=x.device)
-    check(load().fdx_groupnorm_apply_cols(ctypes.byref(act(x, "x")), ctypes.c_int(groups), ptr(cs.ws),
-                                          ctypes.c_int(cs.slots), ctypes.c_int(cs.channels), ctypes.c_int(c0),
-                                          ptr(gamma), ptr(beta), ctypes.c_float(eps), ctypes.c_int(_act_code(act_fn)),
-                                          ctypes.byref(act(out, "out")), ptr(stats), stream_ptr()),
-          "groupnorm_apply_cols")
+    check(load().fdx_groupnorm_apply_cols(act(x, "x"), groups, ptr(cs.ws), cs.slots, cs.channels, c0, ptr(gamma),
+                                          ptr(beta), eps, _act_code(act_fn), act(out, "out"), ptr(stats),
+                                          stream_ptr()), "groupnorm_apply_cols")
     return out, stats
 
 
@@ -228,20 +214,14 @@ def groupnorm_bwd(x, dy, groups, stats, gamma, beta, eps, act_fn, dgamma, dbeta,
     red = torch.empty(2 * x.shape[0] * groups, dtype=torch.float32, device=x.device)
     if addend is not None:
         assert not accumulate
-        check(load().fdx_groupnorm_bwd_add(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")),
-                                           ctypes.c_int(groups), ptr(stats), ptr(gamma), ptr(beta),
-                                           ctypes.c_float(eps), ctypes.c_int(code), ptr(red),
-                                           ptr(dgamma), ptr(dbeta), ctypes.byref(act(dx, "dx")),
-                                           ctypes.byref(act(addend, "addend")), ptr(csum_img), ptr(csum_tot),
-                                           stream_ptr()), "groupnorm_bwd_add")
+        check(load().fdx_groupnorm_bwd_add(act(x, "x"), act(dy, "dy"), groups, ptr(stats), ptr(gamma), ptr(beta),
+                                           eps, code, ptr(red), ptr(dgamma), ptr(dbeta), act(dx, "dx"),
+                                           act(addend, "addend"), ptr(csum_img), ptr(csum_tot), stream_ptr()),
+              "groupnorm_bwd_add")
         return dx
-    check(load().fdx_groupnorm_bwd(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")),
-                                   ctypes.c_int(groups), ptr(stats), ptr(gamma), ptr(beta),
-                                   ctypes.c_float(eps), ctypes.c_int(code), ptr(red),
-                                   ptr(dgamma), ptr(dbeta), ctypes.byref(act(dx, "dx")),
-                                   ctypes.c_int(1 if accumulate else 0), ptr(csum_img), ptr(csum_tot),
-                                   stream_ptr()),
-          "groupnorm_bwd")
+    check(load().fdx_groupnorm_bwd(act(x, "x"), act(dy, "dy"), groups, ptr(stats), ptr(gamma), ptr(beta), eps,
+                                   code, ptr(red), ptr(dgamma), ptr(dbeta), act(dx, "dx"), int(accumulate),
+                                   ptr(csum_img), ptr(csum_tot), stream_ptr()), "groupnorm_bwd")
     return dx
 
 
@@ -257,8 +237,7 @@ def groupnorm_coeffs(stats, gamma, beta, hw: int, eps: float) -> torch.Tensor:
     n, groups = stats.shape[0], stats.shape[1]
     c = gamma.numel()
     ab = torch.empty((n, 2, c), dtype=torch.float32, device=stats.device)
-    check(load().fdx_groupnorm_coeffs(ptr(stats), ptr(gamma), ptr(beta), ctypes.c_int(n), ctypes.c_int(hw),
-                                      ctypes.c_int(c), ctypes.c_int(groups), ctypes.c_float(eps), ptr(ab),
+    check(load().fdx_groupnorm_coeffs(ptr(stats), ptr(gamma), ptr(beta), n, hw, c, groups, eps, ptr(ab),
                                       stream_ptr()), "groupnorm_coeffs")
     return ab
 
@@ -270,9 +249,8 @@ def conv3x3_dgrad_gn(dy: torch.Tensor, w_hwio: torch.Tensor, dz: torch.Tensor, x
     ACT_SILU or ACT_MISH; mish runs on the transposed engine only (_gn_fuse_default) and raises elsewhere."""
     n, c = dz.shape[0], dz.shape[-1]
     ws = torch.empty((slots, n, 2, c), dtype=torch.float32, device=dz.device)
-    check(load().fdx_conv3x3_dgrad_gn_act(ctypes.byref(act(dy, "dy")), ptr(w_hwio), ctypes.byref(act(dz, "dz")),
-                                          ctypes.byref(act(x, "x")), ptr(ab), ptr(ws), ctypes.c_int(slots),
-                                          ctypes.c_int(_act_code(act_fn)), stream_ptr()), "conv3x3_dgrad_gn")
+    check(load().fdx_conv3x3_dgrad_gn_act(act(dy, "dy"), ptr(w_hwio), act(dz, "dz"), act(x, "x"), ptr(ab), ptr(ws),
+                                          slots, _act_code(act_fn), stream_ptr()), "conv3x3_dgrad_gn")
     return ws
 
 
@@ -280,19 +258,15 @@ def groupnorm_bwd_dz(x, dz, groups, stats, gamma, eps, ws_slots, dgamma, dbeta, 
                      accumulate: bool = False, csum_img=None, csum_tot=None, addend=None) -> torch.Tensor:
     if addend is not None:
         assert not accumulate, "groupnorm_bwd_dz: addend and accumulate are exclusive"
-        check(load().fdx_groupnorm_bwd_dz_add(ctypes.byref(act(x, "x")), ctypes.byref(act(dz, "dz")),
-                                              ctypes.c_int(groups), ptr(stats), ptr(gamma), ctypes.c_float(eps),
-                                              ptr(ws_slots), ctypes.c_int(ws_slots.shape[0]), None, ptr(dgamma),
-                                              ptr(dbeta), ctypes.byref(act(dx, "dx")),
-                                              ctypes.byref(act(addend, "addend")), ptr(csum_img), ptr(csum_tot),
+        check(load().fdx_groupnorm_bwd_dz_add(act(x, "x"), act(dz, "dz"), groups, ptr(stats), ptr(gamma), eps,
+                                              ptr(ws_slots), ws_slots.shape[0], None, ptr(dgamma), ptr(dbeta),
+                                              act(dx, "dx"), act(addend, "addend"), ptr(csum_img), ptr(csum_tot),
                                               stream_ptr()), "groupnorm_bwd_dz_add")
         return dx
-    check(load().fdx_groupnorm_bwd_dz(ctypes.byref(act(x, "x")), ctypes.byref(act(dz, "dz")),
-                                      ctypes.c_int(groups), ptr(stats), ptr(gamma), ctypes.c_float(eps),
-                                      ptr(ws_slots), ctypes.c_int(ws_slots.shape[0]), None, ptr(dgamma),
-                                      ptr(dbeta), ctypes.byref(act(dx, "dx")),
-                                      ctypes.c_int(1 if accumulate else 0), ptr(csum_img), ptr(csum_tot),
-                                      stream_ptr()), "groupnorm_bwd_dz")
+    check(load().fdx_groupnorm_bwd_dz(act(x, "x"), act(dz, "dz"), groups, ptr(stats), ptr(gamma), eps, ptr(ws_slots),
+                                      ws_slots.shape[0], None, ptr(dgamma), ptr(dbeta), act(dx, "dx"),
+                                      int(accumulate), ptr(csum_img), ptr(csum_tot), stream_ptr()),
+          "groupnorm_bwd_dz")
     return dx
 
 
@@ -334,16 +308,13 @@ def conv_dgrad_groupnorm_bwd(dy, w_hwio, x, groups, stats, gamma, beta, eps, dga
 def rmsnorm_fwd(x, scale, eps: float, out=None) -> torch.Tensor:
     if out is None:
         out = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device)
-    check(load().fdx_rmsnorm_fwd(ctypes.byref(act(x, "x")), ptr(scale), ctypes.c_float(eps),
-                                 ctypes.byref(act(out, "out")), stream_ptr()), "rmsnorm_fwd")
+    check(load().fdx_rmsnorm_fwd(act(x, "x"), ptr(scale), eps, act(out, "out"), stream_ptr()), "rmsnorm_fwd")
     return out
 
 
 def rmsnorm_bwd(x, dy, scale, eps, dx, dscale, accumulate: bool = False) -> torch.Tensor:
-    check(load().fdx_rmsnorm_bwd(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")), ptr(scale),
-                                 ctypes.c_float(eps), ctypes.byref(act(dx, "dx")),
-                                 ctypes.c_int(1 if accumulate else 0), ptr(dscale), stream_ptr()),
-          "rmsnorm_bwd")
+    check(load().fdx_rmsnorm_bwd(act(x, "x"), act(dy, "dy"), ptr(scale), eps, act(dx, "dx"), int(accumulate),
+                                 ptr(dscale), stream_ptr()), "rmsnorm_bwd")
     return dx
 
 
@@ -361,12 +332,9 @@ def diffuse_forward(x0: torch.Tensor, eps: torch.Tensor, alpha, sigma, c_in, nor
     x_t = torch.empty(tuple(x0.shape), dtype=torch.float32, device=x0.device)
     target = torch.empty_like(x_t)
     model_in = torch.empty(tuple(x0.shape), dtype=torch.bfloat16, device=x0.device)
-    check(load().fdx_diffuse_forward(ptr(x0), ctypes.c_int(1 if x0.dtype == torch.uint8 else 0),
-                                     ptr(eps), ptr(_f32c(alpha)), ptr(_f32c(sigma)), ptr(_f32c(c_in)),
-                                     ctypes.c_int(B), ctypes.c_longlong(E),
-                                     ctypes.c_int(1 if normalize else 0), ctypes.c_int(target_kind),
-                                     ptr(x_t), ptr(target), ptr(model_in), stream_ptr()),
-          "diffuse_forward")
+    check(load().fdx_diffuse_forward(ptr(x0), int(x0.dtype == torch.uint8), ptr(eps), ptr(_f32c(alpha)),
+                                     ptr(_f32c(sigma)), ptr(_f32c(c_in)), B, E, int(normalize), target_kind,
+                                     ptr(x_t), ptr(target), ptr(model_in), stream_ptr()), "diffuse_forward")
     return x_t, target, model_in
 
 
@@ -384,8 +352,7 @@ def loss_fwd_bwd(F: torch.Tensor, x_t, target, c_out, c_skip, weight, want_grad:
     loss = torch.empty(1, dtype=torch.float32, device=F.device)
     dF = torch.empty_like(F) if want_grad else None
     check(load().fdx_loss_fwd_bwd(ptr(F), ptr(x_t), ptr(target), ptr(_f32c(c_out)), ptr(_f32c(c_skip)),
-                                  ptr(_f32c(weight)), ctypes.c_int(B), ctypes.c_longlong(E), ptr(loss),
-                                  ptr(dF), stream_ptr()), "loss_fwd_bwd")
+                                  ptr(_f32c(weight)), B, E, ptr(loss), ptr(dF), stream_ptr()), "loss_fwd_bwd")
     return loss, dF
 
 
@@ -408,12 +375,10 @@ def affine_combine(inputs, coef1: torch.Tensor, coef2: Optional[torch.Tensor] = 
     out2 = torch.empty_like(x) if coef2 is not None else None
     outb = torch.empty(tuple(x.shape), dtype=torch.bfloat16, device=x.device) if want_bf16 else None
     lo, hi = (clip if clip is not None else (0.0, 0.0))
-    check(load().fdx_affine_combine(ctypes.c_int(n_in), arr, ptr(coef1), ptr(coef2),
+    check(load().fdx_affine_combine(n_in, arr, ptr(coef1), ptr(coef2),
                                     ptr(_f32c(bf16_scale)) if bf16_scale is not None else ptr(None),
-                                    ctypes.c_int(B), ctypes.c_longlong(E), ptr(out1), ptr(out2),
-                                    ptr(outb), ctypes.c_int(1 if clip is not None else 0),
-                                    ctypes.c_float(lo), ctypes.c_float(hi), stream_ptr()),
-          "affine_combine")
+                                    B, E, ptr(out1), ptr(out2), ptr(outb), int(clip is not None), lo, hi,
+                                    stream_ptr()), "affine_combine")
     return out1, out2, outb
 
 
@@ -440,8 +405,7 @@ def _random(entry: str, key, shape, dtype, device, out, *args):
         k0, k1, key_dev = 0, 0, ptr(key)
     else:
         k0, k1, key_dev = int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF, ptr(None)
-    check(getattr(load(), "fdx_" + entry)(ctypes.c_uint32(k0), ctypes.c_uint32(k1), key_dev, ctypes.c_longlong(n),
-                                          *args, ptr(out), stream_ptr()), entry)
+    check(getattr(load(), "fdx_" + entry)(k0, k1, key_dev, n, *args, ptr(out), stream_ptr()), entry)
     return out
 
 
@@ -452,8 +416,7 @@ def random_bits(key, shape, device=None, out=None) -> torch.Tensor:
 
 def random_uniform(key, shape, minval: float = 0.0, maxval: float = 1.0, device=None, out=None) -> torch.Tensor:
     """jax.random.uniform(key, shape, float32, minval, maxval)."""
-    return _random("random_uniform", key, shape, torch.float32, device, out,
-                   ctypes.c_float(minval), ctypes.c_float(maxval))
+    return _random("random_uniform", key, shape, torch.float32, device, out, minval, maxval)
 
 
 def random_normal(key, shape, device=None, out=None) -> torch.Tensor:
@@ -463,19 +426,14 @@ def random_normal(key, shape, device=None, out=None) -> torch.Tensor:
 
 def random_randint(key, shape, minval: int, maxval: int, device=None, out=None) -> torch.Tensor:
     """jax.random.randint(key, shape, minval, maxval, int32), minval < maxval."""
-    return _random("random_randint", key, shape, torch.int32, device, out,
-                   ctypes.c_int(int(minval)), ctypes.c_int(int(maxval)))
+    return _random("random_randint", key, shape, torch.int32, device, out, int(minval), int(maxval))
 
 
 def adamw_ema_step(p, g, m, v, ema, shadow, lr, b1, b2, eps, weight_decay, step, ema_decay,
                    grad_scale: float = 1.0, gnorm_sq=None, clip_norm: float = 0.0, dyn=None):
-    check(load().fdx_adamw_ema_step(ptr(p), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(shadow),
-                                    ctypes.c_longlong(p.numel()), ctypes.c_float(lr),
-                                    ctypes.c_float(b1), ctypes.c_float(b2), ctypes.c_float(eps),
-                                    ctypes.c_float(weight_decay), ctypes.c_int(step),
-                                    ctypes.c_float(ema_decay), ctypes.c_float(grad_scale),
-                                    ptr(gnorm_sq), ctypes.c_float(clip_norm), ptr(dyn), stream_ptr()),
-          "adamw_ema_step")
+    check(load().fdx_adamw_ema_step(ptr(p), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(shadow), p.numel(), lr, b1, b2,
+                                    eps, weight_decay, step, ema_decay, grad_scale, ptr(gnorm_sq), clip_norm,
+                                    ptr(dyn), stream_ptr()), "adamw_ema_step")
 
 
 def optimizer_step(kind: int, p, g, m, v, ema, shadow, lr, b1, b2, eps, weight_decay, step, ema_decay=0.999,
@@ -494,21 +452,19 @@ def optimizer_step(kind: int, p, g, m, v, ema, shadow, lr, b1, b2, eps, weight_d
         assert seg_offsets.dtype == torch.int64
         d.seg_offsets, d.nseg = ptr(seg_offsets), seg_offsets.numel()
         d.seg_norms, d.u_ws = ptr(seg_norms), ptr(u_ws)
-    check(load().fdx_optimizer_step(ctypes.byref(d), stream_ptr()), "optimizer_step")
+    check(load().fdx_optimizer_step(d, stream_ptr()), "optimizer_step")
 
 
 def ema_update(ema: torch.Tensor, p: torch.Tensor, decay: float):
     """ema = decay * ema + (1 - decay) * p over the flat buffers (TrainState.apply_ema)."""
-    check(load().fdx_ema_update(ptr(ema), ptr(p), ctypes.c_longlong(p.numel()), ctypes.c_float(decay),
-                                stream_ptr()), "ema_update")
+    check(load().fdx_ema_update(ptr(ema), ptr(p), p.numel(), decay, stream_ptr()), "ema_update")
 
 
 def grad_stats(g: torch.Tensor, dynscale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """-> f32[2] = (sum (g / dynscale[0])^2 or sum g^2, number of non-finite elements of g).  Pass the same
     DynamicScale state as to optimizer_step: its clip reads the norm with the loss scale removed."""
     out = torch.empty(2, dtype=torch.float32, device=g.device)
-    check(load().fdx_grad_stats(ptr(g), ctypes.c_longlong(g.numel()), ptr(dynscale), ptr(out), stream_ptr()),
-          "grad_stats")
+    check(load().fdx_grad_stats(ptr(g), g.numel(), ptr(dynscale), ptr(out), stream_ptr()), "grad_stats")
     return out
 
 
@@ -518,9 +474,8 @@ def sumsq(g: torch.Tensor) -> torch.Tensor:
 
 def dynscale_update(state3: torch.Tensor, gstats: torch.Tensor, growth_factor=2.0, backoff_factor=0.5,
                     growth_interval=2000, minimum_scale=1.1754943508222875e-38):
-    check(load().fdx_dynscale_update(ptr(state3), ptr(gstats), ctypes.c_float(growth_factor),
-                                     ctypes.c_float(backoff_factor), ctypes.c_int(growth_interval),
-                                     ctypes.c_float(minimum_scale), stream_ptr()), "dynscale_update")
+    check(load().fdx_dynscale_update(ptr(state3), ptr(gstats), growth_factor, backoff_factor, growth_interval,
+                                     minimum_scale, stream_ptr()), "dynscale_update")
 
 
 # --------------------------------------------------------------------------- data-parallel exchange
@@ -537,16 +492,15 @@ class Comm:
     def __init__(self, rank: int, world: int, uid: bytes):
         assert len(uid) == 128
         self._h = ctypes.c_void_p()
-        check(load().fdx_comm_init(ctypes.byref(self._h), ctypes.c_int(rank), ctypes.c_int(world),
-                                   ctypes.create_string_buffer(uid, 128)), "comm_init")
+        check(load().fdx_comm_init(ctypes.byref(self._h), rank, world, ctypes.create_string_buffer(uid, 128)),
+              "comm_init")
         self.rank, self.world = rank, world
 
     def allreduce_avg_(self, buf: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
         """In-place mean over ranks of a contiguous f32 CUDA tensor (a bucket of the flat gradient buffer)."""
         assert buf.dtype == torch.float32 and buf.is_contiguous()
         st = ctypes.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
-        check(load().fdx_comm_allreduce_avg(self._h, ptr(buf), ctypes.c_longlong(buf.numel()), st),
-              "comm_allreduce_avg")
+        check(load().fdx_comm_allreduce_avg(self._h, ptr(buf), buf.numel(), st), "comm_allreduce_avg")
         return buf
 
     def destroy(self):
@@ -563,8 +517,7 @@ def cast_f32_bf16(src: torch.Tensor, dst: Optional[torch.Tensor] = None) -> torc
     assert src.dtype == torch.float32 and src.is_contiguous()
     if dst is None:
         dst = torch.empty(tuple(src.shape), dtype=torch.bfloat16, device=src.device)
-    check(load().fdx_cast_f32_bf16(ptr(src), ptr(dst), ctypes.c_longlong(src.numel()), stream_ptr()),
-          "cast_f32_bf16")
+    check(load().fdx_cast_f32_bf16(ptr(src), ptr(dst), src.numel(), stream_ptr()), "cast_f32_bf16")
     return dst
 
 
@@ -572,21 +525,17 @@ def upsample2x(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Ten
     n, h, w, c = x.shape
     if out is None:
         out = torch.empty((n, 2 * h, 2 * w, c), dtype=torch.bfloat16, device=x.device)
-    check(load().fdx_upsample2x(ctypes.byref(act(x, "x")), ctypes.byref(act(out, "out")), stream_ptr()),
-          "upsample2x")
+    check(load().fdx_upsample2x(act(x, "x"), act(out, "out"), stream_ptr()), "upsample2x")
     return out
 
 
 def upsample2x_bwd(dy: torch.Tensor, dx: torch.Tensor, accumulate: bool = False) -> torch.Tensor:
-    check(load().fdx_upsample2x_bwd(ctypes.byref(act(dy, "dy")), ctypes.byref(act(dx, "dx")),
-                                    ctypes.c_int(1 if accumulate else 0), stream_ptr()),
-          "upsample2x_bwd")
+    check(load().fdx_upsample2x_bwd(act(dy, "dy"), act(dx, "dx"), int(accumulate), stream_ptr()), "upsample2x_bwd")
     return dx
 
 
 def act_add(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-    check(load().fdx_act_add(ctypes.byref(act(a, "a")), ctypes.byref(act(b, "b")),
-                             ctypes.byref(act(out, "out")), stream_ptr()), "act_add")
+    check(load().fdx_act_add(act(a, "a"), act(b, "b"), act(out, "out"), stream_ptr()), "act_add")
     return out
 
 
@@ -594,8 +543,7 @@ def colsum(x: torch.Tensor, per_image: bool, out: Optional[torch.Tensor] = None)
     if out is None:
         shape = (x.shape[0], x.shape[-1]) if per_image else (x.shape[-1],)
         out = torch.empty(shape, dtype=torch.float32, device=x.device)
-    check(load().fdx_colsum(ctypes.byref(act(x, "x")), ptr(out), ctypes.c_int(1 if per_image else 0),
-                            stream_ptr()), "colsum")
+    check(load().fdx_colsum(act(x, "x"), ptr(out), int(per_image), stream_ptr()), "colsum")
     return out
 
 
@@ -605,8 +553,7 @@ def upconv3x3_pack(w_hwio: torch.Tensor) -> torch.Tensor:
     assert w_hwio.dtype == torch.float32 and w_hwio.is_contiguous() and w_hwio.shape[:2] == (3, 3)
     cin, cout = w_hwio.shape[2], w_hwio.shape[3]
     weff = torch.empty((16, cin, cout), dtype=torch.bfloat16, device=w_hwio.device)
-    check(load().fdx_upconv3x3_pack(ptr(w_hwio), ctypes.c_int(cin), ctypes.c_int(cout), ptr(weff), stream_ptr()),
-          "upconv3x3_pack")
+    check(load().fdx_upconv3x3_pack(ptr(w_hwio), cin, cout, ptr(weff), stream_ptr()), "upconv3x3_pack")
     return weff
 
 
@@ -615,18 +562,17 @@ def upconv3x3_fwd(x: torch.Tensor, weff: torch.Tensor, bias: Optional[torch.Tens
     """out[B,2h,2w,Cout] = conv3x3_SAME(nearest2x(x)) + bias, without the upsampled tensor."""
     if colstats is not None:
         d = colstats[0].desc(colstats[1])
-        check(load().fdx_upconv3x3_fwd_stats(ctypes.byref(act(x, "x")), ptr(weff), ptr(bias),
-                                             ctypes.byref(act(out, "out")), ctypes.byref(d), stream_ptr()),
+        check(load().fdx_upconv3x3_fwd_stats(act(x, "x"), ptr(weff), ptr(bias), act(out, "out"), d, stream_ptr()),
               "upconv3x3_fwd_stats")
         return out
-    check(load().fdx_upconv3x3_fwd(ctypes.byref(act(x, "x")), ptr(weff), ptr(bias), ctypes.byref(act(out, "out")),
-                                   stream_ptr()), "upconv3x3_fwd")
+    check(load().fdx_upconv3x3_fwd(act(x, "x"), ptr(weff), ptr(bias), act(out, "out"), stream_ptr()),
+          "upconv3x3_fwd")
     return out
 
 
 def upconv3x3_dgrad(dy: torch.Tensor, weff: torch.Tensor, dx: torch.Tensor, accumulate: bool = False) -> torch.Tensor:
-    check(load().fdx_upconv3x3_dgrad(ctypes.byref(act(dy, "dy")), ptr(weff), ctypes.byref(act(dx, "dx")),
-                                     ctypes.c_int(1 if accumulate else 0), stream_ptr()), "upconv3x3_dgrad")
+    check(load().fdx_upconv3x3_dgrad(act(dy, "dy"), ptr(weff), act(dx, "dx"), int(accumulate), stream_ptr()),
+          "upconv3x3_dgrad")
     return dx
 
 
@@ -634,8 +580,8 @@ def upconv3x3_wgrad(x: torch.Tensor, dy: torch.Tensor, dw_hwio: torch.Tensor) ->
     """Accumulates d(loss)/dw of the 3x3 kernel (f32 HWIO) into dw_hwio."""
     assert dw_hwio.dtype == torch.float32 and dw_hwio.is_contiguous()
     ws = torch.empty((16, x.shape[-1], dy.shape[-1]), dtype=torch.float32, device=x.device)
-    check(load().fdx_upconv3x3_wgrad(ctypes.byref(act(x, "x")), ctypes.byref(act(dy, "dy")), ptr(ws), ptr(dw_hwio),
-                                     stream_ptr()), "upconv3x3_wgrad")
+    check(load().fdx_upconv3x3_wgrad(act(x, "x"), act(dy, "dy"), ptr(ws), ptr(dw_hwio), stream_ptr()),
+          "upconv3x3_wgrad")
     return dw_hwio
 
 
@@ -657,8 +603,7 @@ def conv_in_fwd_direct(x_bf16: torch.Tensor, w: torch.Tensor, bias, out: torch.T
     n, h, w_, c = x_bf16.shape
     assert c == 3 and x_bf16.dtype == torch.bfloat16 and x_bf16.is_contiguous()
     assert w.dtype == torch.float32 and w.is_contiguous()
-    check(load().fdx_conv_in_fwd(ptr(x_bf16), ctypes.c_int(n), ctypes.c_int(h), ctypes.c_int(w_),
-                                 ptr(w), ptr(bias), ctypes.byref(act(out, "out")), stream_ptr()),
+    check(load().fdx_conv_in_fwd(ptr(x_bf16), n, h, w_, ptr(w), ptr(bias), act(out, "out"), stream_ptr()),
           "conv_in_fwd")
     return out
 
@@ -667,9 +612,8 @@ def im2col3(src: torch.Tensor, sgn: int, ones_col: bool) -> torch.Tensor:
     n, h, w, c = src.shape
     assert c == 3 and src.is_contiguous() and src.dtype in (torch.float32, torch.bfloat16)
     col = torch.empty((n * h * w, 32), dtype=torch.bfloat16, device=src.device)
-    check(load().fdx_im2col3x3_c3(ptr(src), ctypes.c_int(1 if src.dtype == torch.float32 else 0),
-                                  ctypes.c_int(sgn), ctypes.c_int(n), ctypes.c_int(h), ctypes.c_int(w),
-                                  ctypes.c_int(1 if ones_col else 0), ptr(col), stream_ptr()), "im2col3x3_c3")
+    check(load().fdx_im2col3x3_c3(ptr(src), int(src.dtype == torch.float32), sgn, n, h, w, int(ones_col), ptr(col),
+                                  stream_ptr()), "im2col3x3_c3")
     return col
 
 
@@ -687,8 +631,7 @@ def conv_in_wgrad(x_bf16, dy, dw, dbias):
 
 def conv_in_wgrad_direct(x_bf16, dy, dw, dbias):
     """Workspace-free CUDA-core variant (fdx_conv_in_wgrad)."""
-    check(load().fdx_conv_in_wgrad(ptr(x_bf16), ctypes.byref(act(dy, "dy")), ptr(dw), ptr(dbias),
-                                   stream_ptr()), "conv_in_wgrad")
+    check(load().fdx_conv_in_wgrad(ptr(x_bf16), act(dy, "dy"), ptr(dw), ptr(dbias), stream_ptr()), "conv_in_wgrad")
 
 
 def conv_out_fwd(x: torch.Tensor, w: torch.Tensor, bias) -> torch.Tensor:
@@ -705,8 +648,7 @@ def conv_out_fwd(x: torch.Tensor, w: torch.Tensor, bias) -> torch.Tensor:
 def col2im3(col: torch.Tensor, bias, n: int, h: int, w: int) -> torch.Tensor:
     """y f32 (n, h, w, 3) = bias + the nine taps' partial sums of col f32 [n*h*w, 32] (column t*3+k), SAME padding."""
     y = torch.empty((n, h, w, 3), dtype=torch.float32, device=col.device)
-    check(load().fdx_col2im3x3_c3(ptr(col), ptr(bias), ctypes.c_int(n), ctypes.c_int(h), ctypes.c_int(w),
-                                  ptr(y), stream_ptr()), "col2im3x3_c3")
+    check(load().fdx_col2im3x3_c3(ptr(col), ptr(bias), n, h, w, ptr(y), stream_ptr()), "col2im3x3_c3")
     return y
 
 
@@ -714,8 +656,7 @@ def conv_out_fwd_direct(x: torch.Tensor, w: torch.Tensor, bias) -> torch.Tensor:
     """Workspace-free CUDA-core variant (fdx_conv_out_fwd)."""
     n, h, w_, c = x.shape
     y = torch.empty((n, h, w_, 3), dtype=torch.float32, device=x.device)
-    check(load().fdx_conv_out_fwd(ctypes.byref(act(x, "x")), ptr(w), ptr(bias), ptr(y), stream_ptr()),
-          "conv_out_fwd")
+    check(load().fdx_conv_out_fwd(act(x, "x"), ptr(w), ptr(bias), ptr(y), stream_ptr()), "conv_out_fwd")
     return y
 
 
@@ -735,8 +676,7 @@ def _pad4(t: torch.Tensor) -> torch.Tensor:
 
 
 def conv_out_dgrad_direct(dF: torch.Tensor, w: torch.Tensor, dx: torch.Tensor) -> torch.Tensor:
-    check(load().fdx_conv_out_dgrad(ptr(dF), ptr(w), ctypes.byref(act(dx, "dx")), stream_ptr()),
-          "conv_out_dgrad")
+    check(load().fdx_conv_out_dgrad(ptr(dF), ptr(w), act(dx, "dx"), stream_ptr()), "conv_out_dgrad")
     return dx
 
 
@@ -756,8 +696,7 @@ def conv_out_wgrad(x, dF, dw, dbias, col: Optional[torch.Tensor] = None):
 
 def conv_out_wgrad_direct(x, dF, dw, dbias):
     """Workspace-free CUDA-core variant (fdx_conv_out_wgrad)."""
-    check(load().fdx_conv_out_wgrad(ctypes.byref(act(x, "x")), ptr(dF), ptr(dw), ptr(dbias),
-                                    stream_ptr()), "conv_out_wgrad")
+    check(load().fdx_conv_out_wgrad(act(x, "x"), ptr(dF), ptr(dw), ptr(dbias), stream_ptr()), "conv_out_wgrad")
 
 
 # --------------------------------------------------------------------------- GEGLU
@@ -766,8 +705,7 @@ def geglu_fwd(u: torch.Tensor) -> torch.Tensor:
     rows, two = u.shape
     assert u.dtype == torch.bfloat16 and u.is_contiguous() and two % 16 == 0
     g = torch.empty((rows, two // 2), dtype=torch.bfloat16, device=u.device)
-    check(load().fdx_geglu_fwd(ptr(u), ctypes.c_longlong(rows), ctypes.c_int(two // 2), ptr(g), stream_ptr()),
-          "geglu_fwd")
+    check(load().fdx_geglu_fwd(ptr(u), rows, two // 2, ptr(g), stream_ptr()), "geglu_fwd")
     return g
 
 
@@ -775,8 +713,7 @@ def geglu_bwd(u: torch.Tensor, dg: torch.Tensor) -> torch.Tensor:
     rows, two = u.shape
     assert dg.shape == (rows, two // 2) and dg.is_contiguous() and dg.dtype == torch.bfloat16
     du = torch.empty_like(u)
-    check(load().fdx_geglu_bwd(ptr(u), ptr(dg), ctypes.c_longlong(rows), ctypes.c_int(two // 2), ptr(du),
-                               stream_ptr()), "geglu_bwd")
+    check(load().fdx_geglu_bwd(ptr(u), ptr(dg), rows, two // 2, ptr(du), stream_ptr()), "geglu_bwd")
     return du
 
 
@@ -815,7 +752,7 @@ def attention_fwd(q, k, v, heads: int, dh: int, scale: float, out=None):
     o = out if out is not None else torch.empty((B, L, HD), dtype=torch.bfloat16, device=q.device)
     lse = torch.empty((B, heads, L), dtype=torch.float32, device=q.device)
     a = _attn_desc(q, k, v, o, lse, heads, dh, scale)
-    check(load().fdx_attention_fwd(ctypes.byref(a), stream_ptr()), "attention_fwd")
+    check(load().fdx_attention_fwd(a, stream_ptr()), "attention_fwd")
     return o, lse
 
 
@@ -832,7 +769,7 @@ def attention_bwd(q, k, v, o, lse, d_o, heads: int, dh: int, scale: float):
     a.dq, a.dq_ld, a.dq_bs = ptr(dq), dq.stride(1), dq.stride(0)
     a.dk, a.dk_ld, a.dk_bs = ptr(dk), dk.stride(1), dk.stride(0)
     a.dv, a.dv_ld, a.dv_bs = ptr(dv), dv.stride(1), dv.stride(0)
-    check(load().fdx_attention_bwd(ctypes.byref(a), stream_ptr()), "attention_bwd")
+    check(load().fdx_attention_bwd(a, stream_ptr()), "attention_bwd")
     return dq, dk, dv
 
 
@@ -845,7 +782,7 @@ def attention_fwd_masked(q, k, v, heads: int, dh: int, scale: float, causal: boo
         assert key_mask.dtype == torch.int32 and key_mask.is_contiguous() and key_mask.shape == (B, k.shape[1])
     o = out if out is not None else torch.empty((B, L, HD), dtype=torch.bfloat16, device=q.device)
     a = _attn_desc(q, k, v, o, None, heads, dh, scale)
-    check(load().fdx_attention_fwd_masked(ctypes.byref(a), 1 if causal else 0, ptr(key_mask), stream_ptr()),
+    check(load().fdx_attention_fwd_masked(a, int(causal), ptr(key_mask), stream_ptr()),
           "attention_fwd_masked")
     return o
 
@@ -940,7 +877,7 @@ def dit_adaln_bwd(x, dy, L: int, mean, rstd, d0: torch.Tensor, d1: torch.Tensor,
     ld1 = d1.stride(0) if d1.dim() == 2 else 0
     check(load().fdx_dit_adaln_bwd(ptr(x), ptr(dy), rows, L, C, ptr(a), ld, scale_off, ptr(gamma), ptr(mean),
                                    ptr(rstd), ptr(addend), ptr(dx), ptr(ws), nch, ptr(d0), ld0, ptr(d1), ld1,
-                                   1 if reduce_samples else 0, 1 if accumulate else 0, stream_ptr()), "dit_adaln_bwd")
+                                   int(reduce_samples), int(accumulate), stream_ptr()), "dit_adaln_bwd")
     return dx
 
 
@@ -983,7 +920,7 @@ def dit_rope(t: torch.Tensor, L: int, heads: int, d: int, dp: int, nmat: int = 1
              inverse: bool = False) -> torch.Tensor:
     """RoPE in place on nmat head matrices (mat_off columns apart) of the bf16 rows of t [rows, >= ...]."""
     assert t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1
-    check(load().fdx_dit_rope(ptr(t), t.shape[0], L, t.stride(0), heads, d, dp, nmat, mat_off, 1 if inverse else 0,
+    check(load().fdx_dit_rope(ptr(t), t.shape[0], L, t.stride(0), heads, d, dp, nmat, mat_off, int(inverse),
                               stream_ptr()), "dit_rope")
     return t
 
@@ -993,7 +930,7 @@ def dit_patchify(x: torch.Tensor, p: int, ld: int) -> torch.Tensor:
     B, H, W, C = x.shape
     assert x.is_contiguous() and x.dtype in (torch.float32, torch.bfloat16)
     out = torch.empty((B * (H // p) * (W // p), ld), dtype=torch.bfloat16, device=x.device)
-    check(load().fdx_dit_patchify(ptr(x), 1 if x.dtype == torch.float32 else 0, B, H, W, C, p, ld, ptr(out),
+    check(load().fdx_dit_patchify(ptr(x), int(x.dtype == torch.float32), B, H, W, C, p, ld, ptr(out),
                                   stream_ptr()), "dit_patchify")
     return out
 
@@ -1272,9 +1209,8 @@ def time_embed_fwd(t, freqs, W1, b1, W2, b2):
     h2 = torch.empty_like(four)
     emb = torch.empty_like(four)
     emb16 = torch.empty((B, D), dtype=torch.bfloat16, device=dev)
-    check(load().fdx_time_embed_fwd(ptr(_f32c(t)), ptr(freqs), ptr(W1), ptr(b1), ptr(W2), ptr(b2),
-                                    ctypes.c_int(B), ctypes.c_int(D), ptr(four), ptr(h1), ptr(h2),
-                                    ptr(emb), ptr(emb16), stream_ptr()), "time_embed_fwd")
+    check(load().fdx_time_embed_fwd(ptr(_f32c(t)), ptr(freqs), ptr(W1), ptr(b1), ptr(W2), ptr(b2), B, D, ptr(four),
+                                    ptr(h1), ptr(h2), ptr(emb), ptr(emb16), stream_ptr()), "time_embed_fwd")
     return emb, emb16, (four, h1, h2)
 
 
@@ -1283,9 +1219,8 @@ def time_embed_bwd(demb, saved, W2, dW1, db1, dW2, db2):
     B, D = demb.shape
     ws1 = torch.empty_like(demb)
     ws2 = torch.empty_like(demb)
-    check(load().fdx_time_embed_bwd(ptr(demb), ptr(four), ptr(h1), ptr(h2), ptr(W2), ctypes.c_int(B),
-                                    ctypes.c_int(D), ptr(ws1), ptr(ws2), ptr(dW1), ptr(db1), ptr(dW2),
-                                    ptr(db2), stream_ptr()), "time_embed_bwd")
+    check(load().fdx_time_embed_bwd(ptr(demb), ptr(four), ptr(h1), ptr(h2), ptr(W2), B, D, ptr(ws1), ptr(ws2),
+                                    ptr(dW1), ptr(db1), ptr(dW2), ptr(db2), stream_ptr()), "time_embed_bwd")
 
 
 def softmax_fwd(S: torch.Tensor, valid: Optional[int] = None) -> torch.Tensor:
@@ -1293,8 +1228,7 @@ def softmax_fwd(S: torch.Tensor, valid: Optional[int] = None) -> torch.Tensor:
     Lp = S.shape[-1]
     L = Lp if valid is None else valid
     P = torch.empty(tuple(S.shape), dtype=torch.bfloat16, device=S.device)
-    check(load().fdx_softmax_fwd(ptr(S), ctypes.c_longlong(S.numel() // Lp), ctypes.c_int(L), ctypes.c_int(Lp),
-                                 ptr(P), stream_ptr()), "softmax_fwd")
+    check(load().fdx_softmax_fwd(ptr(S), S.numel() // Lp, L, Lp, ptr(P), stream_ptr()), "softmax_fwd")
     return P
 
 
@@ -1302,8 +1236,8 @@ def softmax_bwd(P: torch.Tensor, dP: torch.Tensor, scale: float, valid: Optional
     Lp = P.shape[-1]
     L = Lp if valid is None else valid
     dS = torch.empty(tuple(P.shape), dtype=torch.bfloat16, device=P.device)
-    check(load().fdx_softmax_bwd(ptr(P), ptr(dP), ctypes.c_longlong(P.numel() // Lp), ctypes.c_int(L),
-                                 ctypes.c_int(Lp), ctypes.c_float(scale), ptr(dS), stream_ptr()), "softmax_bwd")
+    check(load().fdx_softmax_bwd(ptr(P), ptr(dP), P.numel() // Lp, L, Lp, scale, ptr(dS), stream_ptr()),
+          "softmax_bwd")
     return dS
 
 

@@ -11,7 +11,6 @@ Prints, with the card's name, power limit and clocks read in the same run:
     the launches the host makes per step (graph replays + libfdx launches outside a graph) for both.
 It needs a GPU and fails without one; it changes no device setting."""
 import argparse
-import ctypes
 import os
 import subprocess
 import sys
@@ -70,7 +69,6 @@ def probe_sampler(dev, name, res, B, steps, acfg, text, rounds):
     params = model.init(4, device=dev)
     smp = EulerAncestralSampler(model, sched, KarrasPredictionTransform(0.5), cfg, guidance_scale=3.0 if text else 0.0)
     lib = _lib.load()
-    lib.fdx_launch_count.restype = ctypes.c_ulonglong
     replays = [0]
     orig = torch.cuda.CUDAGraph.replay
 

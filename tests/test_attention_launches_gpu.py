@@ -2,7 +2,6 @@
 pure or full, runs one program (Unet._tblock_fwd / _tblock_bwd around _mha_fwd / _mha_bwd); the counts below pin
 how many libfdx kernels each configuration issues, so a change that adds or drops one shows here.
 tests/gpu_probe_op_trace.py prints the calls behind each count."""
-import ctypes
 
 import pytest
 import torch
@@ -66,7 +65,6 @@ def unet_fwd_bwd(block: str, d: int, dev, unet=Unet):
 
 def launch_count() -> int:
     lib = _lib.load()
-    lib.fdx_launch_count.restype = ctypes.c_ulonglong
     return lib.fdx_launch_count()
 
 

@@ -1,5 +1,6 @@
 """The C-ABI shared library loads without a GPU / libcuda and exports every symbol that
-include/fdx.h declares.  No compute entry point is called here."""
+include/fdx.h declares, and the ctypes binding mirrors the header type for type.  No compute
+entry point is called here."""
 import ctypes
 import os
 import re
@@ -28,8 +29,113 @@ def test_exports_every_declared_symbol(lib):
 
 def test_version_and_error_string(lib):
     assert lib.fdx_version() >= 100
-    lib.fdx_last_error.restype = ctypes.c_char_p
     assert isinstance(lib.fdx_last_error(), bytes)
+
+
+# ------------------------------------------------------------------- the ctypes mirror of include/fdx.h
+# _lib.SIGNATURES' mapping rule: the C type of every parameter, struct field and return value -> its ctypes type.
+DESCRIPTORS = ("fdx_act", "fdx_colstats", "fdx_gemm_desc", "fdx_opt_desc", "fdx_attn_desc")
+SCALARS = {"int": ctypes.c_int, "long long": ctypes.c_longlong, "float": ctypes.c_float, "uint32_t": ctypes.c_uint32}
+RETURNS = {"int": ctypes.c_int, "unsigned long long": ctypes.c_ulonglong, "const char*": ctypes.c_char_p}
+
+
+def _ctype(c: str):
+    from flaxdiff_b200 import _lib
+    if c in SCALARS:
+        return SCALARS[c]
+    m = re.fullmatch(r"(?:const )?(\w+)\*", c)
+    if m and m.group(1) in DESCRIPTORS:
+        return ctypes.POINTER(getattr(_lib, m.group(1)))
+    assert c.endswith("*"), f"fdx.h: no ctypes type for the C type {c!r}"
+    return ctypes.c_void_p
+
+
+def _norm(c: str) -> str:
+    """C type with single spaces and none around '*': 'const float * const *' -> 'const float*const*'."""
+    return re.sub(r"\s*\*\s*", "*", " ".join(c.split()))
+
+
+def _header():
+    """-> ([(name, return type, [parameter types])] of the fdx_* prototypes, {typedef name: [(field, type)]} of the
+    structs), in declaration order.  Every statement must be a prototype, a struct typedef or an opaque typedef."""
+    src = open(os.path.join(ROOT, "include", "fdx.h")).read()
+    src = re.sub(r"/\*.*?\*/|//[^\n]*", " ", src, flags=re.S)
+    src = re.sub(r"#ifdef __cplusplus.*?#endif", " ", src, flags=re.S)
+    src = re.sub(r"^\s*#.*$", " ", src, flags=re.M)
+    structs = {}
+
+    def struct(m):
+        fields = []
+        for decl in filter(str.strip, m.group(1).split(";")):
+            # one base type, then declarators: 'long long a_ld, a_s1, a_s2', 'const void* A'
+            base, decls = re.fullmatch(r"\s*(.*?)\s*(\**\s*\w+(?:\s*,\s*\**\s*\w+)*)\s*", decl, re.S).groups()
+            for d in decls.split(","):
+                stars, field = re.fullmatch(r"(\**)\s*(\w+)", d.strip()).groups()
+                fields.append((field, _norm(base + stars)))
+        structs[m.group(2)] = fields
+        return " "
+    src = re.sub(r"typedef\s+struct\s*\w*\s*\{(.*?)\}\s*(\w+)\s*;", struct, src, flags=re.S)
+    protos = []
+    for stmt in src.split(";"):
+        stmt = " ".join(stmt.split())
+        if not stmt or re.fullmatch(r"typedef struct (\w+) \1", stmt):
+            continue
+        m = re.fullmatch(r"(.+?) ?\b(fdx_\w+) ?\((.*)\)", stmt)
+        assert m, f"fdx.h: cannot parse {stmt!r}"
+        params = []
+        for p in ([] if m.group(3) == "void" else m.group(3).split(",")):
+            pm = re.fullmatch(r"(.*[\s*])(\w+)", p.strip())
+            assert pm, f"fdx.h: {m.group(2)}: unnamed or unparsed parameter {p!r}"
+            params.append(_norm(pm.group(1)))
+        protos.append((m.group(2), _norm(m.group(1)), params))
+    return protos, structs
+
+
+def test_signature_table_names_every_header_function():
+    """_lib.SIGNATURES declares exactly the functions of include/fdx.h, in the header's order."""
+    from flaxdiff_b200 import _lib
+    names = [name for name, _, _ in _header()[0]]
+    missing = [n for n in names if n not in _lib.SIGNATURES]
+    extra = [n for n in _lib.SIGNATURES if n not in names]
+    assert not missing and not extra, f"missing from _lib.SIGNATURES: {missing}; not declared in fdx.h: {extra}"
+    assert list(_lib.SIGNATURES) == names, "_lib.SIGNATURES is not in fdx.h's order"
+
+
+def test_signature_table_matches_header_types():
+    """Each entry's restype and argtypes are the header's return and parameter types, position by position."""
+    from flaxdiff_b200 import _lib
+    for name, ret, params in _header()[0]:
+        restype, argtypes = _lib.SIGNATURES[name]
+        assert ret in RETURNS, f"{name}: no ctypes type for the return type {ret!r}"
+        assert restype is RETURNS[ret], f"{name} returns {ret}: the table has {restype.__name__}"
+        assert len(argtypes) == len(params), f"{name}: {len(params)} parameters in fdx.h, {len(argtypes)} in the table"
+        for k, (c, t) in enumerate(zip(params, argtypes)):
+            assert t is _ctype(c), f"{name}: parameter {k} is {c} ({_ctype(c).__name__}), the table has {t.__name__}"
+
+
+def test_descriptor_structs_match_header():
+    """fdx_act, fdx_colstats, fdx_gemm_desc, fdx_opt_desc and fdx_attn_desc: the ctypes _fields_ are the header's
+    fields, with the same names and types in the same order."""
+    from flaxdiff_b200 import _lib
+    structs = _header()[1]
+    assert sorted(structs) == sorted(DESCRIPTORS)
+    for name in DESCRIPTORS:
+        want = [(f, _ctype(c)) for f, c in structs[name]]
+        have = list(getattr(_lib, name)._fields_)
+        for k in range(max(len(want), len(have))):
+            w, h = (want[k] if k < len(want) else None), (have[k] if k < len(have) else None)
+            assert w == h, (f"{name} field {k}: fdx.h has {w and (w[0], w[1].__name__)}, "
+                            f"_lib has {h and (h[0], h[1].__name__)}")
+
+
+def test_load_declares_every_entry_point(lib):
+    """After load(), every function of the header carries the table's restype and argtypes."""
+    from flaxdiff_b200 import _lib
+    raw = lib._lib if isinstance(lib, _lib._TracingLib) else lib
+    for name, _, _ in _header()[0]:
+        restype, argtypes = _lib.SIGNATURES[name]
+        fn = getattr(raw, name)
+        assert fn.restype is restype and tuple(fn.argtypes) == tuple(argtypes), name
 
 
 def test_no_libcuda_link_dependency():

@@ -509,7 +509,6 @@ def replay(d: Desc, kind: str, name: str, seed: int):
               alpha=alpha, bias=bias, res=res, r_ld=d.r_ld, r_s=d.r_s, atomic=d.atomic,
               reduce_batch=d.reduce_batch)
     lib = _lib.load()
-    lib.fdx_kernel_kind_name.restype = ctypes.c_char_p
     ran = lib.fdx_kernel_kind_name(lib.fdx_last_kernel_kind()).decode()
     assert ran == "fdx_tc_kernel", f"{name}: ran {ran}"
     assert_outside_intact(Dbuf, D)

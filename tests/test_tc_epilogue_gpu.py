@@ -5,7 +5,6 @@ that is not a multiple of the tile, tiles with rows past the image, an odd numbe
 64-column tile, and tap pairing in the weight gradient.  The shapes are ones the transposed engine declines
 (multiples of 256 columns, 8 x 8 and 24 x 24 images, stride 2, 768 columns, GEMMs).  Each launch is checked to
 have run fdx_tc_kernel, and its result against fp32 torch."""
-import ctypes
 
 import pytest
 import torch
@@ -27,7 +26,6 @@ def rel(a, b):
 
 def last_kernel():
     lib = _lib.load()
-    lib.fdx_kernel_kind_name.restype = ctypes.c_char_p
     return lib.fdx_kernel_kind_name(lib.fdx_last_kernel_kind()).decode()
 
 

@@ -2,7 +2,6 @@
 channel slot of a wider buffer, the fused GroupNorm backward at 320 and 192 columns, in-place accumulation where
 the last tile has no second pixel half (H % 32 == 16 at 64 columns), and 1x1 convolutions through the engine.
 Each launch is checked to have run fdx_tct_kernel, and its result against fp32 torch."""
-import ctypes
 
 import pytest
 import torch
@@ -21,7 +20,6 @@ def rel(a, b):
 
 def last_kernel():
     lib = _lib.load()
-    lib.fdx_kernel_kind_name.restype = ctypes.c_char_p
     return lib.fdx_kernel_kind_name(lib.fdx_last_kernel_kind()).decode()
 
 

@@ -2,7 +2,6 @@
 CTA's tile sequence, so the edge cases are one tile in all, an odd number of tiles per CTA, fewer tiles than SMs,
 and layers of 128 or 384 columns that run as several 64-column blocks.  Each launch is checked to have run
 fdx_tct_kernel, and its result against fp32 torch."""
-import ctypes
 
 import pytest
 import torch
@@ -21,7 +20,6 @@ def rel(a, b):
 
 def last_kernel():
     lib = _lib.load()
-    lib.fdx_kernel_kind_name.restype = ctypes.c_char_p
     return lib.fdx_kernel_kind_name(lib.fdx_last_kernel_kind()).decode()
 
 

@@ -8,7 +8,6 @@ accumulate source), the channels beside the slot are random sentinels that must 
 launch must have run fdx_tct_kernel.  A bf16 output may differ from the float64 value by its rounding (2^-8
 relative) plus the f32 accumulation error, bounded by 2^-12 of the same sum over absolute values; the fused
 GroupNorm backward adds the error of its tanh.approx sigmoid."""
-import ctypes
 
 import pytest
 import torch
@@ -23,7 +22,6 @@ f64 = torch.float64
 
 def last_kernel():
     lib = _lib.load()
-    lib.fdx_kernel_kind_name.restype = ctypes.c_char_p
     return lib.fdx_kernel_kind_name(lib.fdx_last_kernel_kind()).decode()
 
 

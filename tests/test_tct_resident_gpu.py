@@ -5,7 +5,6 @@ cases are one tile, fewer tiles than SMs, an odd tile count on one CTA, a pixel-
 last group short, and column-block counts that do not divide the SM count (320 and 448 columns on a 132-SM
 part).  Outputs start as NaN, so a tile that is never written fails; every
 launch is checked to have run fdx_tct_kernel, and its result against fp32 torch."""
-import ctypes
 
 import pytest
 import torch
@@ -24,7 +23,6 @@ def rel(a, b):
 
 def last_kernel():
     lib = _lib.load()
-    lib.fdx_kernel_kind_name.restype = ctypes.c_char_p
     return lib.fdx_kernel_kind_name(lib.fdx_last_kernel_kind()).decode()
 
 

@@ -8,7 +8,6 @@ the same view), 64 to 448 columns, and tile counts
 from one tile to several per CTA, so that each warpgroup's buffer ring wraps across tiles.  Outputs inside the slot
 start as NaN (except where they are the accumulate source), every launch must have run fdx_tct_kernel, and
 results are checked against fp32 torch at the tolerances of test_tct_resident_gpu.py."""
-import ctypes
 
 import pytest
 import torch
@@ -27,7 +26,6 @@ def rel(a, b):
 
 def last_kernel():
     lib = _lib.load()
-    lib.fdx_kernel_kind_name.restype = ctypes.c_char_p
     return lib.fdx_kernel_kind_name(lib.fdx_last_kernel_kind()).decode()
 
 
