@@ -52,13 +52,13 @@ class SimpleMMDiT(SimpleDiT):
                  num_heads: int = 12, mlp_ratio: int = 4, dropout_rate: float = 0.0, dtype=None, precision=None,
                  use_flash_attention: bool = False, force_fp32_for_softmax: bool = True, norm_epsilon: float = 1e-5,
                  learn_sigma: bool = False, use_hilbert: bool = False, norm_groups: int = 0, activation=None,
-                 context_dim: Optional[int] = None):
+                 context_dim: Optional[int] = None, use_remat: bool = False):
         super().__init__(output_channels=output_channels, patch_size=patch_size, emb_features=emb_features,
                          num_layers=num_layers, num_heads=num_heads, mlp_ratio=mlp_ratio, dropout_rate=dropout_rate,
                          dtype=dtype, precision=precision, use_flash_attention=use_flash_attention,
                          force_fp32_for_softmax=force_fp32_for_softmax, norm_epsilon=norm_epsilon,
                          learn_sigma=learn_sigma, norm_groups=norm_groups, activation=activation,
-                         context_dim=context_dim)
+                         context_dim=context_dim, use_remat=use_remat)
         self.use_hilbert = use_hilbert
 
     # ------------------------------------------------------------------ structure
@@ -67,7 +67,7 @@ class SimpleMMDiT(SimpleDiT):
         keys = ("output_channels", "patch_size", "emb_features", "num_layers", "num_heads", "mlp_ratio",
                 "dropout_rate", "dtype", "precision", "use_flash_attention", "force_fp32_for_softmax", "norm_epsilon",
                 "learn_sigma", "use_hilbert", "norm_groups", "activation", "context_dim")
-        return {k: getattr(self, k) for k in keys}
+        return self._config(keys)
 
     def param_specs(self):
         if not self.context_dim:
@@ -254,7 +254,8 @@ class HierarchicalMMDiT(SimpleMMDiT):
                  num_layers=(4, 4, 14), num_heads=(8, 12, 16), mlp_ratio: int = 4, dropout_rate: float = 0.0,
                  dtype=None, precision=None, use_flash_attention: bool = False, force_fp32_for_softmax: bool = True,
                  norm_epsilon: float = 1e-5, learn_sigma: bool = False, use_hilbert: bool = False,
-                 norm_groups: int = 0, activation=None, context_dim: Optional[int] = None):
+                 norm_groups: int = 0, activation=None, context_dim: Optional[int] = None,
+                 use_remat: bool = False):
         name = type(self).__name__
         Fs, Ls, Hs = tuple(emb_features), tuple(num_layers), tuple(num_heads)
         if not Fs or not len(Fs) == len(Ls) == len(Hs):
@@ -292,6 +293,7 @@ class HierarchicalMMDiT(SimpleMMDiT):
         self.norm_groups = norm_groups
         self.activation = activation
         self.context_dim = context_dim
+        self.use_remat = use_remat
         self._layouts = {}
         self._consts = {}
         self._stage = {n: s for s in range(len(Fs)) for n in self._stage_blocks("encoder", s) +
@@ -303,7 +305,7 @@ class HierarchicalMMDiT(SimpleMMDiT):
         keys = ("output_channels", "base_patch_size", "emb_features", "num_layers", "num_heads", "mlp_ratio",
                 "dropout_rate", "dtype", "precision", "use_flash_attention", "force_fp32_for_softmax", "norm_epsilon",
                 "learn_sigma", "use_hilbert", "norm_groups", "activation", "context_dim")
-        return {k: getattr(self, k) for k in keys}
+        return self._config(keys)
 
     def _stage_blocks(self, kind: str, s: int):
         return [f"{kind}_block_stage{s}_{i}" for i in range(self.num_layers[s])]
@@ -404,10 +406,13 @@ class HierarchicalMMDiT(SimpleMMDiT):
         tok, rows = self._embed_fwd(x, W32, W16, HP, WP, order, save)
         # without save only the skips that the decoders' concat LayerNorms read are kept, each until it is read
         recs, skips, merges = {}, [], []
+
+        def block(n, x, s, L):
+            return self._remat_fwd(lambda x, sv: self._mm_block_fwd(n, x, conds[s], W32, W16, B, L, sv), x, save)
         for s in range(N):                                                   # encoder, fine to coarse
             L = grids[s][0] * grids[s][1]
             for n in self._stage_blocks("encoder", s):
-                tok, recs[n] = self._mm_block_fwd(n, tok, conds[s], W32, W16, B, L, save)
+                tok, recs[n] = block(n, tok, s, L)
             if save or s < N - 1:
                 skips.append(tok)
             if s < N - 1:
@@ -437,7 +442,7 @@ class HierarchicalMMDiT(SimpleMMDiT):
             tok = ops.linear_fwd(c, W16[f"fusion_dense_{s}/kernel"], bias=W32[f"fusion_dense_{s}/bias"])
             del c
             for n in self._stage_blocks("decoder", s):
-                tok, recs[n] = self._mm_block_fwd(n, tok, conds[s], W32, W16, B, L, save)
+                tok, recs[n] = block(n, tok, s, L)
         out, final = self._final_fwd(tok, W32, W16, B, H, W, grids[0][0] * grids[0][1], order, save)
         if not save:
             return out, None
@@ -456,11 +461,15 @@ class HierarchicalMMDiT(SimpleMMDiT):
         dconds = [torch.zeros((B, 2 * F), dtype=F32, device=dev) for F in Fs]
         dx = self._final_bwd(saved["final"], dF, saved["order"], W32, Gd, grids[0][0] * grids[0][1])
         dskips = [None] * N
+
+        def block_bwd(n, dx, s, L):
+            rec = self._remat_record(lambda x, sv: self._mm_block_fwd(n, x, conds[s], W32, W16, B, L, sv), recs[n])
+            return self._mm_block_bwd(rec, dx, conds[s], dconds[s], W32, W16, Gd, B, L)
         for s, tin, u, em, er, e, c, cm, cr in reversed(saved["dec"]):      # decoder, fine to coarse
             hc, wc = grids[s + 1]
             L = grids[s][0] * grids[s][1]
             for n in reversed(self._stage_blocks("decoder", s)):
-                dx = self._mm_block_bwd(recs[n], dx, conds[s], dconds[s], W32, W16, Gd, B, L)
+                dx = block_bwd(n, dx, s, L)
             _dense_wgrad(Gd[f"fusion_dense_{s}/kernel"], c, dx)
             ops.colsum_rows(dx, Gd[f"fusion_dense_{s}/bias"])
             dc = _dense_dgrad(dx, W16[f"fusion_dense_{s}/kernel"])
@@ -488,7 +497,7 @@ class HierarchicalMMDiT(SimpleMMDiT):
                                                W32[m + "norm/scale"], mm, mr, Gd[m + "norm/scale"],
                                                Gd[m + "norm/bias"], grid=(hc, wc), dx0=dskips[s], accumulate0=True)
             for n in reversed(self._stage_blocks("encoder", s)):
-                dx = self._mm_block_bwd(recs[n], dx, conds[s], dconds[s], W32, W16, Gd, B, L)
+                dx = block_bwd(n, dx, s, L)
         self._embed_bwd(saved["rows"], dx, Gd)
 
         # conditioning: the stage projections, then the base embeddings

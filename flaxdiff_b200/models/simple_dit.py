@@ -11,6 +11,10 @@ over the concatenated, head-padded kernels), attention on the fused kernels; the
 fdx_dit.cu's: adaLN LayerNorm, the gated residual, RoPE in place on the QKV output, bias + tanh-gelu, patchify /
 unpatchify.  The backward is an explicit tape; every per-sample column sum is deterministic.  Raster patch order
 only: the Hilbert / zigzag scans are refused at construction.
+
+use_remat=True (the reference UViT's flag, taken by every transformer model here) trades compute for memory: the
+training forward keeps only each trunk block's input, and the backward re-runs the block's forward from it right
+before the block's backward (_remat_fwd / _remat_record).  The recomputed record is the taped one bit for bit.
 """
 from __future__ import annotations
 
@@ -62,7 +66,7 @@ class SimpleDiT:
                  num_heads: int = 12, mlp_ratio: int = 4, dropout_rate: float = 0.0, dtype=None, precision=None,
                  use_flash_attention: bool = False, force_fp32_for_softmax: bool = True, norm_epsilon: float = 1e-5,
                  learn_sigma: bool = False, use_hilbert: bool = False, use_zigzag: bool = False, norm_groups: int = 0,
-                 activation=None, context_dim: Optional[int] = None):
+                 activation=None, context_dim: Optional[int] = None, use_remat: bool = False):
         self.output_channels = output_channels
         self.patch_size = patch_size
         self.emb_features = emb_features
@@ -82,6 +86,7 @@ class SimpleDiT:
         self.activation = activation
         # width of `textcontext`: text_context_proj exists only when init saw a context (as Unet.context_dim)
         self.context_dim = context_dim
+        self.use_remat = use_remat
         if use_hilbert or use_zigzag:
             raise FdxError("SimpleDiT: the Hilbert / zigzag patch orders are not supported (raster order only)")
         if use_flash_attention:
@@ -177,7 +182,15 @@ class SimpleDiT:
         keys = ("output_channels", "patch_size", "emb_features", "num_layers", "num_heads", "mlp_ratio",
                 "dropout_rate", "dtype", "precision", "use_flash_attention", "force_fp32_for_softmax", "norm_epsilon",
                 "learn_sigma", "use_hilbert", "use_zigzag", "norm_groups", "activation", "context_dim")
-        return {k: getattr(self, k) for k in keys}
+        return self._config(keys)
+
+    def _config(self, keys) -> dict:
+        """The constructor arguments named by `keys`, plus use_remat when it is set: a config written without the
+        flag compares, serialises and parses as before, and one that carries it rebuilds a model with it set."""
+        cfg = {k: getattr(self, k) for k in keys}
+        if self.use_remat:
+            cfg["use_remat"] = True
+        return cfg
 
     # ------------------------------------------------------------------ init
     def init(self, key, x=None, temb=None, textcontext=None, device=None) -> FlatParams:
@@ -283,10 +296,26 @@ class SimpleDiT:
         """The blocks between the patch embedding and final_norm -> (tokens, tape; None unless save)."""
         blocks = []
         for n, fwd, _ in self._blocks():
-            tok, rec = fwd(n, tok, cond16, W32, W16, B, L, save=save)
+            tok, rec = self._remat_fwd(lambda x, s: fwd(n, x, cond16, W32, W16, B, L, save=s), tok, save)
             if save:
                 blocks.append(rec)
         return tok, (blocks if save else None)
+
+    def _remat_fwd(self, fwd, x, save: bool):
+        """One trunk block of the forward, fwd(input, save) -> (output, tape entry; None unless save).  Under
+        use_remat the training forward runs the block with save=False and its tape entry is the block's input itself:
+        a reference, so an input that is live anyway (a skip of the U models) is not stored twice."""
+        if save and self.use_remat:
+            return fwd(x, False)[0], x
+        return fwd(x, save)
+
+    def _remat_record(self, fwd, entry):
+        """The record a block's backward reads: its tape entry, or under use_remat the record of the block's forward
+        re-run with save=True from the taped input.  That is the training forward's launches on the same input, so
+        the record is the taped one bit for bit.  Everything runs on the current stream, so once the caller drops
+        the record after enqueueing the block's backward, the caching allocator hands its blocks only to work queued
+        after their last reader, in eager runs and inside a graph capture alike."""
+        return fwd(entry, True)[1] if self.use_remat else entry
 
     def _embed_fwd(self, x, W32, W16, HP: int, WP: int, order, save: bool = True):
         """Patch rows (in the patch order) x the patch embedding [+ the position table] -> (tokens bf16, patch rows;
@@ -547,8 +576,10 @@ class SimpleDiT:
 
     def _trunk_bwd(self, tape, dx, cond16, dcond, W32, W16, Gd, B: int, L: int, ready):
         """Backward of _trunk_fwd -> d(its input tokens); ready(leaf) announces every gradient from `leaf` on final."""
-        for (n, _, bwd), rec in zip(reversed(self._blocks()), reversed(tape)):
+        for (n, fwd, bwd), entry in zip(reversed(self._blocks()), reversed(tape)):
+            rec = self._remat_record(lambda x, s: fwd(n, x, cond16, W32, W16, B, L, save=s), entry)
             dx = bwd(rec, dx, cond16, dcond, W32, W16, Gd, B, L)
+            del rec
             ready(self._ada_leaf(n))
         return dx
 

@@ -97,7 +97,8 @@ class HybridSSMAttentionDiT(SimpleDiT):
                  norm_epsilon: float = 1e-5, learn_sigma: bool = False, use_hilbert: bool = False,
                  use_zigzag: bool = False, norm_groups: int = 0, activation=None,
                  block_pattern: Optional[Sequence[str]] = None, ssm_attention_ratio: str = "3:1",
-                 bidirectional_ssm: bool = True, use_2d_fusion: bool = False, context_dim: Optional[int] = None):
+                 bidirectional_ssm: bool = True, use_2d_fusion: bool = False, context_dim: Optional[int] = None,
+                 use_remat: bool = False):
         if use_hilbert and use_zigzag:
             raise FdxError("HybridSSMAttentionDiT: use_hilbert and use_zigzag are mutually exclusive")
         if use_2d_fusion:
@@ -111,7 +112,7 @@ class HybridSSMAttentionDiT(SimpleDiT):
                          dtype=dtype, precision=precision, use_flash_attention=use_flash_attention,
                          force_fp32_for_softmax=force_fp32_for_softmax, norm_epsilon=norm_epsilon,
                          learn_sigma=learn_sigma, norm_groups=norm_groups, activation=activation,
-                         context_dim=context_dim)
+                         context_dim=context_dim, use_remat=use_remat)
         self.use_hilbert = use_hilbert
         self.use_zigzag = use_zigzag
         self.ssm_state_dim = N

@@ -50,7 +50,7 @@ class SimpleUDiT(SimpleDiT):
                  num_heads: int = 12, mlp_ratio: int = 4, dropout_rate: float = 0.0, dtype=None, precision=None,
                  use_flash_attention: bool = False, force_fp32_for_softmax: bool = True, norm_epsilon: float = 1e-5,
                  learn_sigma: bool = False, use_hilbert: bool = False, norm_groups: int = 0, activation=None,
-                 context_dim: Optional[int] = None):
+                 context_dim: Optional[int] = None, use_remat: bool = False):
         if num_layers % 2:
             raise FdxError(f"{type(self).__name__}: num_layers={num_layers} must be even (a U of num_layers / 2 down "
                            "and up blocks around a middle block)")
@@ -59,7 +59,7 @@ class SimpleUDiT(SimpleDiT):
                          dtype=dtype, precision=precision, use_flash_attention=use_flash_attention,
                          force_fp32_for_softmax=force_fp32_for_softmax, norm_epsilon=norm_epsilon,
                          learn_sigma=learn_sigma, norm_groups=norm_groups, activation=activation,
-                         context_dim=context_dim)
+                         context_dim=context_dim, use_remat=use_remat)
         self.use_hilbert = use_hilbert
 
     # ------------------------------------------------------------------ structure
@@ -68,7 +68,7 @@ class SimpleUDiT(SimpleDiT):
         keys = ("output_channels", "patch_size", "emb_features", "num_layers", "num_heads", "mlp_ratio",
                 "dropout_rate", "dtype", "precision", "use_flash_attention", "force_fp32_for_softmax", "norm_epsilon",
                 "learn_sigma", "use_hilbert", "norm_groups", "activation", "context_dim")
-        return {k: getattr(self, k) for k in keys}
+        return self._config(keys)
 
     def _blocks(self):
         """The DiT blocks in forward order; up_dense_{i} precedes up_block_{i} in the layout (_block_specs)."""
@@ -117,10 +117,13 @@ class SimpleUDiT(SimpleDiT):
         Without save only the skip stack is kept, and each skip is released once its up_dense is enqueued."""
         h = self.num_layers // 2
         recs, skips, ups = {}, [], []
+
+        def block(n, x):
+            return self._remat_fwd(lambda x, s: self._block_fwd(n, x, cond16, W32, W16, B, L, s), x, save)
         for i in range(h):
-            tok, recs[f"down_block_{i}"] = self._block_fwd(f"down_block_{i}", tok, cond16, W32, W16, B, L, save)
+            tok, recs[f"down_block_{i}"] = block(f"down_block_{i}", tok)
             skips.append(tok)
-        tok, recs["mid_block"] = self._block_fwd("mid_block", tok, cond16, W32, W16, B, L, save)
+        tok, recs["mid_block"] = block("mid_block", tok)
         for i in range(h):
             u = f"up_dense_{i}"
             if save:
@@ -128,7 +131,7 @@ class SimpleUDiT(SimpleDiT):
             skip = skips[h - 1 - i] if save else skips.pop()
             tok = ops.linear_cat_fwd(tok, skip, W16[u + "/kernel"], bias=W32[u + "/bias"])
             del skip
-            tok, recs[f"up_block_{i}"] = self._block_fwd(f"up_block_{i}", tok, cond16, W32, W16, B, L, save)
+            tok, recs[f"up_block_{i}"] = block(f"up_block_{i}", tok)
         return tok, ((recs, skips, ups) if save else None)
 
     def _final_fwd(self, tok, W32, W16, B, H, W, L, order, save: bool = True):
@@ -161,9 +164,13 @@ class SimpleUDiT(SimpleDiT):
         recs, skips, ups = tape
         h, F = self.num_layers // 2, self.emb_features
         dys = [None] * h                    # dys[j]: the output gradient of the up_dense whose skip is down_block_j
+
+        def block_bwd(n, dx):
+            rec = self._remat_record(lambda x, s: self._block_fwd(n, x, cond16, W32, W16, B, L, s), recs[n])
+            return self._block_bwd(rec, dx, cond16, dcond, W32, W16, Gd, B, L)
         for i in reversed(range(h)):
             n, u = f"up_block_{i}", f"up_dense_{i}"
-            dx = self._block_bwd(recs[n], dx, cond16, dcond, W32, W16, Gd, B, L)
+            dx = block_bwd(n, dx)
             ready(self._ada_leaf(n))
             j = h - 1 - i
             g = Gd[u + "/kernel"]
@@ -173,12 +180,12 @@ class SimpleUDiT(SimpleDiT):
             dys[j] = dx
             dx = _dense_dgrad(dx, W16[u + "/kernel"][:F])
             ready(u + "/kernel")
-        dx = self._block_bwd(recs["mid_block"], dx, cond16, dcond, W32, W16, Gd, B, L)
+        dx = block_bwd("mid_block", dx)
         ready(self._ada_leaf("mid_block"))
         for j in reversed(range(h)):
             n = f"down_block_{j}"
             dx = _dense_dgrad(dys[j], W16[f"up_dense_{h - 1 - j}/kernel"][F:], res=dx)
             dys[j] = None
-            dx = self._block_bwd(recs[n], dx, cond16, dcond, W32, W16, Gd, B, L)
+            dx = block_bwd(n, dx)
             ready(self._ada_leaf(n))
         return dx

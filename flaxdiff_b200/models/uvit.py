@@ -28,11 +28,13 @@ What differs from SimpleUDiT, and how it runs:
     bf16(W - bf16(W)) through fdx_gemm_cat, then fdx_col2im3x3_c3).
   * The residual stream is stored in bf16, as in every model here; the reference carries it in f32 from the position
     add on.  Each add runs in f32 inside a GEMM epilogue or a streaming kernel and is rounded once (DESIGN.md, UViT).
+  * use_remat=True recomputes each block in the backward, as every transformer model here does with the flag
+    (SimpleDiT._remat_fwd): the training tape keeps a block's input instead of its record.
 
 Refused with FdxError: use_flash_attention=True, a dtype other than bf16, odd num_layers, emb_features not a multiple
 of num_heads or of 64 or above 1024, head widths above 256, images not divisible by the patch size or with more
 patches than pos_encoding has rows, inputs with other than 3 channels, 2-D text, and the head with output_channels != 3.
-dropout_rate, norm_groups, force_fp32_for_softmax, use_remat and precision are accepted and ignored.
+dropout_rate, norm_groups, force_fp32_for_softmax and precision are accepted and ignored.
 """
 from __future__ import annotations
 
@@ -80,8 +82,8 @@ class UViT(SimpleDiT):
         self.emb_features = emb_features
         self.num_layers = num_layers
         self.num_heads = num_heads
-        self.dropout_rate = dropout_rate        # accepted and ignored, with norm_groups, force_fp32_for_softmax,
-        self.norm_groups = norm_groups          # use_remat and precision, as SimpleUDiT does with its equivalents
+        self.dropout_rate = dropout_rate        # accepted and ignored, with norm_groups, force_fp32_for_softmax
+        self.norm_groups = norm_groups          # and precision, as SimpleUDiT does with its equivalents
         self.force_fp32_for_softmax = force_fp32_for_softmax
         self.use_remat = use_remat
         self.precision = precision
@@ -303,10 +305,13 @@ class UViT(SimpleDiT):
         Without save only the skip stack is kept, and each skip is released once its up_dense is enqueued."""
         h = self.num_layers // 2
         recs, skips, ups = {}, [], []
+
+        def block(n, x):
+            return self._remat_fwd(lambda x, s: self._block_fwd(n, x, W32, W16, B, L, s), x, save)
         for i in range(h):
-            tok, recs[f"down_block_{i}"] = self._block_fwd(f"down_block_{i}", tok, W32, W16, B, L, save)
+            tok, recs[f"down_block_{i}"] = block(f"down_block_{i}", tok)
             skips.append(tok)
-        tok, recs["mid_block"] = self._block_fwd("mid_block", tok, W32, W16, B, L, save)
+        tok, recs["mid_block"] = block("mid_block", tok)
         for i in range(h):
             u = f"up_dense_{i}"
             if save:
@@ -314,7 +319,7 @@ class UViT(SimpleDiT):
             skip = skips[h - 1 - i] if save else skips.pop()
             tok = ops.linear_cat_fwd(tok, skip, W16[u + "/kernel"], bias=W32[u + "/bias"])
             del skip
-            tok, recs[f"up_block_{i}"] = self._block_fwd(f"up_block_{i}", tok, W32, W16, B, L, save)
+            tok, recs[f"up_block_{i}"] = block(f"up_block_{i}", tok)
         return tok, ((recs, skips, ups) if save else None)
 
     def _final_fwd(self, tok, W32, W16, B, H, W, N, L, order, save: bool = True):
@@ -464,9 +469,13 @@ class UViT(SimpleDiT):
         recs, skips, ups = tape
         h, F = self.num_layers // 2, self.emb_features
         dys = [None] * h
+
+        def block_bwd(n, dx):
+            rec = self._remat_record(lambda x, s: self._block_fwd(n, x, W32, W16, B, L, s), recs[n])
+            return self._block_bwd(rec, dx, W32, W16, Gd, B, L)
         for i in reversed(range(h)):
             n, u = f"up_block_{i}", f"up_dense_{i}"
-            dx = self._block_bwd(recs[n], dx, W32, W16, Gd, B, L)
+            dx = block_bwd(n, dx)
             j = h - 1 - i
             g = Gd[u + "/kernel"]
             _dense_wgrad(g[:F], ups[i], dx)
@@ -475,12 +484,12 @@ class UViT(SimpleDiT):
             dys[j] = dx
             dx = _dense_dgrad(dx, W16[u + "/kernel"][:F])
             ready(u + "/kernel")
-        dx = self._block_bwd(recs["mid_block"], dx, W32, W16, Gd, B, L)
+        dx = block_bwd("mid_block", dx)
         ready(self._ada_leaf("mid_block"))
         for j in reversed(range(h)):
             n = f"down_block_{j}"
             dx = _dense_dgrad(dys[j], W16[f"up_dense_{h - 1 - j}/kernel"][F:], res=dx)
             dys[j] = None
-            dx = self._block_bwd(recs[n], dx, W32, W16, Gd, B, L)
+            dx = block_bwd(n, dx)
             ready(self._ada_leaf(n))
         return dx
